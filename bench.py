@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- genes/s of the full deseq2() hot path (dispersion + IRLS + Wald) on B200, next to the CPU path.
+"""bench.py -- genes/s of the full deseq2() hot path (dispersion + IRLS + Wald) on H100, next to the CPU path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--cpu-steps C] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -21,6 +21,14 @@ Prints ONE JSON line (rank 0).  `value` = device-resident throughput (counts alr
 CUDA events on the library's stream, L2 flushed between steps, max over ranks.  `e2e` = the same metric through the
 reference-facing plugin calls with HOST buffers (H2D/D2H inside the timed region; page-locked and pageable variants).
 `roofline` describes the dominant kernel, `cpu_baseline` the oracle port (joblib over genes, like the reference).
+
+Every timed loop on the GPU, and the CPU arm `--impl reference`, runs exactly K steps after W warm-up steps; the device-resident
+loops warm up with at least 3 passes, because the first pass runs eagerly and the second captures the pass as a CUDA graph that
+the timed steps replay.  The CPU baseline reported next to a GPU run is a separate measurement of seconds per pass, so its pass
+count is its own option, `--cpu-steps` (default 3).  `--dump-outputs DIR` writes the per-gene results of the last timed step of
+the headline workload (rank 0's shard) as DIR/<name>.npy in float64, at most 64 MiB in all: above that, the same fixed, seeded
+sample of genes from every per-gene array, with the sampled indices in DIR/gene_index.npy.  The inputs are seeded, so two builds
+given the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -50,18 +58,27 @@ KERNEL_OF = {"alpha_mle_genewise": "k_alpha_mle", "alpha_mle_map": "k_alpha_mle"
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=5, help="timed steps of every GPU measurement (>= 1)")
+    ap.add_argument("--warmup", type=int, default=3, help="warm-up steps before timing (device-resident loops: at least 3)")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--genes", type=int, default=20000)
     ap.add_argument("--samples", type=int, default=200)
     ap.add_argument("--design", default="two_level", choices=["two_level", "factorial", "continuous"])
     ap.add_argument("--cpu-sample-genes", type=int, default=20000,
-                    help="genes of the workload the CPU baseline is timed on (20 000 x 200 is ~6 s per pass on the GPU box)")
+                    help="genes of the workload the CPU baseline is timed on")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--cpu-steps", type=int, default=3, help="timed passes of the CPU baseline that accompanies a GPU run (>= 1)")
     ap.add_argument("--no-extra-configs", action="store_true", help="skip the `configs` block (C3 / C5 shard / C4 shard)")
     ap.add_argument("--lanes", type=int, default=0, help="lanes per gene override (0 = auto)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the results of the last timed step as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1 or args.cpu_steps < 1:
+        ap.error("--steps and --cpu-steps must be at least 1")
+    if args.warmup < 0:
+        ap.error("--warmup must not be negative")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs records the GPU path's results; it does not apply to --impl reference")
+    return args
 
 
 def make_workload(samples, genes, design, rank, dist=None):
@@ -84,9 +101,9 @@ def make_workload(samples, genes, design, rank, dist=None):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region, and the board's power limit."""
 
-    Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
+    Q = ("clocks.sm,clocks.max.sm,power.draw,power.limit,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
     def __init__(self, index):
@@ -117,22 +134,35 @@ class ClockSampler:
     def summary(self):
         sm = [float(r[0]) for r in self.rows if r and r[0].replace(".", "").isdigit()]
         mx = [float(r[1]) for r in self.rows if len(r) > 1 and r[1].replace(".", "").isdigit()]
+        lim = [float(r[3]) for r in self.rows if len(r) > 3 and r[3].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
-        reasons = sorted({n for r in self.rows if len(r) >= 7 for n, v in zip(names, r[3:7]) if v.lower().startswith("active")})
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
-                "samples": len(sm)}
+        reasons = sorted({n for r in self.rows if len(r) >= 8 for n, v in zip(names, r[4:8]) if v.lower().startswith("active")})
+        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
+                "power_limit_w": max(lim) if lim else None, "reasons": reasons, "samples": len(sm)}
 
 
-def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, STREAM-style copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+DUMP_CAP = 64 << 20
 
 
-def profile_record():
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    return json.load(open(path)) if os.path.exists(path) else {}
+def dump_outputs(path, res, cap=DUMP_CAP):
+    """The per-gene arrays a caller of ResidentFit.run receives (and the trend / prior scalars), one float64 .npy each, at most
+    `cap` bytes in all: above that, the rows of one fixed, seeded sample of genes (sorted) from every per-gene array, and the
+    sampled gene indices as gene_index.npy."""
+    os.makedirs(path, exist_ok=True)
+    per_gene = {k: np.asarray(v, dtype=np.float64) for k, v in res.items() if isinstance(v, np.ndarray)}
+    scalars = {"trend_coeffs": np.asarray(res["trend"].coeffs, dtype=np.float64),
+               "prior_var": np.float64(res["prior_var"]), "squared_logres": np.float64(res["squared_logres"])}
+    G = len(res["dispersions"])
+    assert all(v.shape[0] == G for v in per_gene.values())
+    fixed = sum(v.nbytes for v in scalars.values()) + 4096  # scalars + .npy headers
+    row = sum(v.nbytes // max(G, 1) for v in per_gene.values()) + 8  # + its entry of gene_index
+    if fixed + G * (row - 8) + 128 * (len(per_gene) + len(scalars)) > cap:
+        k = max(1, (cap - fixed - 128 * (len(per_gene) + len(scalars) + 1)) // row)
+        idx = np.sort(np.random.default_rng(0).choice(G, size=k, replace=False))
+        per_gene = {n: v[idx] for n, v in per_gene.items()}
+        np.save(os.path.join(path, "gene_index.npy"), idx.astype(np.float64))
+    for k, v in {**per_gene, **scalars}.items():
+        np.save(os.path.join(path, k + ".npy"), v)
 
 
 def cpu_fit(counts, X, sf, n_cpus):
@@ -146,9 +176,9 @@ def cpu_fit(counts, X, sf, n_cpus):
     return time.perf_counter() - t0
 
 
-def cpu_sample_desc(n, args, passes):
+def cpu_sample_desc(n, args, passes, warm):
     return (f"{'all' if n >= args.genes else 'first'} {n} of {args.genes} genes x {args.samples} samples "
-            f"(non-all-zero genes of them), median of {passes} timed passes after a warm-up pass")
+            f"(non-all-zero genes of them), median of {passes} timed passes after {warm} warm-up pass(es)")
 
 
 def run_reference(args, rank, world):
@@ -160,18 +190,18 @@ def run_reference(args, rank, world):
     sample = counts if n_in >= G_in else np.ascontiguousarray(counts[:, :n_in])
     cores = os.cpu_count() or 1
     cpu_fit(sample[:, :256], X, sf, cores)  # spawn the loky pool outside the timed region
-    for _ in range(max(1, min(args.warmup, 2))):
+    for _ in range(args.warmup):
         cpu_fit(sample, X, sf, cores)
-    steps = max(1, min(args.steps, 5))  # bounded: the arm must end within minutes (one pass is ~6 s on 128 cores)
+    steps = args.steps
     times = [cpu_fit(sample, X, sf, cores) for _ in range(steps)]
     dt = float(np.median(times))
     val = n_in / dt
     line = {"impl": "reference", "metric": METRIC, "value": val, "unit": UNIT, "n_gpus": args.gpus, "steps": steps,
-            "warmup": max(1, min(args.warmup, 2)), "ms_per_step": dt * 1e3, "higher_is_better": True, "scaling": "weak",
+            "warmup": args.warmup, "ms_per_step": dt * 1e3, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": config(args, note=f"reference CPU path: oracle port of DefaultInference (numpy/scipy per gene, joblib/loky, "
-                                        f"{cores} processes); each step = {cpu_sample_desc(n_in, args, steps)}"),
-            "cpu_baseline": {"value": val, "unit": UNIT, "cores": cores, "kind": "port", "sample": cpu_sample_desc(n_in, args, steps),
+                                        f"{cores} processes); each step = {cpu_sample_desc(n_in, args, steps, args.warmup)}"),
+            "cpu_baseline": {"value": val, "unit": UNIT, "cores": cores, "kind": "port", "sample": cpu_sample_desc(n_in, args, steps, args.warmup),
                              "pass_s": [round(t, 3) for t in times]},
             "e2e": {"value": val, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line), flush=True)
@@ -227,8 +257,28 @@ class Bench:
             self.uid = uid.cpu().numpy().tobytes()
         self.comm = None
         self.flush = self.ctx.malloc(256 << 20)
-        self.peak, self.peak_src = peaks()
+        self.peak, self.peak_src = self.hbm_peak()
         self.fp64_peak = None
+
+    def hbm_peak(self):
+        """HBM bandwidth of this device, measured: device-to-device copies of a 256 MiB buffer (5x the 50 MB L2 of an H100), read +
+        write bytes over CUDA-event time, best of 5 batches of 10 copies."""
+        n, copies = 256 << 20, 10
+        dst = self.ctx.malloc(n)
+        L, h, c_d = self.ctx.lib, self.ctx.h, self._lib.c_dptr
+        try:
+            best = 0.0
+            for rep in range(6):  # the first batch only warms up
+                self.ctx.record(0)
+                for _ in range(copies):
+                    self.ctx.check(L.pdq_memcpy_d2d(h, c_d(dst), c_d(self.flush), n))
+                self.ctx.record(1)
+                self.ctx.sync()
+                if rep:
+                    best = max(best, 2.0 * n * copies / (self.ctx.elapsed_ms(0, 1) * 1e-3) / 1e9)
+        finally:
+            self.ctx.free(dst)
+        return best, "measured in this run: device-to-device copy of 256 MiB, read + write bytes, best of 5 x 10 copies"
 
     # -- plumbing ---------------------------------------------------------------------------------------------
     def barrier(self):
@@ -293,7 +343,7 @@ class Bench:
         for _ in range(steps):
             self.flush_l2()
             self.barrier()
-            rf.run(events=(0, 1))  # CUDA events around the device work of the pass: first launch ... result copy done
+            self.last = rf.run(events=(0, 1))  # CUDA events around the device work of the pass: first launch ... result copy done
             step_ms.append(self.ctx.elapsed_ms(0, 1))
         self.barrier()
         launches = self.ctx.launches() - launches0
@@ -309,8 +359,8 @@ class Bench:
         return rf, rec
 
     def rooflines(self, stages, N, G, p, step_ms):
-        """HBM roofline of the dominant kernel and of the whole step; FP64 roofline of the dominant kernel (DFMA peak measured in
-        this run; flop count per (gene, sample) from the committed ncu capture of the same kernel, profiles/traffic.json)."""
+        """HBM roofline of the dominant kernel and of the whole step, from the bytes the algorithm needs; the device's DFMA peak,
+        measured in this run, for comparison (the kernels' FP64 operation counts are data dependent and not counted here)."""
         kern = {k: v for k, v in stages.items() if k in ALG_BYTES}
         top = max(kern, key=kern.get)
         achieved = ALG_BYTES[top] * N * G / (kern[top] * 1e-3) / 1e9
@@ -318,30 +368,14 @@ class Bench:
         if "irls_lfc_wald" in kern:
             step_bytes += ALG_BYTES["wald_test"] * N * G  # the fused launch also does the Wald call's work (its mu read is saved)
         kname = KERNEL_OF[top]
-        prof = profile_record()
         roof = {"bound": "hbm", "kernel": f"{kname} ({top})", "achieved": achieved, "peak": self.peak, "unit": "GB/s",
-                "frac": achieved / self.peak, "traffic": prof.get("dram_bytes_per_launch", {}).get(kname),
-                "peak_source": self.peak_src, "algorithmic_bytes_per_launch": ALG_BYTES[top] * N * G, "kernel_ms": kern[top],
+                "frac": achieved / self.peak, "peak_source": self.peak_src, "algorithmic_bytes_per_launch": ALG_BYTES[top] * N * G, "kernel_ms": kern[top],
                 "step": {"algorithmic_bytes": step_bytes, "achieved": step_bytes / (step_ms * 1e-3) / 1e9,
                          "frac": step_bytes / (step_ms * 1e-3) / 1e9 / self.peak},
                 "note": "issue / FP64-pipe bound (log, exp, reciprocal, digamma per gene-sample-iteration), see DESIGN.md §5"}
         if self.fp64_peak is None:
             self.fp64_peak = self.ctx.fp64_peak_tflops()
-        fp64 = {"peak_tflops": self.fp64_peak, "peak_source": "measured in this run (pdq_fp64_peak_tflops: DFMA chains on every SM)"}
-        by_n = prof.get("fp64_flop_per_gene_sample_by_samples", {})
-        if by_n:  # counters exist for the captured sample counts (200, 500): take the nearest
-            key = min(by_n, key=lambda k: abs(int(k) - N))
-            per_pair = by_n[key].get(kname)
-            fp64["flop_counted_at_samples"] = int(key)
-        else:
-            per_pair = prof.get("fp64_flop_per_gene_sample", {}).get(kname)
-        if per_pair:
-            flop = per_pair * N * G
-            fp64.update({"achieved_tflops": flop / (kern[top] * 1e-3) / 1e12, "flop_per_launch": flop,
-                         "frac": flop / (kern[top] * 1e-3) / 1e12 / self.fp64_peak if self.fp64_peak > 0 else None,
-                         "flop_source": prof.get("fp64_flop_source"),
-                         "pipe_active_pct_ncu": prof.get("fp64_pipe_active_pct", {}).get(kname)})
-        roof["fp64"] = fp64
+        roof["fp64"] = {"peak_tflops": self.fp64_peak, "peak_source": "measured in this run (pdq_fp64_peak_tflops: DFMA chains on every SM)"}
         return {"roofline": roof}
 
     def e2e(self, counts, X, sf, G_in, steps, pinned):
@@ -450,6 +484,8 @@ def main():
     # ---------------------------------------------------------------- value: device-resident (headline workload)
     clk = ClockSampler(B.local).__enter__()  # sampled from the warm-up until the end of the e2e loop (steps last only ms)
     rf, head = B.resident(counts, X, sf, G_in, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, B.last)
     stages = dict(head["stages_ms"])
     shard_check = B.check_shards(rf) if world > 1 else None
     exchange_ab = None
@@ -483,12 +519,12 @@ def main():
 
     # ---------------------------------------------------------------- e2e: plugin calls with host buffers
     e2e = B.e2e(counts, X, sf, G_in, args.steps, pinned=True)
-    e2e_pageable = B.e2e(counts, X, sf, G_in, max(2, min(args.steps, 5)), pinned=False)
+    e2e_pageable = B.e2e(counts, X, sf, G_in, args.steps, pinned=False)
     e2e["pageable"] = e2e_pageable
     time.sleep(0.25)  # let nvidia-smi emit at least one more sample
     clk.__exit__()
 
-    full = B.full_deseq2(counts, X, sf, G_in, max(3, min(args.steps, 10))) if world == 1 else None
+    full = B.full_deseq2(counts, X, sf, G_in, args.steps) if world == 1 else None
 
     # ---------------------------------------------------------------- BASELINE's larger shapes, same measurement
     configs = {}
@@ -499,13 +535,13 @@ def main():
             extra.insert(0, ("C3", 60000, 500, "factorial", "BASELINE.json configs[2]: 60 000 genes x 500 samples, 3 covariates, whole on one GPU"))
         for name, g, n, design, what in extra:
             c2, X2, sf2, gin2 = make_workload(n, g, design, rank, B.dist)
-            rf2, rec = B.resident(c2, X2, sf2, gin2, max(3, min(args.steps, 10)), 3)
+            rf2, rec = B.resident(c2, X2, sf2, gin2, args.steps, 3)
             rec["workload"] = f"{what}; {g} genes x {n} samples per GPU, {design} design (p={P_OF[design]})"
             if world > 1:
                 rec["shard_check"] = B.check_shards(rf2)
             rf2.close()
             if name == "C3":
-                rec["e2e"] = B.e2e(c2, X2, sf2, gin2, 3, pinned=True)
+                rec["e2e"] = B.e2e(c2, X2, sf2, gin2, args.steps, pinned=True)
             configs[name] = rec
             del c2, rf2
 
@@ -517,9 +553,9 @@ def main():
         sample = counts if n_in >= G_in else np.ascontiguousarray(counts[:, :n_in])
         cpu_fit(sample[:, :256], X, sf, cores)  # pool start-up outside the timed region
         cpu_fit(sample, X, sf, cores)           # warm-up pass
-        times = [cpu_fit(sample, X, sf, cores) for _ in range(3)]
+        times = [cpu_fit(sample, X, sf, cores) for _ in range(args.cpu_steps)]
         dt = float(np.median(times))
-        cpu = {"value": n_in / dt, "unit": UNIT, "cores": cores, "kind": "port", "sample": cpu_sample_desc(n_in, args, 3),
+        cpu = {"value": n_in / dt, "unit": UNIT, "cores": cores, "kind": "port", "sample": cpu_sample_desc(n_in, args, args.cpu_steps, 1),
                "pass_s": [round(t, 3) for t in times]}
 
     if rank == 0:

@@ -1,5 +1,5 @@
 /*
- * pydeseq2_b200 -- C ABI of the B200 (sm_100a) backend for PyDESeq2's per-gene NB-GLM hot path.
+ * pydeseq2_b200 -- C ABI of the H100 (sm_90a) backend for PyDESeq2's per-gene NB-GLM hot path.
  *
  * Every `pdq_*` compute entry point replaces one method of the reference's plugin interface
  * `pydeseq2.inference.Inference` (reference file:line cited per function).  The reference binds
@@ -37,7 +37,7 @@ typedef enum pdq_status {
     PDQ_ERR_INVALID = -2,     /* bad argument (null pointer, N<=0, p<1, ld<G, ...) */
     PDQ_ERR_UNSUPPORTED = -3, /* p > PDQ_MAX_P */
     PDQ_ERR_NCCL = -4,        /* NCCL missing or a collective failed */
-    PDQ_ERR_NO_DEVICE = -5    /* no CUDA device / not an sm_100 part */
+    PDQ_ERR_NO_DEVICE = -5    /* no CUDA device / not an sm_90 part */
 } pdq_status;
 
 #define PDQ_MAX_P 16 /* design columns supported (p <= 8: register-resident p x p solvers; 9..16: the same code with the small matrices in local memory) */

@@ -1,10 +1,10 @@
 """Unconstrained L-BFGS-B, restated.  TEST INFRASTRUCTURE (see oracle/nbglm.py for the import rules).
 
 The reference fits the apeGLM MAP with ``scipy.optimize.minimize(method="L-BFGS-B", options={"ftol": 1e-8, "gtol": 1e-8})``
-(``/root/reference/pydeseq2/utils.py:1110-1120``) and keeps whatever iterate the optimiser stops at -- on these objectives
+(``pydeseq2/utils.py:1110-1120``) and keeps whatever iterate the optimiser stops at -- on these objectives
 that is 1e-3 .. 1e-2 (relative) away from the true optimum, so a backend can only agree with the reference to better than
 that by walking the same iterates.  scipy (1.18.1 in this image; L-BFGS-B 3.0 of Zhu, Byrd, Lu, Nocedal, translated to C)
-is a third-party dependency that is not under /root/reference; this module restates its published algorithm for the case
+is a third-party dependency that is not part of PyDESeq2; this module restates its published algorithm for the case
 the reference uses -- no bounds -- and is the specification the CUDA routine ``shrink_gene`` (pdq_gene.cuh) implements:
 
 * direction: steepest descent while the memory is empty, otherwise the limited-memory BFGS step with ``m = 10`` pairs and

@@ -1,10 +1,10 @@
 """Generate the golden vectors under tests/golden/ from the REAL reference.  TEST INFRASTRUCTURE.
 
-Runs only in the build container (needs the read-only checkout at /root/reference, imported
-through ``oracle/refshim`` + ``oracle/refshim_orch``; see SURVEY.md Appendix A).  The outputs
-are small ``.npz`` files that travel to the GPU box, where the reference does not exist.
+Needs a PyDESeq2 0.5.3 source checkout, named by the environment variable PYDESEQ2_SRC and
+imported through ``oracle/refshim`` + ``oracle/refshim_orch`` (see SURVEY.md Appendix A).  The
+outputs are small ``.npz`` files; the test suite reads only them and never the reference.
 
-    python oracle/make_golden.py            # rewrites tests/golden/*.npz
+    PYDESEQ2_SRC=<checkout> python oracle/make_golden.py    # rewrites tests/golden/*.npz
 
 Two kinds of fixture:
 
@@ -30,7 +30,9 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import pandas as pd  # noqa: E402
 
-REF = "/root/reference"
+REF = os.environ.get("PYDESEQ2_SRC")
+if not REF:
+    sys.exit("oracle/make_golden.py: set PYDESEQ2_SRC to a PyDESeq2 0.5.3 source checkout (the directory that holds pydeseq2/)")
 OUT = os.path.join(ROOT, "tests", "golden")
 
 

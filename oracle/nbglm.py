@@ -1,7 +1,7 @@
 """CPU oracle for the per-gene negative-binomial GLM hot path.  TEST INFRASTRUCTURE.
 
 This module is a numpy/scipy restatement of the reference's per-gene numerics
-(``/root/reference/pydeseq2/utils.py`` and ``grid_search.py``) and of its joblib gene
+(``pydeseq2/utils.py`` and ``grid_search.py``) and of its joblib gene
 fan-out (``default_inference.py``).  It exists only to *check* the CUDA path:
 
 * importable ONLY from ``tests/``, ``__graft_entry__.smoke()`` and the
@@ -9,11 +9,11 @@ fan-out (``default_inference.py``).  It exists only to *check* the CUDA path:
 * never imported by ``pydeseq2_b200`` (the product fails loudly without its CUDA
   library instead of falling back to this code).
 
-Parity pin: every function below is compared with the *real* reference, imported in
-the build container through ``oracle/refshim``, by ``oracle/make_golden.py``; the
+Parity pin: every function below is compared with the *real* reference, imported from a
+PYDESEQ2_SRC checkout through ``oracle/refshim``, by ``oracle/make_golden.py``; the
 resulting input/output vectors are committed under ``tests/golden/`` and re-checked by
 ``tests/test_oracle_golden.py`` (CPU suite).  Third-party arithmetic the reference
-leans on and that is not under /root/reference (versions of this image):
+leans on and that is not part of PyDESeq2 (versions of this image):
 scipy 1.18.1 ``optimize.minimize(method="L-BFGS-B")``, ``linalg.solve``,
 ``special.gammaln/polygamma``, ``stats.norm.sf``; numpy 2.3.5 ``linalg``;
 scikit-learn 1.9.0 ``LinearRegression`` (least squares, re-expressed with
@@ -399,7 +399,7 @@ class OracleInference:
     """Gene fan-out with the reference's scheduling (default_inference.py:14-198).
 
     joblib/loky, one task per gene, ``batch_size=128``, ``inner_max_num_threads=1`` -- the
-    reference's only parallelism strategy -- so that, timed on the GPU box's host cores, it is
+    reference's only parallelism strategy -- so that, timed on the benchmark machine's host cores, it is
     a like-for-like CPU baseline (``cpu_baseline.kind == "port"``).
     """
 

@@ -1,4 +1,4 @@
-"""pydeseq2_b200 -- B200-native backend for PyDESeq2's per-gene NB-GLM hot path."""
+"""pydeseq2_b200 -- H100-native backend for PyDESeq2's per-gene NB-GLM hot path."""
 __version__ = "0.1.0"
 
 

@@ -1,8 +1,8 @@
 """ctypes binding of ``libpydeseq2_b200.so`` (the C ABI in ``include/pydeseq2_b200.h``).
 
-This is the stub a maintainer of the reference would add to bind the B200 backend
+This is the stub a maintainer of the reference would add to bind the CUDA backend
 (INTEGRATION.md).  There is deliberately no CPU fallback: if the CUDA library has not been
-built, or no sm_100 device is visible, the calls raise.
+built, or no sm_90 (H100) device is visible, the calls raise.
 """
 from __future__ import annotations
 
@@ -25,7 +25,7 @@ ALT_CODES = {None: 0, "greaterAbs": 1, "lessAbs": 2, "greater": 3, "less": 4}
 UNIQUE_ID_BYTES = 128
 PEER_HANDLE_BYTES = 64
 
-STATUS = {0: "ok", -1: "cuda error", -2: "invalid argument", -3: "unsupported", -4: "nccl error", -5: "no sm_100 device"}
+STATUS = {0: "ok", -1: "cuda error", -2: "invalid argument", -3: "unsupported", -4: "nccl error", -5: "no sm_90 device"}
 
 
 class B200Error(RuntimeError):
@@ -134,7 +134,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise B200Error(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). pydeseq2_b200 has no CPU fallback."
+            "(nvcc, sm_90a). pydeseq2_b200 has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in _SIGNATURES.items():
@@ -163,7 +163,7 @@ class Context:
         if rc != 0:
             n = self.lib.pdq_device_count()
             raise B200Error(f"pdq_ctx_create(device={device}) failed: {STATUS.get(rc, rc)} ({n} CUDA device(s) visible); "
-                            "this backend needs an sm_100 (B200) GPU and has no CPU fallback")
+                            "this backend needs an sm_90 (H100) GPU and has no CPU fallback")
         self.h = h
         self.device = int(device)
         self._pin_pool = {}  # nbytes -> [addresses] of released page-locked blocks (cudaHostAlloc is expensive)

@@ -1,4 +1,4 @@
-"""Build ``libpydeseq2_b200.so`` in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build ``libpydeseq2_b200.so`` in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -19,7 +19,7 @@ UNITS = [("pdq_api.cu", "pdq_api", ()), ("pdq_dispatch.cu", "pdq_dispatch", ()),
 SOURCES = sorted({u[0] for u in UNITS})
 HEADERS = ["pdq_math.cuh", "pdq_fast.cuh", "pdq_tables.h", "pdq_trend.cuh", "pdq_gene.cuh", "pdq_shrink.cuh", "pdq_internal.h",
            "pdq_host_linalg.h", os.path.join("..", "..", "include", "pydeseq2_b200.h")]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-fopenmp", "--expt-relaxed-constexpr"]
 
 
@@ -77,7 +77,7 @@ def build(force: bool = False, verbose: bool = False, defines=(), out: str | Non
     if failed is not None:
         raise RuntimeError("nvcc failed: " + " ".join(failed))
     if force or _stale(target, objs):
-        cmd = [_nvcc(), "-shared", "-o", target] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static",
+        cmd = [_nvcc(), "-shared", "-o", target] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart_static",
                                                         "-ldl", "-lrt", "-lpthread", "-lgomp"]
         subprocess.run(cmd, check=True)
     return target

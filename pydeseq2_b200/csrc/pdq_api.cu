@@ -228,8 +228,8 @@ static int pick_lgT(const pdq_ctx* c, int G, int N) {
         // fill ~1024 resident threads per SM: T = smallest power of two with G*T >= SMs*1024, capped by 32 -- but never
         // fewer than 8 lanes: a warp then owns 4 adjacent genes = one full 32-byte sector per sample row, and its tile
         // (4 genes x N samples x 16 B for counts + means) stays small enough for the resident warps of an SM to keep
-        // their tiles in L2 across evaluations.  Measured (scripts/lanes_sweep.sh, ms/step, T = 2|4|8|16|32):
-        // 20 000 x 200: -|1.40|1.25|1.35|- ; 60 000 x 500: -|9.05|8.51|9.23|11.6 ; 125 000 x 1000: 25.1|-|21.5|24.9|35.4
+        // their tiles in L2 across evaluations.  The SM count comes from the device (132 on H100); scripts/lanes_sweep.sh
+        // times the alternatives.
         const double want = (double)c->prop.multiProcessorCount * 1024.0 / (double)(G > 0 ? G : 1);
         T = 8;
         while (T < 32 && (double)T < want) T <<= 1;
@@ -243,7 +243,7 @@ static int pick_lgT(const pdq_ctx* c, int G, int N) {
 static LaunchCfg cfg(const pdq_ctx* c, int G, int N) { return LaunchCfg{c->stream, pick_lgT(c, G, N), c->prop.multiProcessorCount, c->tickets, c->debug}; }
 
 // --------------------------------------------------------------------------------------------- context
-extern "C" const char* pdq_version(void) { return "pydeseq2_b200 0.1.0 (sm_100a)"; }
+extern "C" const char* pdq_version(void) { return "pydeseq2_b200 0.1.0 (sm_90a)"; }
 
 extern "C" int pdq_device_count(void) {
     int n = 0;
@@ -265,7 +265,7 @@ extern "C" int pdq_ctx_create(int device, pdq_ctx** out) {
         delete c;
         return PDQ_ERR_NO_DEVICE;
     }
-    if (c->prop.major < 10) {  // the fatbin holds sm_100a SASS only
+    if (c->prop.major != 9 || c->prop.minor != 0) {  // the fatbin holds sm_90a SASS only, which loads on compute capability 9.0 alone
         delete c;
         return PDQ_ERR_NO_DEVICE;
     }
@@ -869,8 +869,8 @@ static int h2d_2d(pdq_ctx* c, void* dst, const void* src, int64_t ld, int N, int
 // mu it got back from the LFC fit once more (ds.py:338) -- each time as a fresh host array, so pointer identity says nothing.
 // The entry points therefore key device copies on a 128-bit checksum of the FULL content, computed at memory bandwidth by a
 // few host threads; an (N, G) OUTPUT is kept on the device under the same checksum, computed there by a reduction kernel, so
-// that handing it back costs a checksum instead of an upload.  A hit replaces a PCIe transfer (50 GB/s page-locked, ~10-25 GB/s
-// pageable) by a read of host memory.  Never by pointer, never by a sample of the content.  PDQ_RESIDENCY=0 switches it off.
+// that handing it back costs a checksum instead of an upload.  A hit replaces a PCIe transfer (slower still from pageable memory)
+// by a read of host memory.  Never by pointer, never by a sample of the content.  PDQ_RESIDENCY=0 switches it off.
 static const size_t kResMinBytes = 1u << 20;
 static const int kHashSlots = 8;
 
@@ -1064,7 +1064,7 @@ extern "C" int pdq_residency_clear(pdq_ctx* c) {
 }
 
 // ---- gene-block pipeline --------------------------------------------------------------------------------------
-// The plugin calls move 32-64 MB each way around a 0.3 ms kernel.  When every large host buffer is page-locked the call
+// The plugin calls move 32-64 MB each way around a sub-millisecond kernel.  When every large host buffer is page-locked the call
 // is split into gene blocks on two streams: the column block k+1 is uploaded while block k computes and block k-1 is
 // downloaded (PCIe is full duplex, the kernels take `ld`, so a block is just a pointer offset).  Per-gene results do not
 // depend on the split (different lane-group widths only change the order of the floating-point sums).
@@ -1771,8 +1771,8 @@ extern "C" int pdq_peer_push_dev(pdq_ctx* c, pdq_peer_group* g, int k, const dou
     a.err = g->err_dev;
     static const unsigned long long timeout_ms = getenv("PDQ_PEER_TIMEOUT_MS") ? strtoull(getenv("PDQ_PEER_TIMEOUT_MS"), nullptr, 10) : 30000ULL;
     a.timeout_ns = timeout_ms * 1000000ULL;
-    // 64 blocks of 512 threads keep the NVLink store path busy (measured on 2 GPUs: 32 MB leave in 36 us with 64, 148 or 296
-    // blocks alike -- profiles/r2s_peer_probe_n2.txt) and leave a short tail before the signal; PDQ_PEER_BLOCKS overrides
+    // 64 blocks of 512 threads: enough stores in flight for the NVLink path, and a short tail before the signal (not re-tuned on
+    // H100: the multi-GPU path has not been measured there); PDQ_PEER_BLOCKS overrides
     static const int forced = getenv("PDQ_PEER_BLOCKS") ? atoi(getenv("PDQ_PEER_BLOCKS")) : 0;
     const int blocks = forced > 0 ? forced : 64;
     k_peer_push<<<blocks, kPeerThreads, 0, c->stream>>>(a);

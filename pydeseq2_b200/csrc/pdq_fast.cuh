@@ -1,8 +1,7 @@
-// pdq_fast.cuh -- FP64 log / exp / reciprocal tuned for the sm_100a FP64 pipe.
+// pdq_fast.cuh -- FP64 log / exp / reciprocal tuned for the sm_90a FP64 pipe.
 //
-// Why not libdevice's `log`, `exp` and the `/` operator: the ncu profile of round 1 (profiles/README.md)
-// showed that 32 % of all issued warp instructions were UMOV / IMAD.MOV pairs materialising 64-bit polynomial
-// coefficients next to every DFMA, plus BSSY/BSYNC/branch scaffolding around each division's slow path.  Here
+// Why not libdevice's `log`, `exp` and the `/` operator: their SASS materialises 64-bit polynomial coefficients with
+// UMOV / IMAD.MOV pairs next to every DFMA and wraps each division's slow path in BSSY/BSYNC/branch scaffolding.  Here
 //   * coefficients live in __constant__ memory, so DFMA takes them as constant-bank operands (no extra instruction);
 //   * the reciprocal is MUFU.RCP64H + two Newton steps, branch-free (operands on this path are normal, finite);
 //   * special cases (NaN, inf, zero, denormal, |x| huge) fall through to libdevice behind one predictable branch.

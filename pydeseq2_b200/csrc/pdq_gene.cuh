@@ -1526,8 +1526,7 @@ PDQ_HD void trim_class(int nc, bool global_mode, int& ntrim, double& scale) {
 // mean of v[s:e) after dropping the ntrim smallest and ntrim largest entries (np.sort + slice + mean), by SELECTION: every lane
 // sorts its own strided share of the cell in place (insertion sort, m = n_c / T entries), then the group pops the smallest and
 // the largest remaining head ntrim times (one argmin / argmax butterfly each); what is left between the lanes' cursors is the
-// kept set, summed directly.  O(m^2 + ntrim log T) per lane instead of the O(n_c^2 / T) rank counting of round 1 (1.1 ms at
-// two cells of 100 samples, 58 ms at two cells of 500).  Ties carry equal values, so which of them is dropped does not matter.
+// kept set, summed directly.  O(m^2 + ntrim log T) per lane instead of the O(n_c^2 / T) rank counting of round 1.  Ties carry equal values, so which of them is dropped does not matter.
 // The cell is left permuted (callers only need it as a multiset).
 PDQ_HD double trimmed_mean_cell(const Group& grp, double* v, int s, int e, int ntrim) {
     const int nc = e - s, T = grp.T;

@@ -86,7 +86,7 @@ int launch_size_factors(const LaunchCfg&, const int64_t* counts, int64_t ld, int
 int launch_select_disp(const LaunchCfg&, const double* gw, const double* mp, const double* fitted, const double* out16,
                        size_t n, double lo, double hi, double* disp, double* outlier);
 
-// largest dynamic shared memory a kernel of this library may ask for (B200: 227 KB per CTA)
+// largest dynamic shared memory a kernel of this library may ask for (H100: 227 KB per CTA)
 constexpr size_t kMaxDynSmem = 227 * 1024;
 
 }  // namespace pdq

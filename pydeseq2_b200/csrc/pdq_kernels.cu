@@ -1,4 +1,4 @@
-// pdq_kernels.cu -- sm_100a kernels of the per-gene NB-GLM hot path and their launchers.
+// pdq_kernels.cu -- sm_90a kernels of the per-gene NB-GLM hot path and their launchers.
 //
 // Every kernel has the same skeleton (DESIGN.md §3):
 //   1. one elected thread stages the design pack (X column-major, size factors, log size factors)
@@ -39,9 +39,9 @@ namespace {
 
 constexpr int kBlock = 128;
 constexpr int kWarps = kBlock / 32;
-// resident blocks per SM the two heavy kernels are compiled for (register cap = 65536 / (128 * blocks)); tuned on B200
-// (scripts/variants_sweep.sh; irls 6|5|4: 0.304|0.310|0.308 ms at 20 000 x 200, 1.93|1.92|1.79 ms at 60 000 x 500;
-//  alpha_mle 5|4|3: 0.249|0.240|0.203 ms and 1.29|1.23|1.09 ms -- the Newton-opening sweep needs the registers)
+// resident blocks per SM the two heavy kernels are compiled for (register cap = 65536 / (128 * blocks)).  The trade-off is set
+// by the 64 K-register file per SM, which H100 has too: fewer resident blocks buy registers for the Newton-opening sweep of
+// alpha_mle.  scripts/variants_sweep.sh times other values.
 #ifndef PDQ_IRLS_MINB
 #define PDQ_IRLS_MINB 4
 #endif
@@ -652,8 +652,8 @@ struct ClusterReducer {
             }
         }
         if (nblocks > 1) cluster.sync(); else __syncthreads();  // release the DSMEM stores / acquire the peers'
-        // k threads add up the blocks' slots, everybody reads the k totals (broadcast reads).  The first version had EVERY thread
-        // add nblocks * k slots itself: 160 shared-memory reads per thread and pass -- that alone was ~5 us of every pass.
+        // k threads add up the blocks' slots, everybody reads the k totals (broadcast reads).  Having EVERY thread
+        // add nblocks * k slots itself would cost 160 shared-memory reads per thread and pass.
         if ((int)threadIdx.x < k) {
             double tot = 0.0;
             for (unsigned r = 0; r < nblocks; ++r) tot += slots[(parity * kTrendMaxCluster + r) * kTrendK + threadIdx.x];
@@ -854,8 +854,7 @@ inline int grid_for(int G, int lgT) {
 inline int alpha_descending() {
     static int v = -1;
     if (v < 0) {
-        // tuning hook, default off: measured slower (alpha_mle_genewise 0.196 vs 0.167 ms at 20 000 x 200, 3.14 vs 2.98 ms at
-        // 125 000 x 1 000) -- with ascending counts the costly high-count tiles overlap the cheap ones' tail just as well
+        // tuning hook, default off: with ascending counts the costly high-count tiles overlap the cheap ones' tail just as well
         const char* e = getenv("PDQ_ALPHA_DESCENDING");
         v = e ? (atoi(e) != 0) : 0;
     }
@@ -990,7 +989,7 @@ __global__ void k_scatter_rows(const double* __restrict__ in, double* __restrict
 }
 
 // ---- content checksum of a device buffer: the device half of the residency cache of pdq_api.cu (host_hash there computes the
-// same two wrapping sums with host threads).  HBM-bound: 32 MB in ~10 us.
+// same two wrapping sums with host threads).  HBM-bound.
 __global__ void __launch_bounds__(256) k_hash(const uint64_t* __restrict__ w, size_t n, unsigned long long* out) {
     unsigned long long a = 0, b = 0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {

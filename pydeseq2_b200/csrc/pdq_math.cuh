@@ -1,7 +1,7 @@
 // pdq_math.cuh -- FP64 building blocks shared by every per-gene routine.
 //
 // Everything here is `__host__ __device__` so that the exact same source is compiled (a) by nvcc
-// for sm_100a and (b) by g++ into the host emulator used by the CPU test-suite
+// for sm_90a and (b) by g++ into the host emulator used by the CPU test-suite
 // (tests/emu/, test infrastructure only -- the product never loads it).
 #pragma once
 

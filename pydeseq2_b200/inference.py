@@ -1,10 +1,10 @@
-"""``B200Inference`` -- drop-in ``pydeseq2.inference.Inference`` backend running on one B200.
+"""``B200Inference`` -- drop-in ``pydeseq2.inference.Inference`` backend running on one H100.
 
-The class mirrors the reference's plugin interface (``/root/reference/pydeseq2/inference.py:9-362``,
+The class mirrors the reference's plugin interface (``pydeseq2/inference.py:9-362``,
 default implementation ``default_inference.py:14-264``): same method names, argument meaning and
 return conventions, so ``DeseqDataSet(..., inference=B200Inference())`` and
 ``DeseqStats(..., inference=B200Inference())`` work unchanged.  Every per-gene method is one call
-through the C ABI (``include/pydeseq2_b200.h``) into hand-written sm_100a kernels batched over all
+through the C ABI (``include/pydeseq2_b200.h``) into hand-written sm_90a kernels batched over all
 genes; host code here only marshals numpy buffers.
 
 Deliberate differences from ``DefaultInference`` (all documented in DESIGN.md):
@@ -29,7 +29,7 @@ from ._lib import ALT_CODES, B200Error, as_f64p, as_i64p
 
 try:  # the reference, when it is importable, provides the ABC we plug into
     from pydeseq2.inference import Inference as _InferenceBase  # type: ignore
-except Exception:  # pragma: no cover - the GPU box has no reference checkout
+except Exception:  # pragma: no cover - pydeseq2 is not installed
 
     class _InferenceBase(ABC):
         """Structural mirror of ``pydeseq2.inference.Inference`` (inference.py:9-362)."""
@@ -185,7 +185,7 @@ class _CudaOps:
 
 
 class B200Inference(_InferenceBase):
-    """B200 implementation of the reference's ``Inference`` plugin API.
+    """CUDA (H100) implementation of the reference's ``Inference`` plugin API.
 
     Parameters
     ----------

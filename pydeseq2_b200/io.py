@@ -1,7 +1,7 @@
 """Count-matrix ingestion (SURVEY.md §8 f-4): CSV -> the (samples, genes) int64 matrix of the hot path, parsed by native host
 threads straight into a page-locked buffer, so that the upload that follows runs at the full PCIe rate and nothing is copied or
 converted on the way.  The reference loads the same files with ``pandas.read_csv(path, index_col=0).T``
-(``/root/reference/examples/plot_pandas_io_example.py:57-66``) and converts to integers at construction (``dds.py:245-249``).
+(``examples/plot_pandas_io_example.py:57-66``) and converts to integers at construction (``dds.py:245-249``).
 """
 from __future__ import annotations
 

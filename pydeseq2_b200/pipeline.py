@@ -1,5 +1,5 @@
 """Hot-path drivers: the order in which ``DeseqDataSet.deseq2()`` + ``DeseqStats.run_wald_test()`` call the
-``Inference`` plugin (``/root/reference/pydeseq2/dds.py:516-562``, ``ds.py:303-360``), without the orchestrator's
+``Inference`` plugin (``pydeseq2/dds.py:516-562``, ``ds.py:303-360``), without the orchestrator's
 AnnData/pandas state and without the stages SURVEY.md §8 marks "next" (Cook's distances / outlier refit,
 independent filtering).
 

@@ -1,7 +1,7 @@
 """Synthetic negative-binomial count generator (SURVEY.md §8(d), BASELINE.md §3).
 
 Modelled on DESeq2's ``makeExampleDESeqDataSet`` (which the reference's shipped
-``datasets/synthetic`` also derives from, ``/root/reference/datasets/README.md:6-8``):
+``datasets/synthetic`` also derives from, ``datasets/README.md:6-8``):
 per gene ``beta0/ln2 ~ N(4, 2)``, other coefficients ``/ln2 ~ N(0, 0.5)``,
 ``alpha_g = 4/exp(beta0) + 0.1``, ``sf_i = exp(N(0, 0.2))``, ``y ~ NB(mean=sf_i*exp(x_i.beta_g),
 size=1/alpha_g)`` as int64 in the reference's native layout: (N samples, G genes), C-contiguous,

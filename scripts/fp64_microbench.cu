@@ -1,5 +1,5 @@
 // FP64 pipe microbenchmark (tuning aid, not part of the library): DFMA throughput as a function of resident warps per SM and
-// independent chains per thread, plus the mixed case DFMA + integer ALU work.  nvcc -O3 -arch=sm_100a -o scripts/bin/fp64_microbench
+// independent chains per thread, plus the mixed case DFMA + integer ALU work.  nvcc -O3 -arch=sm_90a -o /tmp/fp64_microbench
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,5 +1,5 @@
 """Times the four large host-buffer plugin calls for several gene-block pipeline depths (PDQ_PIPELINE).
-Run on a B200:  python scripts/pipe_microbench.py [G] [N]"""
+Run on an H100:  python scripts/pipe_microbench.py [G] [N]"""
 import os
 import sys
 import time

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Build container only: the CPU baseline `bench.py` times on the GPU box is the oracle PORT (the reference cannot travel).  This
-script times the REAL reference's DefaultInference and the port through the same host glue (pipeline.fit_host) on the same
+"""The CPU baseline `bench.py` times is the oracle PORT (the benchmark does not depend on the reference).  This script, run with
+PYDESEQ2_SRC naming a PyDESeq2 0.5.3 source checkout, times the REAL reference's DefaultInference and the port through the same host glue (pipeline.fit_host) on the same
 input, so that the record shows the port is not slower than the code it stands for.  Output: one JSON line."""
 import json
 import os

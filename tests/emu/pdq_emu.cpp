@@ -1,6 +1,6 @@
 // pdq_emu.cpp -- HOST EMULATOR of the device per-gene routines.  TEST INFRASTRUCTURE ONLY.
 //
-// Compiles pydeseq2_b200/csrc/pdq_gene.cuh (the exact source the sm_100a kernels are built from)
+// Compiles pydeseq2_b200/csrc/pdq_gene.cuh (the exact source the sm_90a kernels are built from)
 // with g++, one "lane" per gene (T = 1, Group::sum is the identity), so that the CPU test-suite can
 // check the algorithmic content of the kernels -- IRLS control flow, the bounded root search for
 // the dispersion, Cholesky algebra, special functions -- against the oracle without a GPU.

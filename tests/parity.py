@@ -17,15 +17,16 @@ TOL_WALD = 1e-9
 
 
 def report(kind, name, **fields):
-    """Append one JSON line per parity case to gpurun_out/parity_report.jsonl (measured mismatch fractions / worst errors);
-    the GPU session copies the file to profiles/.  Never fails a test."""
+    """Append one JSON line per parity case (measured mismatch fractions / worst errors) to the file named by the environment
+    variable PDQ_PARITY_REPORT, when it is set.  Never fails a test."""
     import json
     import os
 
+    path = os.environ.get("PDQ_PARITY_REPORT")
+    if not path:
+        return
     try:
-        root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-        os.makedirs(os.path.join(root, "gpurun_out"), exist_ok=True)
-        with open(os.path.join(root, "gpurun_out", "parity_report.jsonl"), "a") as f:
+        with open(path, "a") as f:
             f.write(json.dumps({"kind": kind, "case": name, **fields}) + "\n")
     except OSError:
         pass

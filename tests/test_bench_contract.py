@@ -5,6 +5,8 @@ import os
 import subprocess
 import sys
 
+import numpy as np
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -23,10 +25,68 @@ def test_reference_arm_prints_the_contract_line():
     assert "workload" in line["config"] and line["scaling"] == "weak" and line["dtype"] == "f64"
 
 
+def test_reference_arm_runs_exactly_the_requested_steps():
+    r = _run("--impl", "reference", "--steps", "7", "--warmup", "2", "--genes", "300", "--samples", "12", "--cpu-sample-genes", "100")
+    assert r.returncode == 0, r.stderr[-2000:]
+    line = json.loads(r.stdout.strip().splitlines()[-1])
+    assert line["steps"] == 7 and line["warmup"] == 2 and len(line["cpu_baseline"]["pass_s"]) == 7
+
+
+def test_dump_outputs_is_refused_for_the_reference_arm(tmp_path):
+    r = _run("--impl", "reference", "--steps", "1", "--dump-outputs", str(tmp_path / "d"))
+    assert r.returncode != 0 and "--dump-outputs" in r.stderr and not (tmp_path / "d").exists()
+
+
+def _bench_module():
+    import importlib.util
+
+    spec = importlib.util.spec_from_file_location("bench_under_test", os.path.join(ROOT, "bench.py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+def _fake_result(G, p=2):
+    from types import SimpleNamespace
+
+    rng = np.random.default_rng(1)
+    res = {k: rng.random(G) for k in ("dispersions", "genewise", "map", "pvalue", "stat", "se", "normed_means")}
+    res.update(lfc=rng.random((G, p)), lfc_converged=np.ones(G), trend=SimpleNamespace(coeffs=np.array([0.1, 2.0])),
+               prior_var=0.25, squared_logres=0.5)
+    return res
+
+
+def test_dump_outputs_writes_every_array_below_the_cap(tmp_path):
+    bench = _bench_module()
+    res = _fake_result(500)
+    bench.dump_outputs(str(tmp_path), res)
+    assert not (tmp_path / "gene_index.npy").exists()
+    for k in ("dispersions", "lfc", "lfc_converged", "trend_coeffs", "prior_var"):
+        got = np.load(tmp_path / f"{k}.npy")
+        assert got.dtype == np.float64
+    np.testing.assert_array_equal(np.load(tmp_path / "lfc.npy"), res["lfc"])
+    assert float(np.load(tmp_path / "prior_var.npy")) == 0.25
+
+
+def test_dump_outputs_samples_genes_above_the_cap(tmp_path):
+    bench = _bench_module()
+    res, cap = _fake_result(20000), 200_000
+    for d in ("a", "b"):
+        bench.dump_outputs(str(tmp_path / d), res, cap=cap)
+    files = sorted(os.listdir(tmp_path / "a"))
+    assert sum(os.path.getsize(tmp_path / "a" / f) for f in files) <= cap
+    idx = np.load(tmp_path / "a" / "gene_index.npy").astype(np.int64)
+    assert 1000 < len(idx) < 20000 and np.all(np.diff(idx) > 0)
+    np.testing.assert_array_equal(np.load(tmp_path / "a" / "lfc.npy"), res["lfc"][idx])
+    np.testing.assert_array_equal(np.load(tmp_path / "a" / "pvalue.npy"), res["pvalue"][idx])
+    for f in files:  # the sample is fixed: the same genes every time
+        np.testing.assert_array_equal(np.load(tmp_path / "a" / f), np.load(tmp_path / "b" / f))
+
+
 def test_product_arm_fails_loudly_without_a_gpu():
     import ctypes
 
-    try:  # a visible CUDA device means this is the GPU box: nothing to check here
+    try:  # with a visible CUDA device the product arm runs: nothing to check here
         if ctypes.CDLL("libcuda.so.1").cuInit(0) == 0:
             n = ctypes.c_int(0)
             ctypes.CDLL("libcuda.so.1").cuDeviceGetCount(ctypes.byref(n))

@@ -1,4 +1,4 @@
-"""GPU suite, needs >= 2 devices (skipped otherwise; run with `gpurun --gpus 2`): gene shards over NCCL through the C ABI equal
+"""GPU suite, needs >= 2 devices (skipped otherwise): gene shards over NCCL through the C ABI equal
 the single-GPU fit -- the exchange before the trend step and the end-of-call exchange of the result tables, through grouped NCCL
 all-gathers and through the peer-memory push kernel (CUDA IPC windows, NVLink stores), with ragged shards, eager and as a replayed
 CUDA graph (tests/multi_gpu_worker.py)."""
@@ -34,10 +34,4 @@ def test_sharded_fit_equals_single_gpu_fit(world, N, G, design, exchange):
     line = [l for l in r.stdout.splitlines() if l.startswith("{")]
     assert r.returncode == 0 and line, r.stdout[-2000:] + r.stderr[-2000:]
     rec = json.loads(line[-1])
-    try:
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        with open(os.path.join(ROOT, "gpurun_out", "multi_gpu_check.jsonl"), "a") as f:
-            f.write(json.dumps(rec) + "\n")
-    except OSError:
-        pass
     assert rec["ok"], rec
