@@ -201,6 +201,21 @@ int pdq_lfc_shrink_nbinom_glm(pdq_ctx* ctx, const double* X, const int64_t* coun
  * of log(count) - gene mean (radix select), exponentiated.  `sf_out` (N,).  All entries NaN when every gene holds a zero
  * (the reference then switches to its iterative fallback, dds.py:682-690). */
 int pdq_size_factors(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, double* sf_out, double* logmeans_out /* per-gene mean log count (-inf when the gene holds a zero), may be NULL */);
+/* Size factors of NEW samples against the log means of a fit -- preprocessing.deseq2_norm_transform (preprocessing.py:59-102), what
+ * DeseqDataSet.vst_transform(counts) does with held-out counts (dds.py:478-486).  `logmeans` (G,): genes with a non-finite entry
+ * are left out (the fit's filtered_genes are exactly its finite log means).  A zero count in a kept gene enters the median as
+ * -inf, as in numpy, so a sample with zeros in at least half of the kept genes gets size factor 0.  NaN when no gene is kept. */
+int pdq_size_factors_from_logmeans(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
+                                   double* sf_out);
+
+/* Variance-stabilising transform -- DeseqDataSet.vst_transform (dds.py:438-514) on raw counts: q = counts / size_factors
+ * (a true division, bit-identical to the reference's normed_counts), then per element
+ *   kind 0 (parametric, c0 = a0, c1 = a1):  log2((1 + a1 + 2 a0 q + 2 sqrt(a0 q (1 + a1 + a0 q))) / (4 a0))
+ *   kind 1 (mean, c0 = mean dispersion d):  (2 asinh(sqrt(d q)) - log d - log 4) / log 2
+ * `out` (N, G) with row pitch ld_out.  PDQ_ERR_INVALID for an unknown kind or c0 <= 0.  The counts go through the residency
+ * cache (after the fit calls of vst_fit they are on the device already). */
+int pdq_vst_transform(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, const double* size_factors, int kind, double c0,
+                      double c1, double* out, int64_t ld_out);
 
 /* Cook's distances -- DeseqDataSet.calculate_cooks (dds.py:986-1040) with the trimmed-moments dispersion
  * (utils.py:914-960; cells = identical design rows with >= 3 replicates) -- and the two per-gene decisions derived from them:
@@ -278,6 +293,11 @@ int pdq_lfc_shrink_dev(pdq_ctx* ctx, const pdq_design* design, const int64_t* co
 /* device-resident flavour of pdq_size_factors; `logmeans_out` (G,) may be NULL */
 int pdq_size_factors_dev(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, double* sf_out,
                          double* logmeans_out);
+/* device-resident flavours of pdq_size_factors_from_logmeans and pdq_vst_transform (`size_factors` is device memory here) */
+int pdq_size_factors_from_logmeans_dev(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
+                                       double* sf_out);
+int pdq_vst_transform_dev(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, const double* size_factors, int kind,
+                          double c0, double c1, double* out, int64_t ld_out);
 /* Final dispersions (dds.py:918-932): clip(MAP), except genes with log(genewise) > log(fitted) + 2 sqrt(squared_logres)
  * which keep their clipped genewise value; `trend_out16` is the record written by pdq_trend_fit_dev.
  * `outlier_out` (n,) 0/1 may be NULL. */

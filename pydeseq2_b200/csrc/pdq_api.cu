@@ -749,6 +749,32 @@ extern "C" int pdq_size_factors_dev(pdq_ctx* c, const int64_t* counts, int64_t l
     return done(c, launch_size_factors(cfg(c, G, N), counts, ld, N, G, (double*)lm, (double*)scratch, sf_out), "size_factors");
 }
 
+extern "C" int pdq_size_factors_from_logmeans_dev(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
+                                                  double* sf_out) {
+    CHECK_CTX(c);
+    if (!counts || !logmeans || !sf_out || N <= 0 || G <= 0 || ld < G)
+        return fail(c, PDQ_ERR_INVALID, "pdq_size_factors_from_logmeans_dev: bad arguments");
+    void* scratch;
+    if (int e = ensure(c, kBufB, (size_t)N * G * 8, &scratch)) return e;
+    return done(c, launch_size_factors_from_logmeans(cfg(c, G, N), counts, ld, N, G, logmeans, (double*)scratch, sf_out),
+                "size_factors_from_logmeans");
+}
+
+static int vst_check(pdq_ctx* c, const void* counts, const void* sf, const void* out, int64_t ld, int N, int G, int kind, double c0,
+                     int64_t ld_out, const char* what) {
+    if (!counts || !sf || !out || N <= 0 || G <= 0 || ld < G || ld_out < G) return fail(c, PDQ_ERR_INVALID, "%s: bad arguments", what);
+    if (kind != 0 && kind != 1) return fail(c, PDQ_ERR_INVALID, "%s: unknown kind %d (0 parametric, 1 mean)", what, kind);
+    if (!(c0 > 0.0)) return fail(c, PDQ_ERR_INVALID, "%s: %s must be > 0", what, kind == 0 ? "a0" : "the mean dispersion");
+    return PDQ_OK;
+}
+
+extern "C" int pdq_vst_transform_dev(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, int G, const double* size_factors, int kind,
+                                     double c0, double c1, double* out, int64_t ld_out) {
+    CHECK_CTX(c);
+    if (int e = vst_check(c, counts, size_factors, out, ld, N, G, kind, c0, ld_out, "pdq_vst_transform_dev")) return e;
+    return done(c, launch_vst_transform(cfg(c, G, N), counts, ld, N, G, size_factors, kind, c0, c1, out, ld_out), "vst_transform");
+}
+
 extern "C" int pdq_gather_columns_dev(pdq_ctx* c, const double* in, int64_t ld_in, int N, const int* idx_dev, int R, double* out,
                                       int64_t ld_out) {
     CHECK_CTX(c);
@@ -1447,6 +1473,57 @@ extern "C" int pdq_size_factors(pdq_ctx* c, const int64_t* counts, int64_t ld, i
     CU(c, cudaMemcpyAsync(sf_out, dsf, (size_t)N * 8, cudaMemcpyDeviceToHost, c->stream));
     if (logmeans_out) CU(c, cudaMemcpyAsync(logmeans_out, dlm, (size_t)G * 8, cudaMemcpyDeviceToHost, c->stream));
     return call_end(c, nullptr, {});
+}
+
+extern "C" int pdq_size_factors_from_logmeans(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
+                                              double* sf_out) {
+    CHECK_CTX(c);
+    if (!counts || !logmeans || !sf_out || N <= 0 || G <= 0 || ld < G)
+        return fail(c, PDQ_ERR_INVALID, "pdq_size_factors_from_logmeans: bad arguments");
+    void *dc, *dsf, *dlm;
+    res_begin(c);
+    bool up_c;
+    if (int e = res_input(c, counts, ld, N, G, 8, kBufCounts, &dc, &up_c)) return e;
+    if (int e = ensure(c, kBufE, (size_t)N * 8, &dsf)) return e;
+    if (int e = ensure(c, kBufG, (size_t)G * 8, &dlm)) return e;
+    if (up_c)
+        if (int e = h2d_2d(c, dc, counts, ld, N, G, 8)) return e;
+    if (int e = vec_h2d(c, dlm, logmeans, (size_t)G * 8)) return e;
+    if (int e = pdq_size_factors_from_logmeans_dev(c, (const int64_t*)dc, G, N, G, (const double*)dlm, (double*)dsf)) return e;
+    CU(c, cudaMemcpyAsync(sf_out, dsf, (size_t)N * 8, cudaMemcpyDeviceToHost, c->stream));
+    return call_end(c, nullptr, {});
+}
+
+// counts through the residency cache (after the fit calls of vst_fit they are on the device already), the (N, G) result back
+// through the page-locked staging ring, in gene blocks overlapping the download with the next block's transform
+extern "C" int pdq_vst_transform(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, int G, const double* size_factors, int kind,
+                                 double c0, double c1, double* out, int64_t ld_out) {
+    CHECK_CTX(c);
+    if (int e = vst_check(c, counts, size_factors, out, ld, N, G, kind, c0, ld_out, "pdq_vst_transform")) return e;
+    void *dc, *dsf, *dout;
+    res_begin(c);
+    bool up_c;
+    if (int e = res_input(c, counts, ld, N, G, 8, kBufCounts, &dc, &up_c)) return e;
+    if (int e = ensure(c, kBufE, (size_t)N * 8, &dsf)) return e;
+    if (int e = ensure(c, kBufA, (size_t)N * G * 8, &dout)) return e;
+    if (int e = vec_h2d(c, dsf, size_factors, (size_t)N * 8)) return e;
+    Pipe pp;
+    if (int e = pipe_begin(c, G, {up_c ? (const void*)counts : nullptr, out}, &pp)) return e;
+    for (int b = 0; b < pp.nb; ++b) {
+        if (up_c)
+            if (int e = cols_h2d(c, pp, b, dc, G, counts, ld, N, 8)) return e;
+        if (int e = done(c, launch_vst_transform(pp.cfg_for(b, N), (const int64_t*)dc + pp.g0(b), G, N, pp.gb(b), (const double*)dsf, kind,
+                                                 c0, c1, (double*)dout + pp.g0(b), G),
+                         "vst_transform"))
+            return e;
+        if (ld_out == G) {
+            if (int e = cols_d2h(c, pp, b, out, G, dout, G, N, 8)) return e;
+        } else {
+            CU(c, cudaMemcpy2DAsync((char*)out + (size_t)pp.g0(b) * 8, (size_t)ld_out * 8, (const char*)dout + (size_t)pp.g0(b) * 8,
+                                    (size_t)G * 8, (size_t)pp.gb(b) * 8, N, cudaMemcpyDeviceToHost, pp.st(b)));
+        }
+    }
+    return call_end(c, &pp, {});
 }
 
 extern "C" int pdq_dispersion_trend_gamma_glm(pdq_ctx* c, const double* cov, const double* targets, size_t n, double* coeffs_out,

@@ -83,6 +83,11 @@ int launch_hash(cudaStream_t stream, int sm_count, const void* dptr, size_t word
 int launch_fp64_peak(const LaunchCfg&, double* out /* sm_count * 8 * 256 doubles */, int iters, double* flop);
 int launch_size_factors(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, double* logmeans,
                         double* scratch, double* sf_out);
+int launch_size_factors_from_logmeans(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
+                                      double* scratch, double* sf_out);
+// kind 0 parametric (c0 = a0, c1 = a1), 1 mean (c0 = mean dispersion); see pdq_vst.cuh
+int launch_vst_transform(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, const double* sf, int kind, double c0,
+                         double c1, double* out, int64_t ld_out);
 int launch_select_disp(const LaunchCfg&, const double* gw, const double* mp, const double* fitted, const double* out16,
                        size_t n, double lo, double hi, double* disp, double* outlier);
 

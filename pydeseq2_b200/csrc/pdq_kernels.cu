@@ -17,6 +17,7 @@
 #include "pdq_gene.cuh"
 #include "pdq_trend.cuh"
 #include "pdq_shrink.cuh"
+#include "pdq_vst.cuh"
 #include "pdq_internal.h"
 
 // This file is compiled once per RANGE OF DESIGN WIDTHS (pydeseq2_b200/build.py): the base unit (PDQ_TU_P = 0) holds the kernels
@@ -811,9 +812,8 @@ __global__ void __launch_bounds__(1024) k_size_factor_median(const int64_t* __re
     __syncthreads();
     unsigned cnt = 0;
     for (int g = threadIdx.x; g < G; g += blockDim.x) {
-        const double lm = logmeans[g];
-        const bool keep = fabs(lm) <= 1.7976931348623157e308;  // ~np.isinf(logmeans); NaN cannot occur for counts >= 0
-        row[g] = keep ? log((double)c[g]) - lm : __longlong_as_double(0x7ff8000000000000ll);
+        bool keep;
+        row[g] = log_ratio_entry(c[g], logmeans[g], keep);
         cnt += keep;
     }
     atomicAdd(&cnt_s, cnt);
@@ -841,6 +841,28 @@ __global__ void k_select_disp(const double* __restrict__ gw, const double* __res
     const bool out = log(g) > log(fitted[i]) + 2.0 * sqrt(c->squared_logres);
     disp[i] = out ? g : m;
     if (outlier) outlier[i] = out ? 1.0 : 0.0;
+}
+
+// ---- variance-stabilising transform (dds.py:438-514): (N, G) int64 counts -> (N, G) float64, elementwise ----------------
+// 16 bytes in and 16 bytes out per pair of genes and ~50 FP64 operations per element: bound by HBM, not by the FP64 pipe.
+// With `vec` (both pitches even, both bases 16-byte aligned) a thread moves a pair of genes with one 16-byte load and one
+// 16-byte store; the odd last gene of a row, and every gene without `vec`, takes the scalar path.  blockIdx.y walks the samples.
+__global__ void __launch_bounds__(256) k_vst_transform(const int64_t* __restrict__ counts, int64_t ld, int N, int G,
+                                                       const double* __restrict__ sf, const VstParams prm, double* __restrict__ out,
+                                                       int64_t ld_out, int vec) {
+    const int pairs = vec ? G >> 1 : 0;
+    const int stride = gridDim.x * blockDim.x;
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    for (int n = blockIdx.y; n < N; n += gridDim.y) {
+        const double s = sf[n];
+        const int64_t* row = counts + (int64_t)n * ld;
+        double* orow = out + (int64_t)n * ld_out;
+        for (int j = t; j < pairs; j += stride) {
+            const longlong2 y = reinterpret_cast<const longlong2*>(row)[j];
+            reinterpret_cast<double2*>(orow)[j] = make_double2(vst_value(y.x, s, prm), vst_value(y.y, s, prm));
+        }
+        for (int g = 2 * pairs + t; g < G; g += stride) orow[g] = vst_value(row[g], s, prm);
+    }
 }
 
 #endif  // PDQ_TU_P == 0
@@ -1342,6 +1364,26 @@ int launch_size_factors(const LaunchCfg& c, const int64_t* counts, int64_t ld, i
     k_size_factor_median<<<N, 1024, 0, c.stream>>>(counts, ld, G, logmeans, scratch, sf_out);
     if (int e = check_launch()) return e;
     return 2;
+}
+
+// held-out samples (preprocessing.py:59-102): the medians against the caller's log means, non-finite entries = genes left out
+int launch_size_factors_from_logmeans(const LaunchCfg& c, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
+                                      double* scratch, double* sf_out) {
+    k_size_factor_median<<<N, 1024, 0, c.stream>>>(counts, ld, G, logmeans, scratch, sf_out);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_vst_transform(const LaunchCfg& c, const int64_t* counts, int64_t ld, int N, int G, const double* sf, int kind, double c0,
+                         double c1, double* out, int64_t ld_out) {
+    const bool vec = ld % 2 == 0 && ld_out % 2 == 0 && (reinterpret_cast<uintptr_t>(counts) & 15) == 0 &&
+                     (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    const int units = vec ? (G + 1) / 2 : G;
+    const unsigned bx = (unsigned)((units + 255) / 256);
+    const unsigned by = (unsigned)(N < 65535 ? N : 65535);
+    k_vst_transform<<<dim3(bx, by), 256, 0, c.stream>>>(counts, ld, N, G, sf, VstParams{kind, c0, c1}, out, ld_out, vec ? 1 : 0);
+    if (int e = check_launch()) return e;
+    return 1;
 }
 
 int launch_select_disp(const LaunchCfg& c, const double* gw, const double* mp, const double* fitted, const double* out16,

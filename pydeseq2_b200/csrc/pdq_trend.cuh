@@ -280,8 +280,10 @@ PDQ_HD double median_of(R& red, const double* res, size_t n, size_t cnt, bool ab
     const size_t k = cnt / 2;
     const double hi = select_kth(red, res, n, absdev, center, hist, k);  // upper median
     if (cnt & 1) return hi;
-    // even count: the lower median is the largest value below `hi`, unless `hi` is duplicated down to rank k-1
-    double less = 0.0, mx = -1.7976931348623157e308;
+    // even count: the lower median is the largest value below `hi`, unless `hi` is duplicated down to rank k-1.  The running
+    // maximum starts at -inf, not at the lowest finite double: held-out size factors take medians of log ratios that hold -inf
+    // (a zero count in a gene of the fit), and a lower median of -inf must stay -inf, as in np.median
+    double less = 0.0, mx = -HUGE_VAL;
     for (size_t i = red.tid(); i < n; i += red.nthreads()) {
         const double r = res[i];
         if (!(r == r)) continue;
@@ -295,6 +297,14 @@ PDQ_HD double median_of(R& red, const double* res, size_t n, size_t cnt, bool ab
     mx = red.max_one(mx);
     const double lo = ((size_t)less >= k) ? mx : hi;
     return 0.5 * (lo + hi);
+}
+
+// One entry of a sample's median of ratios (preprocessing.py:52-54, 89-97): log(count) - log mean of the gene, or NaN -- left out of
+// the median -- for a gene whose log mean is not finite (~np.isinf(logmeans); NaN cannot occur for counts >= 0).  A zero count in
+// a kept gene gives -inf, which takes part in the median as in numpy.  `keep` says whether the gene counts.
+PDQ_HD double log_ratio_entry(int64_t y, double logmean, bool& keep) {
+    keep = fabs(logmean) <= 1.7976931348623157e308;
+    return keep ? log((double)y) - logmean : (0.0 / 0.0);
 }
 
 // `res` : n doubles of scratch; `hist`: 514 unsigned in block-shared memory (see select_kth); `trigamma_c` = polygamma(1, (N-p)/2)

@@ -27,6 +27,8 @@ import numpy as np
 from . import _lib
 from ._lib import ALT_CODES, B200Error, as_f64p, as_i64p
 
+VST_KINDS = {"parametric": 0, "mean": 1}  # `kind` of pdq_vst_transform
+
 try:  # the reference, when it is importable, provides the ABC we plug into
     from pydeseq2.inference import Inference as _InferenceBase  # type: ignore
 except Exception:  # pragma: no cover - pydeseq2 is not installed
@@ -154,6 +156,15 @@ class _CudaOps:
         self._io((counts,), (sf,))
         self.ctx.check(self.lib.pdq_size_factors(self.ctx.h, as_i64p(counts), ld, N, G, as_f64p(sf),
                                                  as_f64p(logmeans) if logmeans is not None else None))
+
+    def size_factors_from_logmeans(self, counts, ld, N, G, logmeans, sf):
+        self._io((counts, logmeans), (sf,))
+        self.ctx.check(self.lib.pdq_size_factors_from_logmeans(self.ctx.h, as_i64p(counts), ld, N, G, as_f64p(logmeans), as_f64p(sf)))
+
+    def vst_transform(self, counts, ld, N, G, sf, kind, c0, c1, out, ld_out):
+        self._io((counts, sf), (out,))
+        self.ctx.check(self.lib.pdq_vst_transform(self.ctx.h, as_i64p(counts), ld, N, G, as_f64p(sf), kind, c0, c1, as_f64p(out),
+                                                  ld_out))
 
     def lfc_shrink(self, X, counts, ld, N, G, p, size, offset, prior_no_shrink_scale, prior_scale, shrink_index, lfcs, inv_hessians,
                    conv):
@@ -384,16 +395,30 @@ class B200Inference(_InferenceBase):
             return None
         return np.array([out16[0], out16[1]]), fitted, float(out16[8]), float(out16[9]), int(out16[3])
 
-    def size_factors(self, counts, return_logmeans: bool = False):
+    def size_factors(self, counts, return_logmeans: bool = False, logmeans=None):
         """Median-of-ratios size factors on the device (``preprocessing.deseq2_norm``, preprocessing.py:5-102).
 
         Not part of the ``Inference`` ABC -- the reference computes them in the orchestrator (``dds.py:584-711``) --
         but it is the step that precedes the plugin calls.  Returns ``(normed_counts, size_factors)`` like
         ``deseq2_norm``; raises ``ValueError`` when every gene contains a zero (the reference's cue to switch to its
         iterative estimator, ``dds.py:682-690``).
+
+        ``logmeans`` (G,): normalise NEW counts against the log means of an earlier fit instead
+        (``deseq2_norm_transform``, preprocessing.py:59-102, with ``filtered_genes`` = the finite entries; pass -inf for a gene
+        to leave out).  This is how held-out samples are normalised (dds.py:478-486): a zero count in a kept gene counts as a
+        log ratio of -inf, so a sample can get size factor 0 (and infinite / NaN normalised counts), exactly as in numpy; nothing
+        is raised.
         """
         counts, ld = _rows(counts, np.int64, "counts")
         N, G = counts.shape
+        if logmeans is not None:
+            lm = np.ascontiguousarray(_f64(logmeans, "logmeans", 1))
+            if lm.shape[0] != G:
+                raise ValueError(f"logmeans has {lm.shape[0]} entries for {G} genes")
+            sf = np.empty(N)
+            self._ops.size_factors_from_logmeans(counts, ld, N, G, lm, sf)
+            with np.errstate(divide="ignore", invalid="ignore"):
+                return counts / sf[:, None], sf
         sf = np.empty(N)
         logmeans = np.empty(G) if return_logmeans else None  # what deseq2_norm_fit returns (preprocessing.py:31-59)
         try:
@@ -407,6 +432,27 @@ class B200Inference(_InferenceBase):
         if return_logmeans:
             return counts / sf[:, None], sf, logmeans
         return counts / sf[:, None], sf
+
+    def vst_transform(self, counts, size_factors, kind, coeffs):
+        """Variance-stabilised counts (``DeseqDataSet.vst_transform``, dds.py:438-514) from RAW counts and size factors, one
+        elementwise kernel: ``q = counts / size_factors`` (a true division, the reference's ``normed_counts`` bit for bit), then
+        the parametric closed form with ``coeffs = (a0, a1)`` (``uns["vst_trend_coeffs"]``) or, for ``kind="mean"``, the asinh
+        form with ``coeffs = mean_disp`` (dds.py:503-505).  Returns (N, G) float64."""
+        if kind not in VST_KINDS:
+            raise NotImplementedError(f"Found fit_type '{kind}'. Expected 'parametric' or 'mean'.")  # dds.py:511-514
+        counts, ld = _rows(counts, np.int64, "counts")
+        sf = np.ascontiguousarray(_f64(size_factors, "size_factors", 1))
+        N, G = counts.shape
+        if sf.shape[0] != N:
+            raise ValueError(f"size_factors has {sf.shape[0]} entries for {N} samples")
+        c = np.ravel(np.asarray(coeffs, dtype=np.float64))
+        if len(c) != (2 if kind == "parametric" else 1) or not c[0] > 0:
+            raise ValueError(f"vst_transform({kind!r}) needs " + ("(a0 > 0, a1)" if kind == "parametric" else "a mean dispersion > 0")
+                             + f", got {c}")
+        out = self._ops.empty((N, G))
+        if G and N:
+            self._ops.vst_transform(counts, ld, N, G, sf, VST_KINDS[kind], float(c[0]), float(c[1]) if len(c) > 1 else 0.0, out, G)
+        return out
 
     def calculate_cooks(self, counts, size_factors, design_matrix, mu, hat_diagonals, return_matrix=True):
         """Cook's distances on the device (``DeseqDataSet.calculate_cooks``, dds.py:986-1040; SURVEY.md §8 f-1).

@@ -1,5 +1,6 @@
-"""The wiring a PyDESeq2 maintainer adds for the two steps that are NOT behind the ``Inference`` plugin API but have a device
-implementation here (SURVEY.md §8 f-1, f-2): Cook's distances and median-of-ratios size factors.
+"""The wiring a PyDESeq2 maintainer adds for the steps that are NOT behind the ``Inference`` plugin API but have a device
+implementation here (SURVEY.md §8 f-1, f-2): Cook's distances, median-of-ratios size factors and the variance-stabilising
+transform (``vst()`` / ``vst_transform(counts)``).
 
 ``pydeseq2`` is imported lazily -- this module is only usable where the reference package is installed::
 
@@ -18,9 +19,10 @@ import numpy as np
 
 
 def b200_dataset_class():
-    """Returns a ``DeseqDataSet`` subclass whose ``fit_size_factors`` (plain median-of-ratios case) and ``calculate_cooks`` call the
-    backend when it offers ``size_factors`` / ``calculate_cooks`` (``B200Inference`` does), and fall back to the reference's own
-    implementation otherwise (other fit types, control genes, a different backend)."""
+    """Returns a ``DeseqDataSet`` subclass whose ``fit_size_factors`` (plain median-of-ratios case), ``calculate_cooks`` and
+    ``vst_transform`` call the backend when it offers ``size_factors`` / ``calculate_cooks`` / ``vst_transform`` (``B200Inference``
+    does), and fall back to the reference's own implementation otherwise (other fit types, control genes, a missing VST fit,
+    held-out counts after iteratively fitted size factors, a different backend)."""
     from pydeseq2.dds import DeseqDataSet
 
     class B200DeseqDataSet(DeseqDataSet):
@@ -55,5 +57,32 @@ def b200_dataset_class():
             self.layers["cooks"] = np.full((self.n_obs, self.n_vars), np.nan)
             self.layers["cooks"][:, nz] = cooks
             return None
+
+        def vst_transform(self, counts=None):  # dds.py:438-514
+            # The fit (vst_fit) stays the reference's: it already reaches the backend through the plugin calls.  The transform
+            # runs on the device from the raw counts and the size factors: every size-factor path of the reference sets
+            # normed_counts = X / size_factors exactly (dds.py:676-678, 698-703, 1548).
+            inf, kind = self.inference, getattr(self, "vst_fit_type", None)
+            ok = (hasattr(inf, "vst_transform") and kind in ("parametric", "mean") and "size_factors" in self.obs
+                  and isinstance(self.X, np.ndarray) and (kind == "mean" or "vst_trend_coeffs" in self.uns))
+            if ok and counts is not None:  # held-out samples: normalised against the fit's log means on the device
+                ok = (isinstance(counts, np.ndarray) and counts.dtype.kind in "iu" and getattr(self, "logmeans", None) is not None
+                      and getattr(self, "filtered_genes", None) is not None)
+            if ok:
+                if kind == "parametric":
+                    coeffs = np.asarray(self.uns["vst_trend_coeffs"], dtype=float)
+                    ok = coeffs[0] > 0
+                else:
+                    from scipy.stats import trim_mean
+
+                    gd = self.var["vst_genewise_dispersions"]
+                    coeffs = float(trim_mean(gd[gd > 10 * self.min_disp], proportiontocut=0.001))
+                    ok = coeffs > 0
+            if not ok:  # missing fit (the reference's errors), iterative size factors with new counts, other backends
+                return super().vst_transform(counts)
+            if counts is None:
+                return inf.vst_transform(self.X, self.obs["size_factors"].values, kind, coeffs)
+            sf = inf.size_factors(counts, logmeans=np.where(self.filtered_genes, self.logmeans, -np.inf))[1]
+            return inf.vst_transform(counts, sf, kind, coeffs)
 
     return B200DeseqDataSet

@@ -131,6 +131,37 @@ def _expand(v, nz, G_all):
     return out
 
 
+def genewise_stage(counts, X, inference, sf, normed, normed_means, min_mu, min_disp, max_disp, beta_tol, fresh=None, timed=None):
+    """``fit_genewise_dispersions`` (dds.py:713-797) after the size factors: all-zero mask, method-of-moments start values
+    (dds.py:1140-1162), initial mu_hat by ``lin_reg_mu`` or ``irls``, genewise ``alpha_mle``.  ``max_disp`` is the caller's
+    ``max(max_disp, N)``.  Returns ``(non_zero, counts of the non-zero genes, their normalised means, mom, mu_hat,
+    initial-fit converged flags, genewise dispersions (clipped), genewise converged flags)``.  Shared by :func:`fit_host` and
+    ``workflow.vst``."""
+    fresh = fresh if fresh is not None else (lambda a: a)
+    timed = timed if timed is not None else (lambda key, fn, *a, **k: fn(*a, **k))
+    # dds.py:729-731 `~(X == 0).all(0)`.  Counts are non-negative, so a gene is all-zero exactly when the mean of its normalised
+    # counts is 0: with var["_normed_means"] at hand (dds.py:708) the mask costs O(G) instead of a pass over the (N, G) matrix.
+    normed_means = normed.mean(0) if normed_means is None else np.asarray(normed_means)
+    nz = normed_means != 0
+    all_nz = bool(nz.all())
+    c = counts if all_nz else counts[:, nz]              # no copy when the caller already dropped all-zero genes
+    nn = normed if all_nz else normed[:, nz]
+    normed_means = normed_means[nz]
+
+    rde = timed("fit_rough_dispersions", inference.fit_rough_dispersions, nn, X)       # dds.py:1150-1157
+    mde = timed("fit_moments_dispersions", inference.fit_moments_dispersions, nn, sf)
+    mom = np.clip(np.minimum(rde, mde), min_disp, max_disp)
+    if lin_mu_branch(X):                                 # dds.py:747-765
+        mu_hat = timed("lin_reg_mu", inference.lin_reg_mu, fresh(c), sf, X, min_mu)
+        init_conv = np.ones(c.shape[1])
+    else:  # the orchestrator drops this call's `converged` flag (dds.py:757-765); kept here for diagnostics
+        _, mu_hat, _, init_conv = timed("irls_init", inference.irls, fresh(c), sf, X, mom, min_mu, beta_tol)
+    mu_hat = np.ascontiguousarray(mu_hat)                # layers["_mu_hat"][:, non_zero_idx] is a fresh C array
+    gw, gw_conv = timed("alpha_mle_genewise", inference.alpha_mle, fresh(c), X, fresh(mu_hat), mom, min_disp, max_disp)
+    gw = np.clip(gw, min_disp, max_disp)                 # dds.py:792-794
+    return nz, c, normed_means, mom, mu_hat, init_conv, gw, gw_conv
+
+
 def fit_host(counts, X, inference, contrast=None, size_factors=None, min_mu=0.5, min_disp=1e-8, max_disp=10.0,
              beta_tol=1e-8, fit_type="parametric", lfc_null=0.0, alt_hypothesis=None, timings=None, comm=None,
              normed_counts=None, normed_means=None, reuse_lfc_mu=True, fresh_copies=False) -> FitResult:
@@ -177,26 +208,9 @@ def fit_host(counts, X, inference, contrast=None, size_factors=None, min_mu=0.5,
     else:
         sf = np.asarray(size_factors, dtype=float)
         normed = normed_counts if normed_counts is not None else timed("normed_counts", lambda: counts / sf[:, None])
-    # dds.py:729-731 `~(X == 0).all(0)`.  Counts are non-negative, so a gene is all-zero exactly when the mean of its normalised
-    # counts is 0: with var["_normed_means"] at hand (dds.py:708) the mask costs O(G) instead of a pass over the (N, G) matrix.
-    normed_means = normed.mean(0) if normed_means is None else np.asarray(normed_means)
-    nz = normed_means != 0
+    nz, c, normed_means, mom, mu_hat, init_conv, gw, gw_conv = genewise_stage(
+        counts, X, inference, sf, normed, normed_means, min_mu, min_disp, max_disp, beta_tol, fresh, timed)
     all_nz = bool(nz.all())
-    c = counts if all_nz else counts[:, nz]              # no copy when the caller already dropped all-zero genes
-    nn = normed if all_nz else normed[:, nz]
-    normed_means = normed_means[nz]
-
-    rde = timed("fit_rough_dispersions", inference.fit_rough_dispersions, nn, X)       # dds.py:1150-1157
-    mde = timed("fit_moments_dispersions", inference.fit_moments_dispersions, nn, sf)
-    mom = np.clip(np.minimum(rde, mde), min_disp, max_disp)
-    if lin_mu_branch(X):                                 # dds.py:747-765
-        mu_hat = timed("lin_reg_mu", inference.lin_reg_mu, fresh(c), sf, X, min_mu)
-        init_conv = np.ones(c.shape[1])
-    else:  # the orchestrator drops this call's `converged` flag (dds.py:757-765); kept here for diagnostics
-        _, mu_hat, _, init_conv = timed("irls_init", inference.irls, fresh(c), sf, X, mom, min_mu, beta_tol)
-    mu_hat = np.ascontiguousarray(mu_hat)                # layers["_mu_hat"][:, non_zero_idx] is a fresh C array
-    gw, gw_conv = timed("alpha_mle_genewise", inference.alpha_mle, fresh(c), X, fresh(mu_hat), mom, min_disp, max_disp)
-    gw = np.clip(gw, min_disp, max_disp)                 # dds.py:792-794
     # trend + prior are global over ALL genes of ALL shards (dds.py:799-884): with gene shards the two per-gene vectors are
     # all-gathered first (the only exchange on the path)
     if comm is None:
@@ -375,9 +389,26 @@ class ResidentFit:
         """H2D of this shard's counts (genes that are all-zero must already be dropped, dds.py:729-731)."""
         counts = np.ascontiguousarray(counts, dtype=np.int64)
         assert counts.shape[0] == self.N
+        self._place(counts.shape[1], lambda d: self.ctx.h2d(d, counts))
+        self._h_counts = counts  # the outlier refit (refit_subset) replaces counts of a few genes on the host
+
+    def upload_columns_dev(self, d_src, ld_src: int, cols: np.ndarray):
+        """Like :meth:`upload`, from counts already in HBM: columns ``cols`` (caller's gene order) of the device (N, ld_src) int64
+        table ``d_src`` are gathered on the device -- no (N, G) transfer.  The outlier refit (which edits counts on the host) is
+        not available after this."""
+        cols = np.ascontiguousarray(cols, dtype=np.int32)
+        d_idx = self._dev("src_cols", max(len(cols), 1) * 4)
+        self.ctx.h2d(d_idx, cols)
+        c_d = self._lib_mod.c_dptr
+        self._place(len(cols), lambda d: self.ctx.check(self.lib.pdq_gather_columns_dev(
+            self.ctx.h, c_d(d_src), int(ld_src), self.N, c_d(d_idx), len(cols), c_d(d), len(cols))))
+        self._h_counts = None
+
+    def _place(self, G: int, fill):
+        """Buffers for G genes; ``fill(dptr)`` enqueues the (N, G) int64 counts in the caller's gene order into ``dptr``."""
         self._drop_graph()  # buffers may move
         self._eager_key = None
-        self.G = counts.shape[1]
+        self.G = G
         G, N, p = self.G, self.N, self.p
         ng = N * G * 8
         self.d_counts = self._dev("counts", ng)
@@ -414,14 +445,13 @@ class ResidentFit:
         for name, n in (("fitted", G), ("beta0", G * p), ("hint", 2 * G)):
             setattr(self, "d_" + name, self._dev(name, n * 8))
         self.d_nfb = self._dev("nfb", 64)
-        self._h_counts = counts  # the outlier refit (refit_subset) replaces counts of a few genes on the host
         c_d = self._lib_mod.c_dptr
         self._perm = self._inv = None
         self.d_slab_out = self.d_slab
         if self.sort_genes and G >= 256:
             d_raw = self.ctx.malloc(ng)
             try:
-                self.ctx.h2d(d_raw, counts)
+                fill(d_raw)
                 d_sums = self._dev("colsum", G * 8)
                 self.ctx.check(self.lib.pdq_column_sums_dev(self.ctx.h, c_d(d_raw), G, N, G, c_d(d_sums)))
                 sums = np.empty(G)
@@ -441,7 +471,7 @@ class ResidentFit:
             self.d_slab_out = self._dev("slab_out", total * 8)  # the results in the caller's gene order
             self.ctx.h2d(self.d_slab_out, self._h_slab)
         else:
-            self.ctx.h2d(self.d_counts, counts)
+            fill(self.d_counts)
         self.ctx.sync()
         if self.design is None:
             self.device_size_factors()
@@ -498,6 +528,56 @@ class ResidentFit:
             self.design = None
 
     # -- one pass ----------------------------------------------------------------------------------
+    def _enqueue_genewise(self, check, begin):
+        """Steps 1-3 of a pass (``fit_genewise_dispersions``, dds.py:713-797), enqueued without synchronising."""
+        L, h, d, G = self.lib, self.ctx.h, self.design, self.G
+        c_d = self._lib_mod.c_dptr
+        # 1. method-of-moments start values + normalised means (dds.py:1140-1162, :708)
+        begin("mom_dispersions")
+        #    -- and, on the lin_reg_mu branch (dds.py:747-756), the initial mu_hat from the same projection
+        check(L.pdq_mom_dispersions_dev(h, d, c_d(self.d_counts), G, G, self.min_disp, self.max_disp, c_d(self.d_mom),
+                                        c_d(self.d_means), self.min_mu, c_d(self.d_mu_hat) if self.lin_branch else None, G))
+        # 2. initial mu_hat by IRLS otherwise (dds.py:757-765)
+        if not self.lin_branch:
+            begin("irls_init")
+            check(L.pdq_irls_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mom), self.min_mu, self.beta_tol, -30.0, 30.0,
+                                 250, c_d(self.d_beta0), c_d(self.d_mu_hat), c_d(self.d_hat), G, c_d(self.d_conv),
+                                 c_d(self.d_nfb)))
+        # 3. genewise dispersions (dds.py:778-797)
+        begin("alpha_mle_genewise")
+        #    (its optimum and curvature per gene are kept on the device: the MAP search of step 5 opens from them)
+        check(L.pdq_alpha_mle_hint_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu_hat), G, c_d(self.d_mom), self.min_disp,
+                                       self.max_disp, 1.0, None, 1, 0, c_d(self.d_gw), c_d(self.d_gw_conv), None,
+                                       c_d(self.d_hint) if self.use_hint else None))
+
+    def vst_dispersions(self, fit_type="parametric"):
+        """The fit stage of ``vst_fit`` (dds.py:384-436) on the resident counts: steps 1-3 of :meth:`run` and the dispersion
+        trend (dds.py:1199-1299), then stop.  Returns ``(kind, coeffs, genewise)``: the final kind (``"mean"`` also after a
+        parametric trend that did not converge, with the reference's warning), ``(a0, a1)`` or ``(mean_disp,)``, and the clipped
+        genewise dispersions in the uploaded gene order.  Only per-gene vectors come back; :meth:`run`'s graph is left alone."""
+        ctx, c_d = self.ctx, self._lib_mod.c_dptr
+        self._enqueue_genewise(ctx.check, lambda name: None)
+        if fit_type == "parametric":
+            ctx.check(self.lib.pdq_trend_fit_dev(ctx.h, c_d(self.d_means), c_d(self.d_gw), self.G, self.min_disp, self.max_disp,
+                                                 float(polygamma(1, (self.N - self.p) / 2)), c_d(self.d_t16), None))
+        gw = ctx.pinned_empty((self.G,))
+        ctx.d2h(gw, self.d_gw)
+        t16 = ctx.pinned_empty((16,))
+        ctx.d2h(t16, self.d_t16)
+        ctx.sync()
+        gw = np.clip(gw, self.min_disp, self.max_disp)
+        if self._perm is not None:  # device column j holds the caller's gene perm[j]
+            out = np.empty_like(gw)
+            out[self._perm] = gw
+            gw = out
+        if fit_type == "parametric" and t16[2] == 0.0:
+            return "parametric", np.array([t16[0], t16[1]]), gw
+        if fit_type == "parametric":
+            warnings.warn("The dispersion trend curve fitting did not converge. Switching to a mean-based dispersion trend.",
+                          UserWarning, stacklevel=2)
+        sel = gw > 10 * self.min_disp
+        return "mean", np.array([float(trim_mean(gw[sel], proportiontocut=0.001))]), gw
+
     def run(self, contrast=None, lfc_null=0.0, alt_hypothesis=None, fit_type="parametric", profile=False, copy=True, events=None):
         """One pass of the hot path.  Every stage is enqueued on the context's stream back to back -- the trend and
         the dispersion prior run on the device too -- so the host synchronises exactly once, at the end.
@@ -564,23 +644,7 @@ class ResidentFit:
         d_fitted = d_fit_all + rank * m * 8  # this shard's slice of the fitted curve
 
         def enqueue():
-            # 1. method-of-moments start values + normalised means (dds.py:1140-1162, :708)
-            begin("mom_dispersions")
-            #    -- and, on the lin_reg_mu branch (dds.py:747-756), the initial mu_hat from the same projection
-            check(L.pdq_mom_dispersions_dev(h, d, c_d(self.d_counts), G, G, self.min_disp, self.max_disp, c_d(self.d_mom),
-                                            c_d(self.d_means), self.min_mu, c_d(self.d_mu_hat) if self.lin_branch else None, G))
-            # 2. initial mu_hat by IRLS otherwise (dds.py:757-765)
-            if not self.lin_branch:
-                begin("irls_init")
-                check(L.pdq_irls_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mom), self.min_mu, self.beta_tol, -30.0, 30.0,
-                                     250, c_d(self.d_beta0), c_d(self.d_mu_hat), c_d(self.d_hat), G, c_d(self.d_conv),
-                                     c_d(self.d_nfb)))
-            # 3. genewise dispersions (dds.py:778-797)
-            begin("alpha_mle_genewise")
-            #    (its optimum and curvature per gene are kept on the device: the MAP search of step 5 opens from them)
-            check(L.pdq_alpha_mle_hint_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu_hat), G, c_d(self.d_mom), self.min_disp,
-                                           self.max_disp, 1.0, None, 1, 0, c_d(self.d_gw), c_d(self.d_gw_conv), None,
-                                           c_d(self.d_hint) if self.use_hint else None))
+            self._enqueue_genewise(check, begin)  # steps 1-3
             # 4. trend + prior: global over ALL genes of ALL shards (dds.py:799-884).  With gene shards the per-gene
             #    vectors are exchanged first, device to device (peer-memory push kernel or grouped NCCL all-gathers); the fit itself
             #    is one launch (a thread-block cluster, or a cooperative grid from 65 536 genes).

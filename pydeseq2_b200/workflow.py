@@ -18,9 +18,12 @@ from __future__ import annotations
 from dataclasses import dataclass, field
 from math import ceil, floor
 
-import numpy as np
+import warnings
 
-from .pipeline import LN2, FitResult, fit_host, fit_shrink_prior_var, lin_mu_branch
+import numpy as np
+from scipy.stats import trim_mean
+
+from .pipeline import LN2, FitResult, fit_host, fit_shrink_prior_var, fit_trend, genewise_stage, lin_mu_branch, median_of_ratios
 
 
 def n_or_more_replicates(X: np.ndarray, min_replicates: int) -> np.ndarray:
@@ -350,6 +353,155 @@ def _full(v, nz, G):
     out = np.full(G, np.nan)
     out[nz] = v
     return out
+
+
+# --------------------------------------------------------------------------------------- variance-stabilising transform
+_LEAK_WARNING = ("The size factors were fitted iteratively. They will be re-computed with the counts to be transformed. In a "
+                 "train/test setting with a downstream task, this would result in a leak of data from test to train set.")
+
+
+@dataclass
+class VstFit:
+    """What ``DeseqDataSet.vst_fit()`` leaves behind (dds.py:384-436) plus ``layers["vst_counts"]``.
+
+    ``kind`` is the final ``vst_fit_type``: ``"mean"`` also after a parametric trend that failed to converge.  ``coeffs`` is
+    ``(a0, a1)`` (``uns["vst_trend_coeffs"]``) or ``(mean_disp,)`` (dds.py:503-505).  ``genewise`` has one entry per gene, NaN for
+    all-zero genes (``var["vst_genewise_dispersions"]``); ``vst_counts`` covers every gene, all-zero genes included.
+    ``logmeans`` / ``filtered_genes`` are ``deseq2_norm_fit``'s (preprocessing.py:31-56), None when the size factors were
+    passed in without log means."""
+    size_factors: np.ndarray
+    logmeans: np.ndarray | None
+    filtered_genes: np.ndarray | None
+    kind: str
+    coeffs: np.ndarray
+    genewise: np.ndarray
+    non_zero: np.ndarray
+    vst_counts: np.ndarray | None = None
+    inference: object = field(repr=False, default=None)
+
+    def transform(self, counts) -> np.ndarray:
+        """``vst_transform(counts)`` on NEW samples (dds.py:464-514): their size factors are medians of ratios against the fit's
+        log means (``deseq2_norm_transform``); without log means they are re-fitted on ``counts`` with the reference's warning."""
+        counts = np.ascontiguousarray(counts, dtype=np.int64)
+        if self.logmeans is None:
+            warnings.warn(_LEAK_WARNING, UserWarning, stacklevel=2)
+            sf = _median_of_ratios(counts, self.inference)[1]
+        else:
+            lm = np.where(self.filtered_genes, self.logmeans, -np.inf)
+            sf = self.inference.size_factors(counts, logmeans=lm)[1]
+        return self.inference.vst_transform(counts, sf, self.kind, self.coeffs)
+
+
+def _median_of_ratios(counts, inference):
+    """(normed counts, size factors, log means): on the backend when it has ``size_factors``, else numpy (preprocessing.py:31-102)."""
+    if hasattr(inference, "size_factors"):
+        return inference.size_factors(counts, return_logmeans=True)
+    normed, sf = median_of_ratios(counts)
+    with np.errstate(divide="ignore"):
+        return normed, sf, np.log(counts).mean(0)
+
+
+def mean_dispersion(genewise: np.ndarray, min_disp: float) -> float:
+    """Dispersion of the ``"mean"`` transform: trimmed mean of the genewise dispersions above 10 * min_disp (dds.py:503-505)."""
+    g = np.asarray(genewise, dtype=float)
+    return float(trim_mean(g[g > 10 * min_disp], proportiontocut=0.001))
+
+
+def vst(counts, X, inference, fit_type="parametric", use_design=False, size_factors=None, logmeans=None, min_mu=0.5, min_disp=1e-8,
+        max_disp=10.0, beta_tol=1e-8, transform=True) -> VstFit:
+    """``DeseqDataSet.vst(use_design, fit_type)`` (dds.py:349-436) on bare arrays: median-of-ratios size factors unless
+    ``size_factors`` are given (``logmeans`` then are the fit's, for :meth:`VstFit.transform`), genewise dispersions on an
+    intercept-only design unless ``use_design`` (dds.py:713-797), the parametric trend loop with its fallback to the trimmed mean
+    (dds.py:1199-1299), and the transform of every gene through ``inference.vst_transform``.  ``counts`` (N, G) non-negative
+    integers, ``X`` (N, p) the expanded design."""
+    if fit_type not in ("parametric", "mean"):
+        raise NotImplementedError(f"Found fit_type '{fit_type}'. Expected 'parametric' or 'mean'.")
+    if not hasattr(inference, "vst_transform"):
+        raise TypeError(f"{type(inference).__name__} has no vst_transform")
+    counts = np.ascontiguousarray(counts, dtype=np.int64)
+    N, G = counts.shape
+    max_disp = max(max_disp, N)  # dds.py:312
+    if size_factors is None:
+        normed, sf, logmeans = _median_of_ratios(counts, inference)
+    else:
+        sf = np.asarray(size_factors, dtype=float)
+        normed = counts / sf[:, None]
+    filtered = None if logmeans is None else ~np.isinf(logmeans)
+    if use_design:
+        Xv = np.ascontiguousarray(X, dtype=np.float64)
+        if fit_type == "mean":
+            warnings.warn("use_design=True is only useful when fit_type='parametric'. ", UserWarning, stacklevel=2)
+    else:
+        Xv = np.ones((N, 1))
+    nz, _, means, _, _, _, gw, _ = genewise_stage(counts, Xv, inference, sf, normed, None, min_mu, min_disp, max_disp, beta_tol)
+    kind = fit_type
+    if fit_type == "parametric":
+        trend = fit_trend(inference, means, gw, min_disp, "parametric")  # warns and returns the mean trend when the fit fails
+        kind = trend.kind
+    coeffs = np.asarray(trend.coeffs, dtype=float) if kind == "parametric" else np.array([mean_dispersion(gw, min_disp)])
+    fit = VstFit(sf, logmeans, filtered, kind, coeffs, _full(gw, nz, G), nz, None, inference)
+    if transform:
+        fit.vst_counts = inference.vst_transform(counts, sf, kind, coeffs)
+    return fit
+
+
+def vst_resident(inference, counts, X, fit_type="parametric", use_design=False, size_factors=None, logmeans=None, min_mu=0.5,
+                 min_disp=1e-8, max_disp=10.0, beta_tol=1e-8) -> VstFit:
+    """:func:`vst` with the counts resident in HBM: they go up once, the size factors (median of ratios on the device unless
+    given), the all-zero mask and the fit stage (steps 1-3 of ``ResidentFit.run`` and the trend, on a ``ResidentFit`` of the VST
+    design over the non-zero genes, gathered on the device) run there, and ``pdq_vst_transform_dev`` transforms the full table
+    in the caller's gene order; only ``vst_counts`` comes back.  Every other transfer is a per-sample or per-gene vector.
+    ``inference`` is a ``B200Inference`` (its context is used)."""
+    from . import _lib
+    from .inference import VST_KINDS
+    from .pipeline import ResidentFit
+
+    if fit_type not in ("parametric", "mean"):
+        raise NotImplementedError(f"Found fit_type '{fit_type}'. Expected 'parametric' or 'mean'.")
+    ctx = inference._ops.ctx
+    L, h, c_d = ctx.lib, ctx.h, _lib.c_dptr
+    counts = np.ascontiguousarray(counts, dtype=np.int64)
+    N, G = counts.shape
+    d_counts, d_sf, d_lm, d_sums, d_out = (ctx.malloc(n) for n in (N * G * 8, N * 8, G * 8, G * 8, N * G * 8))
+    rf = None
+    try:
+        ctx.h2d(d_counts, counts)  # the one (N, G) upload
+        if size_factors is None:
+            ctx.check(L.pdq_size_factors_dev(h, c_d(d_counts), G, N, G, c_d(d_sf), c_d(d_lm)))
+            sf, logmeans = np.empty(N), np.empty(G)
+            ctx.d2h(sf, d_sf)
+            ctx.d2h(logmeans, d_lm)
+        else:
+            sf = np.ascontiguousarray(size_factors, dtype=np.float64)
+            ctx.h2d(d_sf, sf)
+        ctx.check(L.pdq_column_sums_dev(h, c_d(d_counts), G, N, G, c_d(d_sums)))
+        sums = np.empty(G)
+        ctx.d2h(sums, d_sums)
+        ctx.sync()
+        if not np.isfinite(sf).all():
+            raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
+        nz = sums != 0  # counts are non-negative (dds.py:729-731)
+        if use_design:
+            Xv = np.ascontiguousarray(X, dtype=np.float64)
+            if fit_type == "mean":
+                warnings.warn("use_design=True is only useful when fit_type='parametric'. ", UserWarning, stacklevel=2)
+        else:
+            Xv = np.ones((N, 1))
+        rf = ResidentFit(ctx, Xv, sf, min_mu=min_mu, min_disp=min_disp, max_disp=max_disp, beta_tol=beta_tol)
+        rf.upload_columns_dev(d_counts, G, np.flatnonzero(nz))
+        kind, coeffs, gw = rf.vst_dispersions(fit_type)
+        ctx.check(L.pdq_vst_transform_dev(h, c_d(d_counts), G, N, G, c_d(d_sf), VST_KINDS[kind], float(coeffs[0]),
+                                          float(coeffs[1]) if len(coeffs) > 1 else 0.0, c_d(d_out), G))
+        out = ctx.pinned_empty((N, G))
+        ctx.d2h(out, d_out)  # the one (N, G) download
+        ctx.sync()
+    finally:
+        if rf is not None:
+            rf.close()
+        for p in (d_counts, d_sf, d_lm, d_sums, d_out):
+            ctx.free(p)
+    filtered = None if logmeans is None else ~np.isinf(logmeans)
+    return VstFit(sf, logmeans, filtered, kind, coeffs, _full(gw, nz, G), nz, out, inference)
 
 
 def _refit_subset(sub, X, sf, inference, fit: FitResult, min_mu, min_disp, max_disp, beta_tol):
