@@ -93,6 +93,9 @@ struct Group {
         return 0;
 #endif
     }
+    // on the device a vote over the whole WARP (every gene of it), not just this group: a superset of the group's vote, so
+    // the branches and loop exits it guards stay warp-uniform, as the full-mask shuffles inside them require (each gene masks
+    // the extra work with its own flags).  The emulator runs one gene at a time and votes over its lanes.
     PDQ_HD bool any(bool p) const {
 #if defined(__CUDA_ARCH__)
         return __any_sync(0xffffffffu, p) != 0;
@@ -202,6 +205,10 @@ PDQ_UNROLL_P
 // f(r) by the recurrence (one log / reciprocal per entry, split over the gene's lanes and stitched with an exclusive
 // scan); counts below kPsiK then cost one shared-memory read, and larger counts always satisfy the z >= 10
 // precondition of the unshifted Stirling series.
+// Accuracy (tests/test_gpu_math.py on an H100, tests/test_math_ref.py on the host; r in [1e-4, 1e8], every T in 1..32): each
+// entry is within 0.07 (lgamma), 0.03 (psi) and 0.14 (psi') of the forward-error bound of its recurrence, start error +
+// 4 eps (k + 1) (|f(r)| + sum_{j<k} |term_j|).  The largest absolute error, 3e-8 in psi' at r = 1e-4, is that conditioning:
+// psi'(1e-4) ~ 1e8.
 // ---------------------------------------------------------------------------------------------
 constexpr int kPsiK = 32;
 

@@ -178,6 +178,10 @@ PDQ_UNROLL_P
 // uses the product P(x) = x (x+1) ... (x+9) and its derivative so that only ONE log and ONE
 // division are spent on it:  lgamma(x) = lgamma(x+10) - log P(x),  psi(x) = psi(x+10) - P'(x)/P(x).
 // Truncation error < 2e-16 absolute at z = 10 for both series (next omitted terms: 4.4e-17 / 1.2e-17).
+// Worst error against mpmath over x in [1e-4, 1e9] (both sides of 10, the roots, integers), relative to max(|f|, 1), on the
+// device (H100, tests/test_gpu_math.py) and the host (tests/test_math_ref.py) alike: lgamma_pos 6.9e-15, digamma_pos 1.4e-15,
+// trigamma_pos 4.7e-16 (relative), lgamma_digamma_pos 6.4e-15 / 1.4e-15.  Asserted: |err| <= 3e-14 + 2e-14 |f| for lgamma /
+// digamma, <= 4e-15 |f| for trigamma.
 // ---------------------------------------------------------------------------------------------
 PDQ_HD void shift10(double x, double& P, double& dP) {
     P = x;

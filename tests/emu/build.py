@@ -6,7 +6,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "_build", "libpdq_emu.so")
 SRC = os.path.join(HERE, "pdq_emu.cpp")
 DEPS = [SRC] + [os.path.join(HERE, "..", "..", "pydeseq2_b200", "csrc", f)
-                for f in ("pdq_gene.cuh", "pdq_math.cuh", "pdq_host_linalg.h", "pdq_trend.cuh", "pdq_fast.cuh", "pdq_shrink.cuh")]
+                for f in ("pdq_gene.cuh", "pdq_math.cuh", "pdq_host_linalg.h", "pdq_trend.cuh", "pdq_fast.cuh", "pdq_shrink.cuh",
+                          "pdq_tables.h")] + [os.path.join(HERE, "..", "gpu_probe", "math_ops.h")]
 
 
 def build(force=False, defines=None):

@@ -115,6 +115,28 @@ class EmuOps:
             with np.errstate(divide="ignore"):
                 logmeans[:] = np.log(np.asarray(counts)[:, :G]).mean(0)
 
+    def elem(self, op, x, y=None):
+        """The host branch of one primitive (op code of tests/gpu_probe/math_ops.h) applied elementwise."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        y = np.zeros_like(x) if y is None else np.ascontiguousarray(np.broadcast_to(y, x.shape), dtype=np.float64)
+        out = np.empty_like(x)
+        assert self.lib.emu_math(int(op), _p(x, f64p), _p(y, f64p), _p(out, f64p), int(x.size)) == 0
+        return out
+
+    def tables(self, r, T):
+        """[G][4 kPsiK]: lgamma, psi, then psi and psi' of build_psi_tri_tables at each r, built by T lane threads."""
+        r = np.ascontiguousarray(r, dtype=np.float64)
+        out = np.empty((r.size, 4 * 32))
+        assert self.lib.emu_tables(_p(r, f64p), int(r.size), int(T), _p(out, f64p)) == 0
+        return out
+
+    def math_table(self):
+        """(kMathTab as compiled into the emulator, {bits, n, split, exp_n})"""
+        tab = np.empty(4096)
+        layout = np.zeros(4, dtype=np.int32)
+        n = self.lib.emu_math_table(_p(tab, f64p), _p(layout, i32p))
+        return tab[:n].copy(), dict(zip(("bits", "n", "split", "exp_n"), (int(v) for v in layout)))
+
     def cooks(self, counts, ld, N, G, sf, X, p, mu, hat, ld2, cutoff, cooks, disp, outlier, replaced):
         assert self.lib.emu_cooks(_p(counts, i64p), C.c_int64(ld), N, G, _p(sf, f64p), _p(X, f64p), p, _p(mu, f64p), _p(hat, f64p),
                                   C.c_int64(ld2), C.c_double(cutoff), _p(cooks, f64p) if cooks is not None else None,

@@ -26,6 +26,7 @@ extern long g_emu_irls_sweeps;
 #include "../../pydeseq2_b200/csrc/pdq_host_linalg.h"
 #include "../../pydeseq2_b200/csrc/pdq_trend.cuh"
 #include "../../pydeseq2_b200/csrc/pdq_shrink.cuh"
+#include "../gpu_probe/math_ops.h"
 
 long g_emu_alpha_evals = 0;
 long g_emu_irls_sweeps = 0;
@@ -434,6 +435,34 @@ double emu_fast_log(double x) { return fast_log(x); }
 double emu_fast_exp(double x) { return fast_exp(x); }
 double emu_lgamma(double x) { return lgamma_pos(x); }
 double emu_digamma(double x) { return digamma_pos(x); }
+// the host branches of every primitive, with the GPU probe's op codes (tests/gpu_probe/math_ops.h)
+int emu_math(int op, const double* x, const double* y, double* out, int n) {
+    if (op < 0 || op >= pdq_probe::kNumOps) return -1;
+    for (int i = 0; i < n; ++i) out[i] = pdq_probe::apply(op, x[i], y[i], host_math_table());
+    return 0;
+}
+// the per-gene tables of G genes, each built by T lanes (threads) with the device's exchange patterns: [G][4 kPsiK]
+int emu_tables(const double* r, int G, int T, double* out) {
+    const int saved = g_lanes;
+    if (emu_set_lanes(T) != 0) return -1;
+    for (int g = 0; g < G; ++g) {
+        double tab[pdq_probe::kTabOut];
+        with_lanes([&](const Group& grp) { pdq_probe::build_tables(grp, tab, r[g], host_math_table()); });
+        memcpy(out + (size_t)g * pdq_probe::kTabOut, tab, sizeof tab);
+    }
+    g_lanes = saved;
+    return 0;
+}
+// kMathTab as the emulator (and the device, from the same initialiser) sees it; layout[] = {kLogTabBits, kLogTabN, kLogTabSplit,
+// kExpTabN}; returns kMathTabLen
+int emu_math_table(double* out, int* layout) {
+    memcpy(out, host_math_table(), sizeof(double) * kMathTabLen);
+    layout[0] = kLogTabBits;
+    layout[1] = kLogTabN;
+    layout[2] = kLogTabSplit;
+    layout[3] = kExpTabN;
+    return kMathTabLen;
+}
 int emu_design_rank_pinv(const double* X, int N, int p, double* pinv) {
     int fr;
     design_linear_algebra(X, N, p, pinv, &fr);
