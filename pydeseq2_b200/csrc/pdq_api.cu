@@ -284,7 +284,7 @@ extern "C" int pdq_ctx_create(int device, pdq_ctx** out) {
     c->res_cap = c->prop.totalGlobalMem / 4;
     if (c->res_cap > ((size_t)16 << 30)) c->res_cap = (size_t)16 << 30;
     if (const char* s = getenv("PDQ_RESIDENCY_BYTES")) c->res_cap = (size_t)atoll(s);
-    if (cudaMalloc((void**)&c->tickets, 64) != cudaSuccess || cudaMalloc(&c->grid_scratch, 4096) != cudaSuccess || cudaStreamCreateWithFlags(&c->pstream[0], cudaStreamNonBlocking) != cudaSuccess ||
+    if (cudaMalloc((void**)&c->tickets, 64) != cudaSuccess || cudaMalloc(&c->grid_scratch, kGridScratchBytes) != cudaSuccess || cudaStreamCreateWithFlags(&c->pstream[0], cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&c->pstream[1], cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->pfork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->pjoin[0], cudaEventDisableTiming) != cudaSuccess ||

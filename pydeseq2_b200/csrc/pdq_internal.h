@@ -24,13 +24,15 @@ struct DesignDev {
     int n_cells, n_in_cells, plan_len;
 };
 
+constexpr size_t kGridScratchBytes = 32768;  // LaunchCfg::grid_scratch (accumulators and value bins of k_trend_prior_grid)
+
 struct LaunchCfg {
     cudaStream_t stream;
     int lgT;       // log2(lanes per gene)
     int sm_count;
     int* tickets;  // device ints: tile counters of the persistent kernels
     int debug;     // PDQ_DEBUG_* test hooks
-    void* grid_scratch = nullptr;  // device scratch of the grid-wide trend fit (launch_trend_fit), 4 KB
+    void* grid_scratch = nullptr;  // device scratch of the grid-wide trend fit (launch_trend_fit), kGridScratchBytes
 };
 
 struct IrlsHost {

@@ -499,6 +499,8 @@ struct ClusterReducer {
     double* totals;     // [2][kTrendK]: the cluster-wide sums, broadcast to the block's threads
     unsigned rank, nblocks;
     int parity;
+    unsigned* vmerged = nullptr;              // [2][kVBins] (median_bins only)
+    unsigned* sel_words = nullptr;            // [2]: candidate cursors (median_bins only)
     __host__ __device__ int tid() const {
 #if defined(__CUDA_ARCH__)
         return rank * blockDim.x + threadIdx.x;
@@ -530,11 +532,6 @@ struct ClusterReducer {
     __host__ __device__ void local_sync() {
 #if defined(__CUDA_ARCH__)
         __syncthreads();
-#endif
-    }
-    __host__ __device__ void sync() {
-#if defined(__CUDA_ARCH__)
-        cooperative_groups::this_cluster().sync();
 #endif
     }
     // cluster-wide maximum of one value per thread (same exchange pattern as sum_many)
@@ -627,19 +624,25 @@ struct ClusterReducer {
         (void)hist; (void)out; (void)k; (void)d; (void)cum;
 #endif
     }
-    __host__ __device__ void sum_many(double* v, int k) {
+    // the last `kmax` of the k values are maxima, not sums (same exchange)
+    __host__ __device__ void sum_many(double* v, int k, int kmax = 0) {
 #if defined(__CUDA_ARCH__)
         namespace cg = cooperative_groups;
         cg::cluster_group cluster = cg::this_cluster();
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, ks = k - kmax;
         for (int j = 0; j < k; ++j) {
             double w = v[j];
+            if (j < ks) {
 #pragma unroll
-            for (int off = 16; off > 0; off >>= 1) w += __shfl_xor_sync(0xffffffffu, w, off);
+                for (int off = 16; off > 0; off >>= 1) w += __shfl_xor_sync(0xffffffffu, w, off);
+            } else {
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) w = fmax(w, __shfl_xor_sync(0xffffffffu, w, off));
+            }
             if (lane == 0) warp_part[warp * kTrendK + j] = w;
         }
         __syncthreads();
-        if ((int)threadIdx.x < k) {
+        if ((int)threadIdx.x < ks) {
             double tot = 0.0;
             const int nw = blockDim.x >> 5;
             for (int w = 0; w < nw; ++w) tot += warp_part[w * kTrendK + threadIdx.x];
@@ -652,13 +655,28 @@ struct ClusterReducer {
                 slots[parity * kTrendMaxCluster * kTrendK + threadIdx.x] = tot;
             }
         }
+        if ((int)threadIdx.x >= ks && (int)threadIdx.x < k) {
+            double m = warp_part[threadIdx.x];
+            const int nw = blockDim.x >> 5;
+            for (int w = 1; w < nw; ++w) m = fmax(m, warp_part[w * kTrendK + threadIdx.x]);
+            if (nblocks > 1) {
+                for (unsigned r = 0; r < nblocks; ++r)
+                    cluster.map_shared_rank(slots, r)[(parity * kTrendMaxCluster + rank) * kTrendK + threadIdx.x] = m;
+            } else {
+                slots[parity * kTrendMaxCluster * kTrendK + threadIdx.x] = m;
+            }
+        }
         if (nblocks > 1) cluster.sync(); else __syncthreads();  // release the DSMEM stores / acquire the peers'
         // k threads add up the blocks' slots, everybody reads the k totals (broadcast reads).  Having EVERY thread
         // add nblocks * k slots itself would cost 160 shared-memory reads per thread and pass.
-        if ((int)threadIdx.x < k) {
+        if ((int)threadIdx.x < ks) {
             double tot = 0.0;
             for (unsigned r = 0; r < nblocks; ++r) tot += slots[(parity * kTrendMaxCluster + r) * kTrendK + threadIdx.x];
             totals[parity * kTrendK + threadIdx.x] = tot;
+        } else if ((int)threadIdx.x < k) {
+            double m = slots[parity * kTrendMaxCluster * kTrendK + threadIdx.x];
+            for (unsigned r = 1; r < nblocks; ++r) m = fmax(m, slots[(parity * kTrendMaxCluster + r) * kTrendK + threadIdx.x]);
+            totals[parity * kTrendK + threadIdx.x] = m;
         }
         __syncthreads();
         for (int j = 0; j < k; ++j) v[j] = totals[parity * kTrendK + j];
@@ -666,8 +684,70 @@ struct ClusterReducer {
 #else
         (void)v;
         (void)k;
+        (void)kmax;
 #endif
     }
+#if defined(__CUDA_ARCH__)
+    // median_bins hooks.  Bin j of the merged histogram lives in block j / (kVBins / nblocks) of the cluster (vmerged[slot]):
+    // every block adds its non-zero bins there with DSMEM atomics, meets the others at one cluster barrier and reads the totals
+    // back.  The candidate cursor lives in block 0 (sel_words[slot]).  Both are zeroed at the start of the kernel, and each slot
+    // serves one selection per launch.
+    __device__ void vhist_merge(unsigned* hist, int slot) {
+        __syncthreads();  // local bins complete
+        if (nblocks == 1) return;
+        namespace cg = cooperative_groups;
+        cg::cluster_group cluster = cg::this_cluster();
+        const unsigned chunk = kVBins / nblocks;
+        unsigned* merged = vmerged + slot * kVBins;
+        for (unsigned j = threadIdx.x; j < (unsigned)kVBins; j += blockDim.x) {
+            const unsigned c = hist[j];
+            if (c) atomicAdd(cluster.map_shared_rank(merged, j / chunk) + j, c);
+        }
+        cluster.sync();
+        for (unsigned j = threadIdx.x; j < (unsigned)kVBins; j += blockDim.x) hist[j] = cluster.map_shared_rank(merged, j / chunk)[j];
+        __syncthreads();
+    }
+    __device__ unsigned cand_index(int slot) {
+        return atomicAdd(cooperative_groups::this_cluster().map_shared_rank(sel_words + slot, 0), 1u);
+    }
+    // cluster-wide maximum of one 64-bit key per thread, as integers, through the slot exchange of max_one (the bits ride in
+    // the double slots untouched).  Not a DSMEM atomicMax: a 64-bit max on shared memory has no native instruction, and the
+    // compiler's fallback for a generic address (QSPC + an ATOMS compare-and-swap loop) does not reach a peer block's memory
+    __device__ unsigned long long max_key(unsigned long long v) {
+        namespace cg = cooperative_groups;
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            const unsigned long long o = __shfl_xor_sync(0xffffffffu, v, off);
+            v = o > v ? o : v;
+        }
+        if (lane == 0) warp_part[warp * kTrendK] = __longlong_as_double((long long)v);
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned long long m = 0ull;
+            const int nw = blockDim.x >> 5;
+            for (int w = 0; w < nw; ++w) {
+                const unsigned long long o = (unsigned long long)__double_as_longlong(warp_part[w * kTrendK]);
+                m = o > m ? o : m;
+            }
+            const double mb = __longlong_as_double((long long)m);
+            if (nblocks > 1) {
+                cg::cluster_group cluster = cg::this_cluster();
+                for (unsigned r = 0; r < nblocks; ++r) cluster.map_shared_rank(slots, r)[(parity * kTrendMaxCluster + rank) * kTrendK] = mb;
+            } else {
+                slots[parity * kTrendMaxCluster * kTrendK] = mb;
+            }
+        }
+        if (nblocks > 1) cg::this_cluster().sync(); else __syncthreads();
+        unsigned long long m = 0ull;
+        for (unsigned r = 0; r < nblocks; ++r) {
+            const unsigned long long o = (unsigned long long)__double_as_longlong(slots[(parity * kTrendMaxCluster + r) * kTrendK]);
+            m = o > m ? o : m;
+        }
+        parity ^= 1;
+        return m;
+    }
+#endif
 };
 
 __global__ void __launch_bounds__(1024) k_trend_prior(const double* __restrict__ x, const double* __restrict__ t,
@@ -678,13 +758,22 @@ __global__ void __launch_bounds__(1024) k_trend_prior(const double* __restrict__
     __shared__ double slots[2 * kTrendMaxCluster * kTrendK];
     __shared__ double totals[2 * kTrendK];
     __shared__ unsigned hist[514];
+    __shared__ SelShared sel;
+    __shared__ unsigned vmerged[2 * kVBins];
+    __shared__ unsigned sel_words[2];
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
-    ClusterReducer red{warp_part, slots, totals, cluster.block_rank(), cluster.num_blocks(), 0};
+    ClusterReducer red{warp_part, slots, totals, cluster.block_rank(), cluster.num_blocks(), 0, vmerged, sel_words};
+    for (int j = threadIdx.x; j < 2 * kVBins; j += blockDim.x) vmerged[j] = 0;  // first used behind the fit's cluster barriers
+    if (threadIdx.x < 2) sel_words[threadIdx.x] = 0;
     double *xs = scratch, *ts = scratch + n, *res = scratch + 2 * n;
     trend_prepare(red, x, t, n, x_is_mean != 0, lo, hi, xs, ts);
-    TrendOut o = trend_fit_outer(red, xs, ts, n, outer != 0);
-    if (with_prior && o.status == 0.0) trend_prior(red, x, t, n, lo, hi, min_disp, trigamma_c, res, hist, o);
+    TrendOut o = trend_fit_outer(red, xs, ts, n, outer != 0, false);
+    // the prior's candidate buffer reuses xs, last read by the fit before the prior's first cluster barrier
+    if (with_prior && o.status == 0.0)
+        trend_prior_dev(red, x, t, n, lo, hi, min_disp, trigamma_c, res, reinterpret_cast<unsigned long long*>(xs), sel, hist, o);
+    else
+        red.sum_many(&o.n_used, 1);
     if (red.tid() == 0) *out = o;
     cluster.sync();  // no block may exit while peers can still address its shared memory
 }
@@ -696,9 +785,12 @@ __global__ void __launch_bounds__(1024) k_trend_prior(const double* __restrict__
 // (p + 2) % 3, last read in pass p - 1 and next used in pass p + 1.
 struct GridScratch {
     double acc[3][kTrendK];
-    unsigned long long maxkey[3];
+    unsigned long long maxkey[3][2];
     unsigned hist[3][256];
+    unsigned vhist[2][kVBins];        // median_bins: merged value bins and candidate cursors, one slot per selection of the launch
+    unsigned cursor[2];
 };
+static_assert(sizeof(GridScratch) <= kGridScratchBytes, "GridScratch outgrew the context's allocation");
 
 struct GridReducer {
     double* warp_part;  // [32][kTrendK] shared
@@ -710,38 +802,79 @@ struct GridReducer {
     __device__ int local_tid() const { return threadIdx.x; }
     __device__ int local_nthreads() const { return blockDim.x; }
     __device__ void local_sync() { __syncthreads(); }
-    __device__ void sync() { cooperative_groups::this_grid().sync(); }
-    __device__ void sum_many(double* v, int k) {
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, slot = p_sum % 3;
+    // the last `kmax` (<= 2) of the k values are maxima, not sums: they go through the maxkey slots as order-preserving keys
+    __device__ void sum_many(double* v, int k, int kmax = 0) {
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, slot = p_sum % 3, mslot = p_max % 3, ks = k - kmax;
         for (int j = 0; j < k; ++j) {
             double w = v[j];
+            if (j < ks) {
 #pragma unroll
-            for (int off = 16; off > 0; off >>= 1) w += __shfl_xor_sync(0xffffffffu, w, off);
+                for (int off = 16; off > 0; off >>= 1) w += __shfl_xor_sync(0xffffffffu, w, off);
+            } else {
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) w = fmax(w, __shfl_xor_sync(0xffffffffu, w, off));
+            }
             if (lane == 0) warp_part[warp * kTrendK + j] = w;
         }
         __syncthreads();
-        if ((int)threadIdx.x < k) {
+        if ((int)threadIdx.x < ks) {
             double tot = 0.0;
             const int nw = blockDim.x >> 5;
             for (int w = 0; w < nw; ++w) tot += warp_part[w * kTrendK + threadIdx.x];
             atomicAdd(&gs->acc[slot][threadIdx.x], tot);
+        } else if ((int)threadIdx.x < k) {
+            double m = warp_part[threadIdx.x];
+            const int nw = blockDim.x >> 5;
+            for (int w = 1; w < nw; ++w) m = fmax(m, warp_part[w * kTrendK + threadIdx.x]);
+            atomicMax(&gs->maxkey[mslot][threadIdx.x - ks], (unsigned long long)f64_key(m));
         }
         cooperative_groups::this_grid().sync();
-        if ((int)threadIdx.x < k) totals[threadIdx.x] = *reinterpret_cast<volatile double*>(&gs->acc[slot][threadIdx.x]);
+        if ((int)threadIdx.x < ks) totals[threadIdx.x] = *reinterpret_cast<volatile double*>(&gs->acc[slot][threadIdx.x]);
+        else if ((int)threadIdx.x < k)
+            totals[threadIdx.x] = f64_from_key(*reinterpret_cast<volatile unsigned long long*>(&gs->maxkey[mslot][threadIdx.x - ks]));
         if (blockIdx.x == 0 && (int)threadIdx.x < kTrendK) gs->acc[(p_sum + 2) % 3][threadIdx.x] = 0.0;
+        if (kmax && blockIdx.x == 0 && threadIdx.x < 2) gs->maxkey[(p_max + 2) % 3][threadIdx.x] = 0ull;
         __syncthreads();
         for (int j = 0; j < k; ++j) v[j] = totals[j];
         __syncthreads();  // totals is overwritten by the next reduction
         ++p_sum;
+        if (kmax) ++p_max;
     }
     __device__ double max_one(double v) {
         const int lane = threadIdx.x & 31, slot = p_max % 3;
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, off));
-        if (lane == 0) atomicMax(&gs->maxkey[slot], (unsigned long long)f64_key(v));
+        if (lane == 0) atomicMax(&gs->maxkey[slot][0], (unsigned long long)f64_key(v));
         cooperative_groups::this_grid().sync();
-        const double m = f64_from_key(*reinterpret_cast<volatile unsigned long long*>(&gs->maxkey[slot]));
-        if (blockIdx.x == 0 && threadIdx.x == 0) gs->maxkey[(p_max + 2) % 3] = 0ull;
+        const double m = f64_from_key(*reinterpret_cast<volatile unsigned long long*>(&gs->maxkey[slot][0]));
+        if (blockIdx.x == 0 && threadIdx.x < 2) gs->maxkey[(p_max + 2) % 3][threadIdx.x] = 0ull;
+        ++p_max;
+        return m;
+    }
+    // median_bins hooks: the same protocol as the cluster's, through global memory (zeroed before the launch) and grid barriers
+    __device__ void vhist_merge(unsigned* hist, int slot) {
+        __syncthreads();  // local bins complete
+        for (int j = threadIdx.x; j < kVBins; j += blockDim.x) {
+            const unsigned c = hist[j];
+            if (c) atomicAdd(&gs->vhist[slot][j], c);
+        }
+        cooperative_groups::this_grid().sync();
+        for (int j = threadIdx.x; j < kVBins; j += blockDim.x) hist[j] = __ldcg(&gs->vhist[slot][j]);
+        __syncthreads();
+    }
+    __device__ unsigned cand_index(int slot) { return atomicAdd(&gs->cursor[slot], 1u); }
+    // grid-wide maximum of one 64-bit key per thread, as integers (global 64-bit atomicMax is native)
+    __device__ unsigned long long max_key(unsigned long long v) {
+        const int slot = p_max % 3;
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            const unsigned long long o = __shfl_xor_sync(0xffffffffu, v, off);
+            v = o > v ? o : v;
+        }
+        if ((threadIdx.x & 31) == 0 && v) atomicMax(&gs->maxkey[slot][0], v);
+        cooperative_groups::this_grid().sync();
+        const unsigned long long m = __ldcg(&gs->maxkey[slot][0]);
+        if (blockIdx.x == 0 && threadIdx.x < 2) gs->maxkey[(p_max + 2) % 3][threadIdx.x] = 0ull;
         ++p_max;
         return m;
     }
@@ -773,11 +906,15 @@ __global__ void __launch_bounds__(1024) k_trend_prior_grid(const double* __restr
     __shared__ double warp_part[32 * kTrendK];
     __shared__ double totals[kTrendK];
     __shared__ unsigned hist[514];
+    __shared__ SelShared sel;
     GridReducer red{warp_part, totals, gs, 0, 0, 0};
     double *xs = scratch, *ts = scratch + n, *res = scratch + 2 * n;
     trend_prepare(red, x, t, n, x_is_mean != 0, lo, hi, xs, ts);
-    TrendOut o = trend_fit_outer(red, xs, ts, n, outer != 0);
-    if (with_prior && o.status == 0.0) trend_prior(red, x, t, n, lo, hi, min_disp, trigamma_c, res, hist, o);
+    TrendOut o = trend_fit_outer(red, xs, ts, n, outer != 0, false);
+    if (with_prior && o.status == 0.0)  // candidate buffer: xs, as in k_trend_prior
+        trend_prior_dev(red, x, t, n, lo, hi, min_disp, trigamma_c, res, reinterpret_cast<unsigned long long*>(xs), sel, hist, o);
+    else
+        red.sum_many(&o.n_used, 1);
     if (red.tid() == 0) *out = o;
 }
 
@@ -1202,6 +1339,9 @@ int PDQ_TUFN(launch_mu_from_lfc)(const LaunchCfg& c, const DesignDev& d, const d
 #if PDQ_TU_P == 0
 int launch_trend_fit(const LaunchCfg& c, const double* x, const double* t, double* scratch3n, size_t n, int x_is_mean,
                      double lo, double hi, int outer, double min_disp, double trigamma_c, int with_prior, double* out16) {
+    if (const char* e = getenv("PDQ_TREND_PRIOR")) {  // tuning hook: PDQ_TREND_PRIOR=0 skips the prior (times the fit alone)
+        if (atoi(e) == 0) with_prior = 0;
+    }
     // large vectors: one block per SM, cooperative launch (k_trend_prior_grid); PDQ_TREND_GRID=0/1 forces the choice
     {
         const char* e = getenv("PDQ_TREND_GRID");

@@ -32,7 +32,7 @@ struct TrendOut {
     double pad[5];
 };
 
-// Reducer concept: tid(), nthreads(), sum(double) -> block-wide total visible to every thread, sync().
+// Reducer concept: tid(), nthreads(), sum(double) -> block-wide total visible to every thread.
 struct SerialReducer {
     PDQ_HD int tid() const { return 0; }
     PDQ_HD int nthreads() const { return 1; }
@@ -166,12 +166,14 @@ PDQ_HD void trend_prepare(R& red, const double* x, const double* t, size_t n, bo
         xs[i] = xv;
         ts[i] = ok ? tv : (0.0 / 0.0);
     }
-    red.sync();
+    // no barrier: xs[i] / ts[i] are owned by the thread that writes them here -- every later pass of the fit (trend_sums, the
+    // drop loop, the `used` count) visits i = tid, tid + nthreads, ... with the same map, so each thread reads only its own writes
 }
 
-// Full outer loop of dds.py:1199-1275 on the prepared vectors; ts[i] is set to NaN when gene i is dropped.
+// Full outer loop of dds.py:1199-1275 on the prepared vectors; ts[i] is set to NaN when gene i is dropped.  With
+// `reduce_used` false, n_used is this thread's share of the count: the caller packs it into its next reduction.
 template <class R>
-PDQ_HD TrendOut trend_fit_outer(R& red, const double* xs, double* ts, size_t n, bool outer) {
+PDQ_HD TrendOut trend_fit_outer(R& red, const double* xs, double* ts, size_t n, bool outer, bool reduce_used = true) {
     double o0 = 0.1, o1 = 0.1, c0 = 1.0, c1 = 1.0, loss = 0.0;
     int rounds = 0, iters = 0;
     bool failed = false, last_conv = false;
@@ -195,12 +197,12 @@ PDQ_HD TrendOut trend_fit_outer(R& red, const double* xs, double* ts, size_t n, 
             const double ratio = tv / fma(c1, xs[i], c0);
             if (ratio < 1e-4 || ratio >= 15.0) ts[i] = 0.0 / 0.0;
         }
-        red.sync();
+        // no barrier: ts[i] stays owned by its thread (see trend_prepare)
     }
     double used = 0.0;
     for (size_t i = red.tid(); i < n; i += red.nthreads()) used += (ts[i] == ts[i]) ? 1.0 : 0.0;
-    red.sum_many(&used, 1);
-    TrendOut o;  // identical in every thread (all decisions were taken on block/cluster-wide sums)
+    if (reduce_used) red.sum_many(&used, 1);
+    TrendOut o;  // identical in every thread (all decisions were taken on block/cluster-wide sums), n_used aside (see above)
     o.c0 = c0;
     o.c1 = c1;
     o.status = failed ? 1.0 : 0.0;
@@ -307,6 +309,24 @@ PDQ_HD double log_ratio_entry(int64_t y, double logmean, bool& keep) {
     return keep ? log((double)y) - logmean : (0.0 / 0.0);
 }
 
+// Log residual of gene i against the fitted trend, or NaN when the gene is not part of the prior
+PDQ_HD double prior_residual(const double* means, const double* t, size_t i, double c0, double c1, double lo, double hi,
+                             double min_disp) {
+    double tv = t[i];
+    tv = (tv < lo) ? lo : ((tv > hi) ? hi : tv);
+    const double fit = c0 + c1 / means[i];
+    const bool use = (tv >= 100.0 * min_disp) && (means[i] == means[i]);
+    return use ? (log(tv) - log(fit)) : (0.0 / 0.0);
+}
+
+PDQ_HD void prior_finish(double mad, double trigamma_c, double cnt, TrendOut& out) {
+    const double sq = mad * mad;
+    out.squared_logres = sq;
+    const double pv = sq - trigamma_c;
+    out.prior_var = (pv > 0.25 || pv != pv) ? pv : 0.25;  // np.maximum propagates NaN
+    out.n_above = cnt;
+}
+
 // `res` : n doubles of scratch; `hist`: 514 unsigned in block-shared memory (see select_kth); `trigamma_c` = polygamma(1, (N-p)/2)
 template <class R>
 PDQ_HD void trend_prior(R& red, const double* means, const double* t, size_t n, double lo, double hi, double min_disp,
@@ -315,22 +335,168 @@ PDQ_HD void trend_prior(R& red, const double* means, const double* t, size_t n, 
     double cnt = 0.0;
     // every thread fills (and later only ever reads) its own stride of the scratch vector: no barrier needed
     for (size_t i = red.tid(); i < n; i += red.nthreads()) {
-        double tv = t[i];
-        tv = (tv < lo) ? lo : ((tv > hi) ? hi : tv);
-        const double fit = c0 + c1 / means[i];
-        const bool use = (tv >= 100.0 * min_disp) && (means[i] == means[i]);
-        res[i] = use ? (log(tv) - log(fit)) : (0.0 / 0.0);
-        cnt += use ? 1.0 : 0.0;
+        res[i] = prior_residual(means, t, i, c0, c1, lo, hi, min_disp);
+        cnt += (res[i] == res[i]) ? 1.0 : 0.0;
     }
     red.sum_many(&cnt, 1);
     const size_t m = (size_t)cnt;
     const double med = median_of(red, res, n, m, false, 0.0, hist);
     const double mad = median_of(red, res, n, m, true, med, hist) * 1.4826022185056018;  // / (sqrt(2) erfinv(1/2))
-    const double sq = mad * mad;
-    out.squared_logres = sq;
-    const double pv = sq - trigamma_c;
-    out.prior_var = (pv > 0.25 || pv != pv) ? pv : 0.25;  // np.maximum propagates NaN
-    out.n_above = cnt;
+    prior_finish(mad, trigamma_c, cnt, out);
 }
+
+#if defined(__CUDACC__)
+// ---------------------------------------------------------------------------------------------------------
+// The prior's medians on the device in a fixed number of cluster- / grid-wide rounds, whatever the key width:
+//   1. the value range [vlo, vhi] comes with the count of prior genes (one packed sum + max reduction);
+//   2. each block counts its slice into kVBins equal-width value bins -- bin(v) = clamp(floor((v - vlo) * scale)) is monotone
+//      non-decreasing in v, so the k-th smallest value lies in the first bin b whose running count exceeds k -- and the blocks
+//      merge their histograms in one round;
+//   3. the values of bin b (their order-preserving keys) go to a global candidate buffer in one round; the same round brings
+//      the largest value below bin b, which is the lower median of an even count when rank k opens bin b;
+//   4. every block picks the exact ranks among the candidates with block-local barriers only.
+// Too many candidates (heavy ties: genes clipped to max_disp), or a range of zero or non-finite width, fall back to the exact
+// 8-digit radix walk of median_of.  Both give the exact order statistics, so the result does not depend on the path.
+// Reducer hooks: sum_many(v, k, kmax) (the last kmax entries are maxima), vhist_merge(hist, slot), cand_index(slot),
+// max_key(key) (integer maximum of 64-bit keys).
+// ---------------------------------------------------------------------------------------------------------
+constexpr int kVBins = 2048;
+constexpr int kCandCap = 1024;
+
+struct SelShared {                       // block-shared memory of median_bins
+    unsigned hist[kVBins];               // the block's bins, then the merged bins
+    unsigned long long keys[kCandCap];   // candidate keys of the chosen bin
+    unsigned warp_sum[32];
+    unsigned bin[3];                     // chosen bin, count before it, count in it
+    unsigned long long pick[2];          // keys at the upper and lower rank
+};
+
+__device__ __forceinline__ int vbin(double v, double vlo, double scale) {
+    const double x = (v - vlo) * scale;
+    return x <= 0.0 ? 0 : (x >= (double)(kVBins - 1) ? kVBins - 1 : (int)x);
+}
+
+// first bin of `hist` whose running count exceeds k -> sh.bin = {bin, count before it, count in it}, visible to the block
+__device__ inline void find_vbin(SelShared& sh, size_t k) {
+    const int per = kVBins / blockDim.x, b0 = threadIdx.x * per;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned tot = 0;
+    for (int j = 0; j < per; ++j) tot += sh.hist[b0 + j];
+    unsigned inc = tot;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const unsigned u = __shfl_up_sync(0xffffffffu, inc, off);
+        if (lane >= off) inc += u;
+    }
+    if (lane == 31) sh.warp_sum[warp] = inc;
+    __syncthreads();
+    unsigned before = inc - tot;
+    for (int w = 0; w < warp; ++w) before += sh.warp_sum[w];
+    const unsigned kk = (unsigned)k;
+    if (before <= kk && kk < before + tot) {  // exactly one thread owns the crossing
+        unsigned run = before;
+        int j = 0;
+        for (; j < per; ++j) {
+            if (run + sh.hist[b0 + j] > kk) break;
+            run += sh.hist[b0 + j];
+        }
+        sh.bin[0] = (unsigned)(b0 + j);
+        sh.bin[1] = run;
+        sh.bin[2] = sh.hist[b0 + j];
+    }
+    __syncthreads();
+}
+
+// k-th smallest of { |res[i] - center| or res[i] } (0-based) over the non-NaN entries; when `lower`, also rank k - 1.  Returns
+// the exact values, as median_of.  [vlo, vhi] bounds the values.  `cand`: kCandCap keys of global scratch no thread reads
+// or writes meanwhile.  `slot` (0, 1) picks the reducer's merge buffers: the two medians of one launch use different slots.
+template <class R>
+__device__ double median_bins(R& red, const double* res, size_t n, size_t cnt, bool absdev, double center, double vlo,
+                              double vhi, int slot, unsigned long long* cand, SelShared& sh, unsigned* hist514) {
+    if (cnt == 0) return 0.0 / 0.0;  // np.median([]) = nan
+    const double width = vhi - vlo, scale = (double)kVBins / width;
+    if (!(width > 0.0 && width <= 1.7976931348623157e308 && scale <= 1.7976931348623157e308))
+        return median_of(red, res, n, cnt, absdev, center, hist514);  // equal values, or infinite ones
+    const size_t k = cnt / 2;
+    const bool even = !(cnt & 1);
+    for (int b = threadIdx.x; b < kVBins; b += blockDim.x) sh.hist[b] = 0;
+    __syncthreads();
+    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
+        const double r = res[i];
+        if (!(r == r)) continue;
+        atomicAdd(&sh.hist[vbin(absdev ? fabs(r - center) : r, vlo, scale)], 1u);
+    }
+    red.vhist_merge(sh.hist, slot);  // one round: sh.hist holds the totals, identical in every block
+    find_vbin(sh, k);
+    const int b = (int)sh.bin[0];
+    const unsigned before = sh.bin[1], inbin = sh.bin[2];
+    if (inbin > (unsigned)kCandCap) return median_of(red, res, n, cnt, absdev, center, hist514);
+    const unsigned r_hi = (unsigned)k - before;
+    const bool below = even && r_hi == 0;  // rank k - 1 is the largest value of the bins below b
+    unsigned long long mx = 0ull;          // below every key of a non-NaN double
+    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
+        const double r = res[i];
+        if (!(r == r)) continue;
+        const double v = absdev ? fabs(r - center) : r;
+        const int bi = vbin(v, vlo, scale);
+        if (bi == b) {
+            cand[red.cand_index(slot)] = f64_key(v);
+        } else if (below && bi < b) {
+            const unsigned long long key = f64_key(v);
+            mx = key > mx ? key : mx;
+        }
+    }
+    // one round: the candidates are written and visible, and every block learns the largest key below bin b.  The keys are
+    // reduced as integers: key 0 (a thread that saw nothing below b) is below every key of a non-NaN double
+    mx = red.max_key(mx);
+    for (unsigned j = threadIdx.x; j < inbin; j += blockDim.x) sh.keys[j] = __ldcg(cand + j);
+    __syncthreads();
+    // exact ranks among the candidates: a key is at rank r when (#smaller) <= r < (#smaller) + (#equal)
+    const bool lower_in_bin = even && !below;
+    for (unsigned i = threadIdx.x; i < inbin; i += blockDim.x) {
+        const unsigned long long key = sh.keys[i];
+        unsigned less = 0, eq = 0;
+        for (unsigned j = 0; j < inbin; ++j) {
+            const unsigned long long o = sh.keys[j];
+            less += o < key;
+            eq += o == key;
+        }
+        if (less <= r_hi && r_hi < less + eq) sh.pick[0] = key;  // equal keys write equal values
+        if (lower_in_bin && less <= r_hi - 1 && r_hi - 1 < less + eq) sh.pick[1] = key;
+    }
+    __syncthreads();
+    const double hi = f64_from_key(sh.pick[0]);
+    const double lo = !even ? hi : f64_from_key(below ? mx : sh.pick[1]);
+    __syncthreads();  // sh is reused by the next selection
+    return even ? 0.5 * (lo + hi) : hi;
+}
+
+// trend_prior on the device: the count of prior genes, the fit's `used` count (this thread's share in out.n_used, see
+// trend_fit_outer) and the residuals' range share one reduction; the two medians run through median_bins.
+template <class R>
+__device__ void trend_prior_dev(R& red, const double* means, const double* t, size_t n, double lo, double hi, double min_disp,
+                                double trigamma_c, double* res, unsigned long long* cand, SelShared& sh, unsigned* hist514,
+                                TrendOut& out) {
+    const double c0 = out.c0, c1 = out.c1;
+    double v[4] = {0.0, out.n_used, -HUGE_VAL, -HUGE_VAL};  // count, used, max, -min
+    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
+        const double r = prior_residual(means, t, i, c0, c1, lo, hi, min_disp);
+        res[i] = r;  // each thread later reads only its own stride of res: no barrier needed
+        if (!(r == r)) continue;
+        v[0] += 1.0;
+        v[2] = fmax(v[2], r);
+        v[3] = fmax(v[3], -r);
+    }
+    red.sum_many(v, 4, 2);
+    out.n_used = v[1];
+    const size_t m = (size_t)v[0];
+    const double rmax = v[2], rmin = -v[3];
+    const double med = median_bins(red, res, n, m, false, 0.0, rmin, rmax, 0, cand, sh, hist514);
+    // |r - med| is largest at an end of the range (r - med is monotone in r); the smallest deviation is >= 0
+    const double dmax = fmax(fabs(rmax - med), fabs(rmin - med));
+    const double mad = median_bins(red, res, n, m, true, med, 0.0, dmax, 1, cand, sh, hist514) * 1.4826022185056018;
+    prior_finish(mad, trigamma_c, v[0], out);
+}
+#endif
 
 }  // namespace pdq
