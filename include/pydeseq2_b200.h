@@ -201,6 +201,17 @@ int pdq_lfc_shrink_nbinom_glm(pdq_ctx* ctx, const double* X, const int64_t* coun
  * of log(count) - gene mean (radix select), exponentiated.  `sf_out` (N,).  All entries NaN when every gene holds a zero
  * (the reference then switches to its iterative fallback, dds.py:682-690). */
 int pdq_size_factors(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, double* sf_out, double* logmeans_out /* per-gene mean log count (-inf when the gene holds a zero), may be NULL */);
+/* DeseqDataSet.fit_size_factors (dds.py:584-711) for fit_type "ratio" (kind 0) or "poscounts" (kind 1), over every gene or over
+ * control genes only (DESeq2's controlGenes, dds.py:628-651).  `control` (G,) 0/1 per gene, NULL = every gene.
+ *   kind 0: log means as pdq_size_factors; medians over the control genes with a finite log mean (dds.py:693-703).
+ *   kind 1: log means over ALL samples with a zero count taken as log 1 = 0 (dds.py:658-660); per sample the median of
+ *           log(count) - log mean over the control genes with a log mean > 0 and a POSITIVE count (dds.py:663-669), exponentiated,
+ *           then divided by the geometric mean over samples (dds.py:675).
+ * A sample without a usable gene gets NaN (poscounts: every size factor is then NaN, as np.mean propagates it).  `logmeans_out`
+ * (may be NULL) receives the raw log means, not masked by `control`.  kind 0 with control NULL equals pdq_size_factors byte for
+ * byte.  PDQ_ERR_INVALID for an unknown kind. */
+int pdq_size_factors_ex(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control, double* sf_out,
+                        double* logmeans_out);
 /* Size factors of NEW samples against the log means of a fit -- preprocessing.deseq2_norm_transform (preprocessing.py:59-102), what
  * DeseqDataSet.vst_transform(counts) does with held-out counts (dds.py:478-486).  `logmeans` (G,): genes with a non-finite entry
  * are left out (the fit's filtered_genes are exactly its finite log means).  A zero count in a kept gene enters the median as
@@ -293,6 +304,9 @@ int pdq_lfc_shrink_dev(pdq_ctx* ctx, const pdq_design* design, const int64_t* co
 /* device-resident flavour of pdq_size_factors; `logmeans_out` (G,) may be NULL */
 int pdq_size_factors_dev(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, double* sf_out,
                          double* logmeans_out);
+/* device-resident flavour of pdq_size_factors_ex (`control` is device memory here, may be NULL) */
+int pdq_size_factors_ex_dev(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control,
+                            double* sf_out, double* logmeans_out);
 /* device-resident flavours of pdq_size_factors_from_logmeans and pdq_vst_transform (`size_factors` is device memory here) */
 int pdq_size_factors_from_logmeans_dev(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
                                        double* sf_out);

@@ -100,6 +100,8 @@ _SIGNATURES = {
     "pdq_lfc_shrink_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, c_dptr, C.c_double, C.c_double, C.c_int, c_dptr,
                                      c_dptr, c_dptr, c_dptr]),
     "pdq_size_factors_dev": (C.c_int, [c_ctx, c_dptr, C.c_int64, C.c_int, C.c_int, c_dptr, c_dptr]),
+    "pdq_size_factors_ex": (C.c_int, [c_ctx, i64p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, f64p, f64p]),
+    "pdq_size_factors_ex_dev": (C.c_int, [c_ctx, c_dptr, C.c_int64, C.c_int, C.c_int, C.c_int, c_dptr, c_dptr, c_dptr]),
     "pdq_size_factors_from_logmeans": (C.c_int, [c_ctx, i64p, C.c_int64, C.c_int, C.c_int, f64p, f64p]),
     "pdq_size_factors_from_logmeans_dev": (C.c_int, [c_ctx, c_dptr, C.c_int64, C.c_int, C.c_int, c_dptr, c_dptr]),
     "pdq_vst_transform": (C.c_int, [c_ctx, i64p, C.c_int64, C.c_int, C.c_int, f64p, C.c_int, C.c_double, C.c_double, f64p,

@@ -749,6 +749,26 @@ extern "C" int pdq_size_factors_dev(pdq_ctx* c, const int64_t* counts, int64_t l
     return done(c, launch_size_factors(cfg(c, G, N), counts, ld, N, G, (double*)lm, (double*)scratch, sf_out), "size_factors");
 }
 
+static int sf_ex_check(pdq_ctx* c, const void* counts, const void* sf_out, int64_t ld, int N, int G, int kind, const char* what) {
+    if (!counts || !sf_out || N <= 0 || G <= 0 || ld < G) return fail(c, PDQ_ERR_INVALID, "%s: bad arguments", what);
+    if (kind != 0 && kind != 1) return fail(c, PDQ_ERR_INVALID, "%s: unknown kind %d (0 ratio, 1 poscounts)", what, kind);
+    return PDQ_OK;
+}
+
+extern "C" int pdq_size_factors_ex_dev(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control,
+                                       double* sf_out, double* logmeans_out) {
+    CHECK_CTX(c);
+    if (int e = sf_ex_check(c, counts, sf_out, ld, N, G, kind, "pdq_size_factors_ex_dev")) return e;
+    void *lm = logmeans_out, *kept, *scratch;
+    if (!lm)
+        if (int e = ensure(c, kBufF, (size_t)G * 8, &lm)) return e;
+    if (int e = ensure(c, kBufC, (size_t)G * 8, &kept)) return e;
+    if (int e = ensure(c, kBufB, (size_t)N * G * 8, &scratch)) return e;
+    return done(c, launch_size_factors_ex(cfg(c, G, N), counts, ld, N, G, kind, control, (double*)lm, (double*)kept, (double*)scratch,
+                                          sf_out),
+                "size_factors_ex");
+}
+
 extern "C" int pdq_size_factors_from_logmeans_dev(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
                                                   double* sf_out) {
     CHECK_CTX(c);
@@ -1470,6 +1490,29 @@ extern "C" int pdq_size_factors(pdq_ctx* c, const int64_t* counts, int64_t ld, i
     if (up_c)
         if (int e = h2d_2d(c, dc, counts, ld, N, G, 8)) return e;
     if (int e = pdq_size_factors_dev(c, (const int64_t*)dc, G, N, G, (double*)dsf, (double*)dlm)) return e;
+    CU(c, cudaMemcpyAsync(sf_out, dsf, (size_t)N * 8, cudaMemcpyDeviceToHost, c->stream));
+    if (logmeans_out) CU(c, cudaMemcpyAsync(logmeans_out, dlm, (size_t)G * 8, cudaMemcpyDeviceToHost, c->stream));
+    return call_end(c, nullptr, {});
+}
+
+extern "C" int pdq_size_factors_ex(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control,
+                                   double* sf_out, double* logmeans_out) {
+    CHECK_CTX(c);
+    if (int e = sf_ex_check(c, counts, sf_out, ld, N, G, kind, "pdq_size_factors_ex")) return e;
+    void *dc, *dsf, *dlm = nullptr, *dctl = nullptr;
+    res_begin(c);
+    bool up_c;
+    if (int e = res_input(c, counts, ld, N, G, 8, kBufCounts, &dc, &up_c)) return e;
+    if (int e = ensure(c, kBufE, (size_t)N * 8, &dsf)) return e;
+    if (logmeans_out)
+        if (int e = ensure(c, kBufG, (size_t)G * 8, &dlm)) return e;
+    if (control)
+        if (int e = ensure(c, kBufKeep, (size_t)G, &dctl)) return e;
+    if (up_c)
+        if (int e = h2d_2d(c, dc, counts, ld, N, G, 8)) return e;
+    if (control)
+        if (int e = vec_h2d(c, dctl, control, (size_t)G)) return e;
+    if (int e = pdq_size_factors_ex_dev(c, (const int64_t*)dc, G, N, G, kind, (const uint8_t*)dctl, (double*)dsf, (double*)dlm)) return e;
     CU(c, cudaMemcpyAsync(sf_out, dsf, (size_t)N * 8, cudaMemcpyDeviceToHost, c->stream));
     if (logmeans_out) CU(c, cudaMemcpyAsync(logmeans_out, dlm, (size_t)G * 8, cudaMemcpyDeviceToHost, c->stream));
     return call_end(c, nullptr, {});

@@ -85,6 +85,9 @@ int launch_hash(cudaStream_t stream, int sm_count, const void* dptr, size_t word
 int launch_fp64_peak(const LaunchCfg&, double* out /* sm_count * 8 * 256 doubles */, int iters, double* flop);
 int launch_size_factors(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, double* logmeans,
                         double* scratch, double* sf_out);
+// kind kSfRatio / kSfPoscounts (pdq_trend.cuh); `control` (G,) may be NULL; `kept` (G,) scratch, NULL only for ratio over every gene
+int launch_size_factors_ex(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control,
+                           double* logmeans, double* kept, double* scratch, double* sf_out);
 int launch_size_factors_from_logmeans(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
                                       double* scratch, double* sf_out);
 // kind 0 parametric (c0 = a0, c1 = a1), 1 mean (c0 = mean dispersion); see pdq_vst.cuh

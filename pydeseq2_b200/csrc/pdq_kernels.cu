@@ -918,24 +918,33 @@ __global__ void __launch_bounds__(1024) k_trend_prior_grid(const double* __restr
     if (red.tid() == 0) *out = o;
 }
 
-// ---- median-of-ratios size factors (preprocessing.py:31-102), SURVEY.md §8 f-2 -------------------------------------
-// 1. per-gene mean of log counts (-inf when the gene holds a zero: such genes are filtered out, preprocessing.py:52-54)
-__global__ void __launch_bounds__(kBlock) k_log_means(const int64_t* __restrict__ counts, int64_t ld, int N, int G, int lgT,
-                                                      double* __restrict__ logmeans) {
+// ---- size factors: median of ratios (preprocessing.py:31-102) and poscounts, over all or control genes (dds.py:628-679) --------
+// SURVEY.md §8 f-2
+// 1. per-gene mean over all samples of log_mean_term (ratio: -inf when the gene holds a zero, such genes are filtered out,
+//    preprocessing.py:52-54).  `kept` (may be NULL): the log mean each gene enters the medians with, NaN when it is left out
+//    (kept_logmean; `control` (G,) may be NULL = every gene)
+__global__ void __launch_bounds__(kBlock) k_log_means(const int64_t* __restrict__ counts, int64_t ld, int N, int G, int lgT, int kind,
+                                                      const uint8_t* __restrict__ control, double* __restrict__ logmeans,
+                                                      double* __restrict__ kept) {
     Group grp;
     int g;
     bool valid;
     map_lanes(lgT, G, grp, g, valid);
     const int64_t* yp = counts + g + (int64_t)grp.si * ld;
     double s = 0.0;
-    for (int n = grp.si; n < N; n += grp.T, yp += (int64_t)grp.T * ld) s += log((double)*yp);  // libdevice log: log(0) = -inf
+    for (int n = grp.si; n < N; n += grp.T, yp += (int64_t)grp.T * ld) s += log_mean_term(*yp, kind);  // libdevice log: log(0) = -inf
     s = grp.sum(s);
-    if (valid && grp.si == 0) logmeans[g] = s / (double)N;
+    if (valid && grp.si == 0) {
+        const double lm = s / (double)N;
+        logmeans[g] = lm;
+        if (kept) kept[g] = kept_logmean(lm, kind, control == nullptr || control[g] != 0);
+    }
 }
 
-// 2. one block per sample: log ratios of the sample against the gene means, exact median by radix select
+// 2. one block per sample: log ratios of the sample against the gene means, exact median by radix select.  `skip_zero`: zero
+//    counts are left out (poscounts)
 __global__ void __launch_bounds__(1024) k_size_factor_median(const int64_t* __restrict__ counts, int64_t ld, int G,
-                                                             const double* __restrict__ logmeans, double* scratch,
+                                                             const double* __restrict__ logmeans, int skip_zero, double* scratch,
                                                              double* sf_out) {
     __shared__ unsigned hist[514];
     __shared__ double warp_part[32 * kTrendK];
@@ -950,7 +959,7 @@ __global__ void __launch_bounds__(1024) k_size_factor_median(const int64_t* __re
     unsigned cnt = 0;
     for (int g = threadIdx.x; g < G; g += blockDim.x) {
         bool keep;
-        row[g] = log_ratio_entry(c[g], logmeans[g], keep);
+        row[g] = log_ratio_entry(c[g], logmeans[g], keep, skip_zero != 0);
         cnt += keep;
     }
     atomicAdd(&cnt_s, cnt);
@@ -958,6 +967,21 @@ __global__ void __launch_bounds__(1024) k_size_factor_median(const int64_t* __re
     ClusterReducer red{warp_part, slots, totals, 0u, 1u, 0};  // one block per sample: the single-block paths of the reducer
     const double med = median_of(red, row, (size_t)G, (size_t)cnt_s, false, 0.0, hist);
     if (threadIdx.x == 0) sf_out[n] = exp(med);
+}
+
+// 3. poscounts only: sf / exp(mean(log sf)) (dds.py:674-675), one block.  A NaN size factor (a sample without a usable gene) makes
+//    the mean, and so every entry, NaN, as in numpy
+__global__ void __launch_bounds__(1024) k_size_factor_geomean(double* sf, int N) {
+    __shared__ double part[32];
+    double s = 0.0;
+    for (int n = threadIdx.x; n < N; n += blockDim.x) s += log(sf[n]);
+    for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+    __syncthreads();  // every read of sf above happens before any write below
+    double tot = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += part[w];
+    const double gm = exp(tot / (double)N);
+    for (int n = threadIdx.x; n < N; n += blockDim.x) sf[n] = sf[n] / gm;
 }
 
 // fitted = c0 + c1 / mean (dds.py:1267-1275) from the device-resident coefficients
@@ -1500,16 +1524,23 @@ int launch_fp64_peak(const LaunchCfg& c, double* out, int iters, double* flop) {
 
 int launch_size_factors(const LaunchCfg& c, const int64_t* counts, int64_t ld, int N, int G, double* logmeans,
                         double* scratch, double* sf_out) {
-    k_log_means<<<grid_for(G, c.lgT), kBlock, 0, c.stream>>>(counts, ld, N, G, c.lgT, logmeans);
-    k_size_factor_median<<<N, 1024, 0, c.stream>>>(counts, ld, G, logmeans, scratch, sf_out);
+    return launch_size_factors_ex(c, counts, ld, N, G, kSfRatio, nullptr, logmeans, nullptr, scratch, sf_out);
+}
+
+// `kept` NULL: median of ratios over every gene, whose medians read the log means directly (-inf = left out)
+int launch_size_factors_ex(const LaunchCfg& c, const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control,
+                           double* logmeans, double* kept, double* scratch, double* sf_out) {
+    k_log_means<<<grid_for(G, c.lgT), kBlock, 0, c.stream>>>(counts, ld, N, G, c.lgT, kind, control, logmeans, kept);
+    k_size_factor_median<<<N, 1024, 0, c.stream>>>(counts, ld, G, kept ? kept : logmeans, kind == kSfPoscounts, scratch, sf_out);
+    if (kind == kSfPoscounts) k_size_factor_geomean<<<1, 1024, 0, c.stream>>>(sf_out, N);
     if (int e = check_launch()) return e;
-    return 2;
+    return kind == kSfPoscounts ? 3 : 2;
 }
 
 // held-out samples (preprocessing.py:59-102): the medians against the caller's log means, non-finite entries = genes left out
 int launch_size_factors_from_logmeans(const LaunchCfg& c, const int64_t* counts, int64_t ld, int N, int G, const double* logmeans,
                                       double* scratch, double* sf_out) {
-    k_size_factor_median<<<N, 1024, 0, c.stream>>>(counts, ld, G, logmeans, scratch, sf_out);
+    k_size_factor_median<<<N, 1024, 0, c.stream>>>(counts, ld, G, logmeans, 0, scratch, sf_out);
     if (int e = check_launch()) return e;
     return 1;
 }

@@ -301,11 +301,27 @@ PDQ_HD double median_of(R& red, const double* res, size_t n, size_t cnt, bool ab
     return 0.5 * (lo + hi);
 }
 
+// Size-factor estimators (`kind` of pdq_size_factors_ex): median of ratios (preprocessing.py:31-102) and DESeq2's "poscounts"
+// (dds.py:656-679)
+enum { kSfRatio = 0, kSfPoscounts = 1 };
+
+// One sample's term of a gene's log mean over ALL samples: log(count), -inf for a zero (ratio: the gene is then left out,
+// preprocessing.py:52-54), or for poscounts the log of a positive count and 0 for a zero (dds.py:658-660)
+PDQ_HD double log_mean_term(int64_t y, int kind) { return (kind == kSfPoscounts && y == 0) ? 0.0 : log((double)y); }
+
+// The log mean a gene enters the medians with, or NaN when it is left out: not a control gene, a non-finite log mean, or for
+// poscounts a log mean not above 0 -- every positive count 1, or an all-zero gene (dds.py:663-664, 696)
+PDQ_HD double kept_logmean(double lm, int kind, bool control) {
+    const bool keep = control && fabs(lm) <= 1.7976931348623157e308 && (kind != kSfPoscounts || lm > 0.0);
+    return keep ? lm : (0.0 / 0.0);
+}
+
 // One entry of a sample's median of ratios (preprocessing.py:52-54, 89-97): log(count) - log mean of the gene, or NaN -- left out of
-// the median -- for a gene whose log mean is not finite (~np.isinf(logmeans); NaN cannot occur for counts >= 0).  A zero count in
-// a kept gene gives -inf, which takes part in the median as in numpy.  `keep` says whether the gene counts.
-PDQ_HD double log_ratio_entry(int64_t y, double logmean, bool& keep) {
-    keep = fabs(logmean) <= 1.7976931348623157e308;
+// the median -- for a gene whose log mean is not finite (~np.isinf(logmeans), or NaN from kept_logmean).  A zero count in a kept
+// gene gives -inf, which takes part in the median as in numpy, unless `skip_zero` (poscounts: only positive counts enter,
+// dds.py:668-669).  `keep` says whether the entry counts.
+PDQ_HD double log_ratio_entry(int64_t y, double logmean, bool& keep, bool skip_zero = false) {
+    keep = fabs(logmean) <= 1.7976931348623157e308 && !(skip_zero && y == 0);
     return keep ? log((double)y) - logmean : (0.0 / 0.0);
 }
 

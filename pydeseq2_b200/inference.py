@@ -28,6 +28,27 @@ from . import _lib
 from ._lib import ALT_CODES, B200Error, as_f64p, as_i64p
 
 VST_KINDS = {"parametric": 0, "mean": 1}  # `kind` of pdq_vst_transform
+SF_KINDS = {"ratio": 0, "poscounts": 1}  # `kind` of pdq_size_factors_ex
+
+
+def control_mask(control_genes, G):
+    """Boolean (G,) mask of control genes (DESeq2's ``controlGenes``, dds.py:628-651) from a boolean mask of length G or integer
+    positions; None stays None (every gene).  Gene names are resolved by the caller (``DeseqDataSet._normalize_indices``)."""
+    if control_genes is None:
+        return None
+    c = np.asarray(control_genes.values if hasattr(control_genes, "values") else control_genes)
+    if c.dtype == bool:
+        if c.shape != (G,):
+            raise ValueError(f"control_genes is a mask of shape {c.shape} for {G} genes")
+        return c.copy()
+    if c.ndim != 1 or (c.size and c.dtype.kind not in "iu"):
+        raise ValueError("control_genes must be a boolean mask or integer gene positions")
+    mask = np.zeros(G, dtype=bool)
+    try:
+        mask[c.astype(np.int64)] = True
+    except IndexError as e:
+        raise ValueError(f"control_genes: {e}") from None
+    return mask
 
 try:  # the reference, when it is importable, provides the ABC we plug into
     from pydeseq2.inference import Inference as _InferenceBase  # type: ignore
@@ -156,6 +177,11 @@ class _CudaOps:
         self._io((counts,), (sf,))
         self.ctx.check(self.lib.pdq_size_factors(self.ctx.h, as_i64p(counts), ld, N, G, as_f64p(sf),
                                                  as_f64p(logmeans) if logmeans is not None else None))
+
+    def size_factors_ex(self, counts, ld, N, G, kind, control, sf, logmeans):
+        self._io((counts,) + ((control,) if control is not None else ()), (sf, logmeans))
+        self.ctx.check(self.lib.pdq_size_factors_ex(self.ctx.h, as_i64p(counts), ld, N, G, kind,
+                                                    control.ctypes.data if control is not None else None, as_f64p(sf), as_f64p(logmeans)))
 
     def size_factors_from_logmeans(self, counts, ld, N, G, logmeans, sf):
         self._io((counts, logmeans), (sf,))
@@ -395,7 +421,7 @@ class B200Inference(_InferenceBase):
             return None
         return np.array([out16[0], out16[1]]), fitted, float(out16[8]), float(out16[9]), int(out16[3])
 
-    def size_factors(self, counts, return_logmeans: bool = False, logmeans=None):
+    def size_factors(self, counts, return_logmeans: bool = False, logmeans=None, fit_type: str = "ratio", control_genes=None):
         """Median-of-ratios size factors on the device (``preprocessing.deseq2_norm``, preprocessing.py:5-102).
 
         Not part of the ``Inference`` ABC -- the reference computes them in the orchestrator (``dds.py:584-711``) --
@@ -403,14 +429,34 @@ class B200Inference(_InferenceBase):
         ``deseq2_norm``; raises ``ValueError`` when every gene contains a zero (the reference's cue to switch to its
         iterative estimator, ``dds.py:682-690``).
 
+        ``fit_type="poscounts"`` fits DESeq2's poscounts estimator instead (dds.py:656-679): log means over all samples with zeros
+        taken as log 1, medians over the genes with a log mean > 0 and over each sample's positive counts only, scaled to a
+        geometric mean of 1.  It never raises: a sample without a usable gene makes every size factor NaN, as in numpy.
+        ``control_genes`` (boolean mask of length G, or integer positions): take the medians over these genes only (DESeq2's
+        ``controlGenes``, dds.py:628-651), for either fit type.  The log means returned are not masked by them; with ``"ratio"``,
+        a control set without a finite log mean gives NaN size factors, and a table in which every gene holds a zero still raises.
+
         ``logmeans`` (G,): normalise NEW counts against the log means of an earlier fit instead
         (``deseq2_norm_transform``, preprocessing.py:59-102, with ``filtered_genes`` = the finite entries; pass -inf for a gene
         to leave out).  This is how held-out samples are normalised (dds.py:478-486): a zero count in a kept gene counts as a
         log ratio of -inf, so a sample can get size factor 0 (and infinite / NaN normalised counts), exactly as in numpy; nothing
         is raised.
         """
+        if fit_type not in SF_KINDS:
+            raise ValueError(f"fit_type must be one of {sorted(SF_KINDS)} on the device, got {fit_type!r}")
+        if logmeans is not None and (fit_type != "ratio" or control_genes is not None):
+            raise ValueError("logmeans= normalises held-out counts; it takes no fit_type or control_genes")
         counts, ld = _rows(counts, np.int64, "counts")
         N, G = counts.shape
+        ctl = control_mask(control_genes, G)
+        if fit_type != "ratio" or ctl is not None:
+            sf, lm = np.empty(N), np.empty(G)
+            self._ops.size_factors_ex(counts, ld, N, G, SF_KINDS[fit_type], None if ctl is None else ctl.astype(np.uint8), sf, lm)
+            if fit_type == "ratio" and np.isinf(lm).all():
+                raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
+            with np.errstate(invalid="ignore"):
+                normed = counts / sf[:, None]
+            return (normed, sf, lm) if return_logmeans else (normed, sf)
         if logmeans is not None:
             lm = np.ascontiguousarray(_f64(logmeans, "logmeans", 1))
             if lm.shape[0] != G:

@@ -18,25 +18,41 @@ from __future__ import annotations
 import numpy as np
 
 
-def b200_dataset_class():
+def b200_dataset_class(all_size_factors=False):
     """Returns a ``DeseqDataSet`` subclass whose ``fit_size_factors`` (plain median-of-ratios case), ``calculate_cooks`` and
     ``vst_transform`` call the backend when it offers ``size_factors`` / ``calculate_cooks`` / ``vst_transform`` (``B200Inference``
     does), and fall back to the reference's own implementation otherwise (other fit types, control genes, a missing VST fit,
-    held-out counts after iteratively fitted size factors, a different backend)."""
+    held-out counts after iteratively fitted size factors, a different backend).
+
+    ``all_size_factors=True`` also sends ``"poscounts"`` and control genes (with ``"ratio"`` or ``"poscounts"``, dds.py:628-679) to
+    the backend.  It is opt-in so that the size factors of existing code do not change unnoticed; ``"iterative"``, and ratio when
+    every gene holds a zero, stay with the reference either way."""
     from pydeseq2.dds import DeseqDataSet
+
+    from .pipeline import filtered_genes
 
     class B200DeseqDataSet(DeseqDataSet):
         def fit_size_factors(self, fit_type=None, control_genes=None):  # dds.py:584-711
             kind = self.size_factors_fit_type if fit_type is None else fit_type
-            plain = (kind == "ratio" and control_genes is None and not hasattr(self, "control_genes")
-                     and hasattr(self.inference, "size_factors") and isinstance(self.X, np.ndarray))
-            if plain:
+            # an explicit control_genes= overrides the attribute set at init, which the reference always sets (None by default)
+            control = control_genes if control_genes is not None else getattr(self, "control_genes", None)
+            plain = kind == "ratio" and control is None
+            device = (plain or (all_size_factors and kind in ("ratio", "poscounts"))) and hasattr(self.inference, "size_factors") \
+                and isinstance(self.X, np.ndarray)
+            if device:
+                kw = {}
+                if not plain:
+                    mask = None
+                    if control is not None:  # masks, positions or var names, resolved as the reference does (dds.py:641-647)
+                        mask = np.zeros(self.X.shape[1], dtype=bool)
+                        mask[self._normalize_indices((slice(None), control))[1]] = True
+                    kw = {"fit_type": kind, "control_genes": mask}
                 try:
-                    normed, sf, logmeans = self.inference.size_factors(self.X, return_logmeans=True)
+                    normed, sf, logmeans = self.inference.size_factors(self.X, return_logmeans=True, **kw)
                 except ValueError:  # every gene holds a zero: the reference switches to its iterative estimator (dds.py:682-690)
                     return super().fit_size_factors(fit_type=fit_type, control_genes=control_genes)
-                # what the reference keeps from deseq2_norm_fit (dds.py:693): vst_fit / vst_transform normalise NEW counts with them
-                self.logmeans, self.filtered_genes = logmeans, ~np.isinf(logmeans)
+                # what the reference keeps (dds.py:663, 679, 693): vst_fit / vst_transform normalise NEW counts with them
+                self.logmeans, self.filtered_genes = logmeans, filtered_genes(logmeans, kind)
                 self.layers["normed_counts"] = normed
                 self.obs["size_factors"] = sf
                 self.var["_normed_means"] = normed.mean(0)

@@ -39,6 +39,67 @@ def median_of_ratios(counts: np.ndarray):
     return counts / sf[:, None], sf
 
 
+def filtered_genes(logmeans: np.ndarray, fit_type: str = "ratio") -> np.ndarray:
+    """``DeseqDataSet.filtered_genes`` after ``fit_size_factors``: the genes held-out samples are normalised against
+    (dds.py:478-486).  Finite log means (preprocessing.py:54); for poscounts also above 0 (dds.py:663).  Never masked by control
+    genes."""
+    lm = np.asarray(logmeans)
+    keep = ~np.isinf(lm)
+    return keep & (lm > 0) if fit_type == "poscounts" else keep
+
+
+def size_factors_numpy(counts: np.ndarray, fit_type: str = "ratio", control=None):
+    """``fit_size_factors`` (dds.py:628-703) for ``"ratio"`` / ``"poscounts"`` in numpy, for backends without ``size_factors``.
+    ``control``: boolean mask of the control genes or None.  Returns (normed_counts, size_factors, logmeans)."""
+    counts = np.asarray(counts)
+    use = np.ones(counts.shape[1], dtype=bool) if control is None else np.asarray(control, dtype=bool)
+    with np.errstate(divide="ignore", invalid="ignore"), warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)  # np.median of an empty set: NaN, as in the reference
+        if fit_type == "poscounts":
+            lc = np.zeros_like(counts, dtype=float)
+            np.log(counts, out=lc, where=counts != 0)
+            lm = lc.mean(0)
+            use = use & filtered_genes(lm, "poscounts")
+            sf = np.array([np.exp(np.median(np.log(x[use & (x > 0)]) - lm[use & (x > 0)])) for x in counts])
+            sf = sf / np.exp(np.mean(np.log(sf)))
+        else:
+            lc = np.log(counts)
+            lm = lc.mean(0)
+            if np.isinf(lm).all():
+                raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
+            use = use & ~np.isinf(lm)
+            sf = np.exp(np.median(lc[:, use] - lm[use], axis=1))
+        return counts / sf[:, None], sf, lm
+
+
+def size_factor_kind(fit_type: str) -> int:
+    """``kind`` of pdq_size_factors_ex for a ``size_factors_fit_type`` of the drivers; "iterative" stays with the reference."""
+    from .inference import SF_KINDS
+
+    if fit_type == "iterative":
+        raise NotImplementedError("iterative size factors have no device implementation; fit them with the reference")
+    if fit_type not in SF_KINDS:
+        raise ValueError(f"size_factors_fit_type must be one of {sorted(SF_KINDS)}, got {fit_type!r}")
+    return SF_KINDS[fit_type]
+
+
+def check_size_factors(sf, counts, logmeans, fit_type="ratio", control=None):
+    """Raise for NaN size factors, naming the samples whose median had no entry: no usable gene, or for poscounts no positive count
+    in one.  ``counts`` (N, G) host counts in the gene order of ``logmeans`` and ``control``."""
+    if np.isfinite(sf).all():
+        return
+    usable = filtered_genes(logmeans, fit_type)
+    if control is not None:
+        usable = usable & control
+    counts = np.asarray(counts)
+    if fit_type == "poscounts":
+        bad = np.flatnonzero(~(counts[:, usable] > 0).any(1))
+    else:
+        bad = np.arange(counts.shape[0]) if not usable.any() else np.flatnonzero(~np.isfinite(sf))
+    raise ValueError(f"Size factors are NaN: sample(s) {bad.tolist()} have no usable gene ({fit_type}"
+                     + (", control genes" if control is not None else "") + ")")
+
+
 def lin_mu_branch(X: np.ndarray) -> bool:
     """True when #unique design rows == #columns: mu_hat comes from ``lin_reg_mu`` (dds.py:747-756)."""
     return len(np.unique(X, axis=0)) == X.shape[1]
@@ -314,9 +375,13 @@ class ResidentFit:
     """
 
     def __init__(self, ctx, X, size_factors, min_mu=0.5, min_disp=1e-8, max_disp=10.0, beta_tol=1e-8, comm=None,
-                 with_cooks=False, sort_genes=True):
+                 with_cooks=False, sort_genes=True, size_factors_fit_type="ratio", control_genes=None):
         from . import _lib
 
+        size_factor_kind(size_factors_fit_type)
+        # size factors fitted on the device when none are given (device_size_factors): the estimator, and the control genes as a
+        # boolean mask or integer positions over the uploaded genes in the caller's order
+        self.size_factors_fit_type, self.control_genes = size_factors_fit_type, control_genes
         self._lib_mod = _lib
         self.ctx = ctx
         self.lib = ctx.lib
@@ -363,16 +428,42 @@ class ResidentFit:
         self._eager_key = None
 
     def device_size_factors(self):
-        """Median-of-ratios size factors from the resident counts (preprocessing.py:31-102); rebuilds the design pack.
+        """Size factors from the resident counts -- median of ratios (preprocessing.py:31-102) or poscounts, over every gene or the
+        control genes (``size_factors_fit_type`` / ``control_genes``, dds.py:628-703); rebuilds the design pack.
         With gene shards the medians are over the LOCAL genes only -- pass global size factors in that case."""
+        from .inference import control_mask
+
+        c_d, kind = self._lib_mod.c_dptr, self.size_factors_fit_type
         d_sf = self._dev("sf", self.N * 8)
-        self.ctx.check(self.lib.pdq_size_factors_dev(self.ctx.h, self._lib_mod.c_dptr(self.d_counts), self.G, self.N, self.G,
-                                                     self._lib_mod.c_dptr(d_sf), None))
         sf = np.empty(self.N)
+        ctl = control_mask(self.control_genes, self.G)
+        if kind == "ratio" and ctl is None:
+            self.ctx.check(self.lib.pdq_size_factors_dev(self.ctx.h, c_d(self.d_counts), self.G, self.N, self.G, c_d(d_sf), None))
+            self.ctx.d2h(sf, d_sf)
+            self.ctx.sync()
+            if not np.isfinite(sf).all():
+                raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
+            self._set_size_factors(sf)
+            return sf
+        d_ctl = None
+        if ctl is not None:
+            ctl = ctl if self._perm is None else ctl[self._perm]  # device column j holds the caller's gene perm[j]
+            d_ctl = self._dev("sf_control", self.G)
+            self.ctx.h2d(d_ctl, ctl.astype(np.uint8))
+        d_lm = self._dev("sf_logmeans", self.G * 8)
+        self.ctx.check(self.lib.pdq_size_factors_ex_dev(self.ctx.h, c_d(self.d_counts), self.G, self.N, self.G, size_factor_kind(kind),
+                                                        c_d(d_ctl) if d_ctl else None, c_d(d_sf), c_d(d_lm)))
+        lm = np.empty(self.G)
         self.ctx.d2h(sf, d_sf)
+        self.ctx.d2h(lm, d_lm)
         self.ctx.sync()
-        if not np.isfinite(sf).all():
+        if kind == "ratio" and np.isinf(lm).all():
             raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
+        if not np.isfinite(sf).all():  # the error path only: the counts come back to name the samples
+            counts = np.empty((self.N, self.G), dtype=np.int64)
+            self.ctx.d2h(counts, self.d_counts)
+            self.ctx.sync()
+            check_size_factors(sf, counts, lm, kind, ctl)
         self._set_size_factors(sf)
         return sf
 

@@ -23,7 +23,8 @@ import warnings
 import numpy as np
 from scipy.stats import trim_mean
 
-from .pipeline import LN2, FitResult, fit_host, fit_shrink_prior_var, fit_trend, genewise_stage, lin_mu_branch, median_of_ratios
+from .pipeline import (LN2, FitResult, check_size_factors, filtered_genes, fit_host, fit_shrink_prior_var, fit_trend, genewise_stage,
+                       lin_mu_branch, size_factor_kind, size_factors_numpy)
 
 
 def n_or_more_replicates(X: np.ndarray, min_replicates: int) -> np.ndarray:
@@ -128,7 +129,7 @@ class Deseq2Results:
 def deseq2_results(counts, X, inference, contrast=None, size_factors=None, refit_cooks=True, min_replicates=7, cooks_filter=True,
                    independent_filter=True, alpha=0.05, lfc_null=0.0, alt_hypothesis=None, fit_type="parametric", min_mu=0.5,
                    min_disp=1e-8, max_disp=10.0, beta_tol=1e-8, shrink_coeff=None, shrink_adapt=True, keep_cooks=False,
-                   comm=None) -> Deseq2Results:
+                   comm=None, size_factors_fit_type="ratio", control_genes=None) -> Deseq2Results:
     """The reference's default analysis -- ``dds.deseq2()`` then ``DeseqStats(dds, contrast).summary()`` (and ``lfc_shrink`` when
     ``shrink_coeff`` is given) -- through ``inference``.  ``counts`` (N, G) non-negative integers, ``X`` (N, p) expanded design,
     ``contrast`` (p,) numeric contrast vector (default: last coefficient).
@@ -136,7 +137,11 @@ def deseq2_results(counts, X, inference, contrast=None, size_factors=None, refit
     ``comm`` (``sharding.TorchDistComm`` / ``NcclComm``): ``counts`` is this rank's gene shard and ``size_factors`` must be given.
     Everything per gene -- fits, Cook's distances, the outlier refit -- stays local; the three steps that look at ALL genes are
     exchanged: the dispersion trend / prior (inside ``fit_host``), the multiple-testing step (base means and p-values are
-    all-gathered, adjusted identically on every rank, and the local slice is kept) and the apeGLM prior scale."""
+    all-gathered, adjusted identically on every rank, and the local slice is kept) and the apeGLM prior scale.
+
+    ``size_factors_fit_type`` (``"ratio"`` or ``"poscounts"``) and ``control_genes`` (boolean mask or integer positions) select
+    the size-factor estimator when ``size_factors`` is not given (``DeseqDataSet(size_factors_fit_type=, control_genes=)``,
+    dds.py:584-711); anything but plain ratio goes through ``inference.size_factors``, or numpy for a backend without it."""
     from scipy.stats import f as f_dist
 
     counts = np.ascontiguousarray(counts, dtype=np.int64)
@@ -151,6 +156,8 @@ def deseq2_results(counts, X, inference, contrast=None, size_factors=None, refit
         raise ValueError(f"The alternative hypothesis being {alt_hypothesis}, please provide a positive lfc_null value (got {lfc_null}).")
     if comm is not None and size_factors is None:
         raise ValueError("gene shards: size factors are per sample and global over genes -- pass them in")
+    if size_factors is None and (size_factors_fit_type != "ratio" or control_genes is not None):
+        size_factors = _fit_size_factors(counts, inference, size_factors_fit_type, control_genes)[1]
     fit = fit_host(counts, X, inference, contrast=contrast, size_factors=size_factors, min_mu=min_mu, min_disp=min_disp, max_disp=max_disp,
                    beta_tol=beta_tol, fit_type=fit_type, lfc_null=lfc_null, alt_hypothesis=alt_hypothesis, comm=comm)
     max_disp = max(max_disp, N)
@@ -385,20 +392,27 @@ class VstFit:
         counts = np.ascontiguousarray(counts, dtype=np.int64)
         if self.logmeans is None:
             warnings.warn(_LEAK_WARNING, UserWarning, stacklevel=2)
-            sf = _median_of_ratios(counts, self.inference)[1]
+            sf = _fit_size_factors(counts, self.inference)[1]
         else:
             lm = np.where(self.filtered_genes, self.logmeans, -np.inf)
             sf = self.inference.size_factors(counts, logmeans=lm)[1]
         return self.inference.vst_transform(counts, sf, self.kind, self.coeffs)
 
 
-def _median_of_ratios(counts, inference):
-    """(normed counts, size factors, log means): on the backend when it has ``size_factors``, else numpy (preprocessing.py:31-102)."""
+def _fit_size_factors(counts, inference, fit_type="ratio", control_genes=None):
+    """(normed counts, size factors, log means) of ``fit_size_factors`` (dds.py:584-711): on the backend when it has
+    ``size_factors``, else numpy.  NaN size factors raise, naming the samples without a usable gene."""
+    from .inference import control_mask
+
+    size_factor_kind(fit_type)
+    ctl = control_mask(control_genes, counts.shape[1])
     if hasattr(inference, "size_factors"):
-        return inference.size_factors(counts, return_logmeans=True)
-    normed, sf = median_of_ratios(counts)
-    with np.errstate(divide="ignore"):
-        return normed, sf, np.log(counts).mean(0)
+        kw = {} if fit_type == "ratio" and ctl is None else {"fit_type": fit_type, "control_genes": ctl}
+        normed, sf, lm = inference.size_factors(counts, return_logmeans=True, **kw)
+    else:
+        normed, sf, lm = size_factors_numpy(counts, fit_type, ctl)
+    check_size_factors(sf, counts, lm, fit_type, ctl)
+    return normed, sf, lm
 
 
 def mean_dispersion(genewise: np.ndarray, min_disp: float) -> float:
@@ -408,12 +422,13 @@ def mean_dispersion(genewise: np.ndarray, min_disp: float) -> float:
 
 
 def vst(counts, X, inference, fit_type="parametric", use_design=False, size_factors=None, logmeans=None, min_mu=0.5, min_disp=1e-8,
-        max_disp=10.0, beta_tol=1e-8, transform=True) -> VstFit:
+        max_disp=10.0, beta_tol=1e-8, transform=True, size_factors_fit_type="ratio", control_genes=None) -> VstFit:
     """``DeseqDataSet.vst(use_design, fit_type)`` (dds.py:349-436) on bare arrays: median-of-ratios size factors unless
     ``size_factors`` are given (``logmeans`` then are the fit's, for :meth:`VstFit.transform`), genewise dispersions on an
     intercept-only design unless ``use_design`` (dds.py:713-797), the parametric trend loop with its fallback to the trimmed mean
     (dds.py:1199-1299), and the transform of every gene through ``inference.vst_transform``.  ``counts`` (N, G) non-negative
-    integers, ``X`` (N, p) the expanded design."""
+    integers, ``X`` (N, p) the expanded design.  ``size_factors_fit_type`` / ``control_genes``: the size-factor estimator, as in
+    :func:`deseq2_results`; ``filtered_genes`` (the genes held-out samples are normalised against) follows it."""
     if fit_type not in ("parametric", "mean"):
         raise NotImplementedError(f"Found fit_type '{fit_type}'. Expected 'parametric' or 'mean'.")
     if not hasattr(inference, "vst_transform"):
@@ -422,11 +437,11 @@ def vst(counts, X, inference, fit_type="parametric", use_design=False, size_fact
     N, G = counts.shape
     max_disp = max(max_disp, N)  # dds.py:312
     if size_factors is None:
-        normed, sf, logmeans = _median_of_ratios(counts, inference)
+        normed, sf, logmeans = _fit_size_factors(counts, inference, size_factors_fit_type, control_genes)
     else:
         sf = np.asarray(size_factors, dtype=float)
         normed = counts / sf[:, None]
-    filtered = None if logmeans is None else ~np.isinf(logmeans)
+    filtered = None if logmeans is None else filtered_genes(logmeans, size_factors_fit_type)
     if use_design:
         Xv = np.ascontiguousarray(X, dtype=np.float64)
         if fit_type == "mean":
@@ -446,28 +461,37 @@ def vst(counts, X, inference, fit_type="parametric", use_design=False, size_fact
 
 
 def vst_resident(inference, counts, X, fit_type="parametric", use_design=False, size_factors=None, logmeans=None, min_mu=0.5,
-                 min_disp=1e-8, max_disp=10.0, beta_tol=1e-8) -> VstFit:
+                 min_disp=1e-8, max_disp=10.0, beta_tol=1e-8, size_factors_fit_type="ratio", control_genes=None) -> VstFit:
     """:func:`vst` with the counts resident in HBM: they go up once, the size factors (median of ratios on the device unless
     given), the all-zero mask and the fit stage (steps 1-3 of ``ResidentFit.run`` and the trend, on a ``ResidentFit`` of the VST
     design over the non-zero genes, gathered on the device) run there, and ``pdq_vst_transform_dev`` transforms the full table
     in the caller's gene order; only ``vst_counts`` comes back.  Every other transfer is a per-sample or per-gene vector.
-    ``inference`` is a ``B200Inference`` (its context is used)."""
+    ``inference`` is a ``B200Inference`` (its context is used).  ``size_factors_fit_type`` / ``control_genes`` as in :func:`vst`."""
     from . import _lib
-    from .inference import VST_KINDS
+    from .inference import VST_KINDS, control_mask
     from .pipeline import ResidentFit
 
     if fit_type not in ("parametric", "mean"):
         raise NotImplementedError(f"Found fit_type '{fit_type}'. Expected 'parametric' or 'mean'.")
+    kind_code = size_factor_kind(size_factors_fit_type)
     ctx = inference._ops.ctx
     L, h, c_d = ctx.lib, ctx.h, _lib.c_dptr
     counts = np.ascontiguousarray(counts, dtype=np.int64)
     N, G = counts.shape
-    d_counts, d_sf, d_lm, d_sums, d_out = (ctx.malloc(n) for n in (N * G * 8, N * 8, G * 8, G * 8, N * G * 8))
+    ctl = control_mask(control_genes, G)
+    plain = size_factors_fit_type == "ratio" and ctl is None
+    d_counts, d_sf, d_lm, d_sums, d_out, d_ctl = (ctx.malloc(n) for n in (N * G * 8, N * 8, G * 8, G * 8, N * G * 8, G))
     rf = None
     try:
         ctx.h2d(d_counts, counts)  # the one (N, G) upload
         if size_factors is None:
-            ctx.check(L.pdq_size_factors_dev(h, c_d(d_counts), G, N, G, c_d(d_sf), c_d(d_lm)))
+            if plain:
+                ctx.check(L.pdq_size_factors_dev(h, c_d(d_counts), G, N, G, c_d(d_sf), c_d(d_lm)))
+            else:
+                if ctl is not None:
+                    ctx.h2d(d_ctl, ctl.astype(np.uint8))
+                ctx.check(L.pdq_size_factors_ex_dev(h, c_d(d_counts), G, N, G, kind_code,
+                                                    c_d(d_ctl) if ctl is not None else None, c_d(d_sf), c_d(d_lm)))
             sf, logmeans = np.empty(N), np.empty(G)
             ctx.d2h(sf, d_sf)
             ctx.d2h(logmeans, d_lm)
@@ -478,8 +502,12 @@ def vst_resident(inference, counts, X, fit_type="parametric", use_design=False, 
         sums = np.empty(G)
         ctx.d2h(sums, d_sums)
         ctx.sync()
-        if not np.isfinite(sf).all():
+        if plain and not np.isfinite(sf).all():
             raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
+        if size_factors is None and not plain:
+            if size_factors_fit_type == "ratio" and np.isinf(logmeans).all():
+                raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
+            check_size_factors(sf, counts, logmeans, size_factors_fit_type, ctl)
         nz = sums != 0  # counts are non-negative (dds.py:729-731)
         if use_design:
             Xv = np.ascontiguousarray(X, dtype=np.float64)
@@ -498,9 +526,9 @@ def vst_resident(inference, counts, X, fit_type="parametric", use_design=False, 
     finally:
         if rf is not None:
             rf.close()
-        for p in (d_counts, d_sf, d_lm, d_sums, d_out):
+        for p in (d_counts, d_sf, d_lm, d_sums, d_out, d_ctl):
             ctx.free(p)
-    filtered = None if logmeans is None else ~np.isinf(logmeans)
+    filtered = None if logmeans is None else filtered_genes(logmeans, size_factors_fit_type)
     return VstFit(sf, logmeans, filtered, kind, coeffs, _full(gw, nz, G), nz, out, inference)
 
 
