@@ -162,6 +162,14 @@ int pdq_wald_test(pdq_ctx* ctx, const double* X, int N, int p, const double* dis
                   const double* ridge, const double* contrast, double lfc_null, int alt,
                   double* pvalue_out, double* stat_out, double* se_out);
 
+/* Wald tests of K contrasts from fitted coefficients (ds.py:303-360 once per contrast; utils.py:718-811):
+ * mu = sf * exp(X lfc) on the device, X^T W X factored once per gene.  contrasts (K,p) row-major, lfc_null (K,)
+ * natural log, alt (K,) PDQ_ALT_* codes; outputs (K, ld_out).  K <= 0, an unknown alt or ld_out < G: PDQ_ERR_INVALID. */
+int pdq_wald_contrasts(pdq_ctx* ctx, const double* X, const double* size_factors, int N, int p,
+                       const double* disp /* (G,) */, const double* lfc /* (G,p) */, int G, const double* ridge /* (p,p) */,
+                       int K, const double* contrasts, const double* lfc_null, const int* alt,
+                       double* pvalue_out, double* stat_out, double* se_out, int64_t ld_out);
+
 /* Inference.fit_rough_dispersions  (inference.py:236-258; utils.py:814-853) */
 int pdq_fit_rough_dispersions(pdq_ctx* ctx, const double* normed_counts, int64_t ld, int N, int G,
                               const double* X, int p, double* alpha_out);

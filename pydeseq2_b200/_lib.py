@@ -73,6 +73,8 @@ _SIGNATURES = {
                                 C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, f64p, f64p]),
     "pdq_wald_test": (C.c_int, [c_ctx, f64p, C.c_int, C.c_int, f64p, f64p, f64p, C.c_int64, C.c_int, f64p, f64p,
                                 C.c_double, C.c_int, f64p, f64p, f64p]),
+    "pdq_wald_contrasts": (C.c_int, [c_ctx, f64p, f64p, C.c_int, C.c_int, f64p, f64p, C.c_int, f64p, C.c_int, f64p, f64p,
+                                     C.POINTER(C.c_int), f64p, f64p, f64p, C.c_int64]),
     "pdq_fit_rough_dispersions": (C.c_int, [c_ctx, f64p, C.c_int64, C.c_int, C.c_int, f64p, C.c_int, f64p]),
     "pdq_fit_moments_dispersions": (C.c_int, [c_ctx, f64p, C.c_int64, C.c_int, C.c_int, f64p, f64p, f64p]),
     "pdq_lin_reg_mu_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, C.c_double, c_dptr, C.c_int64]),

@@ -1357,6 +1357,60 @@ extern "C" int pdq_wald_test(pdq_ctx* c, const double* X, int N, int p, const do
     return call_end(c, nullptr, {});
 }
 
+// The test reads G x (p + 1) numbers instead of an (N, G) mu; the (K, G) outputs are the large transfer, so with page-locked
+// outputs they leave block by block through the gene-block pipeline while the next block computes.
+extern "C" int pdq_wald_contrasts(pdq_ctx* c, const double* X, const double* sf, int N, int p, const double* disp, const double* lfc,
+                                  int G, const double* ridge, int K, const double* contrasts, const double* lfc_null, const int* alt,
+                                  double* pv_out, double* stat_out, double* se_out, int64_t ld_out) {
+    CHECK_CTX(c);
+    if (!X || !sf || !disp || !lfc || !ridge || !contrasts || !lfc_null || !alt || !pv_out || !stat_out || !se_out || N <= 0 || p <= 0 ||
+        G <= 0 || K <= 0 || ld_out < G)
+        return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: bad arguments");
+    if (p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
+    std::vector<double> tab((size_t)K * (p + 2));  // rows [contrast | lfc_null | alt] (wald_contrasts_gene)
+    for (int k = 0; k < K; ++k) {
+        if (alt[k] < 0 || alt[k] > 4) return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: unknown alternative %d (contrast %d)", alt[k], k);
+        memcpy(&tab[(size_t)k * (p + 2)], contrasts + (size_t)k * p, (size_t)p * 8);
+        tab[(size_t)k * (p + 2) + p] = lfc_null[k];
+        tab[(size_t)k * (p + 2) + p + 1] = (double)alt[k];
+    }
+    pdq_design* d;
+    if (int e = cached_design(c, X, sf, N, p, &d)) return e;
+    const size_t kg = (size_t)K * G;
+    void *ddisp, *dlfc, *dtab, *dp, *ds, *dse;
+    if (int e = ensure(c, kBufC, (size_t)G * 8, &ddisp)) return e;
+    if (int e = ensure(c, kBufD, (size_t)G * p * 8, &dlfc)) return e;
+    if (int e = ensure(c, kBufMisc, tab.size() * 8, &dtab)) return e;
+    if (int e = ensure(c, kBufA, kg * 8, &dp)) return e;
+    if (int e = ensure(c, kBufB, kg * 8, &ds)) return e;
+    if (int e = ensure(c, kBufG, kg * 8, &dse)) return e;
+    Pipe pp;
+    if (int e = vec_h2d(c, ddisp, disp, (size_t)G * 8)) return e;
+    if (int e = vec_h2d(c, dlfc, lfc, (size_t)G * p * 8)) return e;
+    if (int e = vec_h2d(c, dtab, tab.data(), tab.size() * 8)) return e;
+    if (int e = pipe_begin(c, G, {pv_out, stat_out, se_out}, &pp)) return e;
+    double* outs[3] = {pv_out, stat_out, se_out};
+    void* douts[3] = {dp, ds, dse};
+    for (int b = 0; b < pp.nb; ++b) {
+        const int g0 = pp.g0(b), gb = pp.gb(b);
+        if (int e = done(c, launch_wald_contrasts(pp.cfg_for(b, N), d->d, (const double*)ddisp + g0, (const double*)dlfc + (size_t)g0 * p,
+                                                  gb, ridge, K, (const double*)dtab, (double*)dp + g0, (double*)ds + g0, (double*)dse + g0, G),
+                         "wald_contrasts"))
+            return e;
+        for (int i = 0; i < 3; ++i) {
+            if (pp.on) {
+                if (int e = cols_d2h(c, pp, b, outs[i], ld_out, douts[i], G, K, 8)) return e;
+            } else if (ld_out == G) {
+                if (int e = copy_d2h(c, outs[i], douts[i], kg * 8)) return e;
+            } else {
+                CU(c, cudaMemcpy2DAsync(outs[i], (size_t)ld_out * 8, douts[i], (size_t)G * 8, (size_t)G * 8, K, cudaMemcpyDeviceToHost,
+                                        c->stream));
+            }
+        }
+    }
+    return call_end(c, &pp, {});
+}
+
 extern "C" int pdq_fit_rough_dispersions(pdq_ctx* c, const double* normed, int64_t ld, int N, int G, const double* X, int p,
                                          double* alpha_out) {
     CHECK_CTX(c);

@@ -60,6 +60,15 @@ int launch_wald(const LaunchCfg& c, const DesignDev& d, const double* disp, cons
     PDQ_ROUTE(launch_wald, d.p, c, d, disp, lfc, mu, ld_mu, G, ridge, contrast, lfc_null, alt, pv, stat, se)
 }
 
+#define DECL_WALDK(sfx)                                                                                                \
+    int launch_wald_contrasts##sfx(const LaunchCfg&, const DesignDev&, const double*, const double*, int, const double*, int, \
+                                   const double*, double*, double*, double*, int64_t);
+PDQ_UNITS(DECL_WALDK)
+int launch_wald_contrasts(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
+                          const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
+    PDQ_ROUTE(launch_wald_contrasts, d.p, c, d, disp, lfc, G, ridge, K, tab, pv, stat, se, ld_out)
+}
+
 #define DECL_ROUGH(sfx) int launch_rough##sfx(const LaunchCfg&, const DesignDev&, const double*, int64_t, int, double*);
 PDQ_UNITS(DECL_ROUGH)
 int launch_rough(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {

@@ -244,65 +244,79 @@ struct WaldParams {
     int alt;
 };
 
-// the per-gene algebra once M = X^T W X (W from the caller's mu) is known: H = (M + ridge)^-1, SE, statistic, p-value
+// H = (M + ridge)^-1 for M = X^T W X (W from the caller's mu); `ridge` p x p row-major
 template <int P>
-PDQ_HD void wald_finish(const Group& grp, const Sym<P>& M, const WaldParams<P>& prm, const double* lfc, double* p_out,
-                        double* stat_out, double* se_out, bool valid) {
-    Sym<P> L = M, H;
+PDQ_HD void wald_inverse(const Sym<P>& M, const double* ridge, Sym<P>& H) {
+    Sym<P> L = M;
 PDQ_UNROLL_P
     for (int i = 0; i < P; ++i)
 PDQ_UNROLL_P
-        for (int j = 0; j <= i; ++j) L.a[tri(i, j)] += prm.ridge[i * P + j];
+        for (int j = 0; j <= i; ++j) L.a[tri(i, j)] += ridge[i * P + j];
     chol<P>(L);
     chol_inverse<P>(L, H);
+}
+
+// one contrast against that factor: SE = sqrt(c' H M H c), the statistic and the p-value of alternative `alt` (PDQ_ALT_*)
+template <int P>
+PDQ_HD void wald_contrast(const Sym<P>& M, const Sym<P>& H, const double (&contrast)[P], double lfc_null, int alt, const double* lfc,
+                          double& pv, double& stat, double& se) {
     double Hc[P], MHc[P];
-    sym_matvec<P>(H, prm.contrast, Hc);
+    sym_matvec<P>(H, contrast, Hc);
     sym_matvec<P>(M, Hc, MHc);
     double q = 0.0;
 PDQ_UNROLL_P
     for (int j = 0; j < P; ++j) q = fma(Hc[j], MHc[j], q);
-    const double se = sqrt(q);
+    se = sqrt(q);
     double b[P];
 PDQ_UNROLL_P
     for (int j = 0; j < P; ++j) b[j] = lfc[j];
-    const double t0 = prm.lfc_null;
-    double stat, pv;
+    const double t0 = lfc_null;
     // each variant applies the elementwise transform to every coefficient, then dots with the contrast
     auto greater = [&](double t, double& s, double& p) {
         s = 0.0;
 PDQ_UNROLL_P
-        for (int j = 0; j < P; ++j) s = fma(prm.contrast[j], fmax((b[j] - t) / se, 0.0), s);
+        for (int j = 0; j < P; ++j) s = fma(contrast[j], fmax((b[j] - t) / se, 0.0), s);
         p = norm_sf(s);
     };
     auto less = [&](double t, double& s, double& p) {
         s = 0.0;
 PDQ_UNROLL_P
-        for (int j = 0; j < P; ++j) s = fma(prm.contrast[j], fmin((b[j] - t) / se, 0.0), s);
+        for (int j = 0; j < P; ++j) s = fma(contrast[j], fmin((b[j] - t) / se, 0.0), s);
         p = norm_sf(fabs(s));
     };
-    if (prm.alt == 0) {
+    if (alt == 0) {
         double s = 0.0;
 PDQ_UNROLL_P
-        for (int j = 0; j < P; ++j) s = fma(prm.contrast[j], b[j] - t0, s);
+        for (int j = 0; j < P; ++j) s = fma(contrast[j], b[j] - t0, s);
         stat = s / se;
         pv = 2.0 * norm_sf(fabs(stat));
-    } else if (prm.alt == 1) {  // greaterAbs
+    } else if (alt == 1) {  // greaterAbs
         double s = 0.0;
 PDQ_UNROLL_P
-        for (int j = 0; j < P; ++j) s = fma(prm.contrast[j], sgn(b[j]) * fmax((fabs(b[j]) - t0) / se, 0.0), s);
+        for (int j = 0; j < P; ++j) s = fma(contrast[j], sgn(b[j]) * fmax((fabs(b[j]) - t0) / se, 0.0), s);
         stat = s;
         pv = 2.0 * norm_sf(fabs(s));
-    } else if (prm.alt == 2) {  // lessAbs
+    } else if (alt == 2) {  // lessAbs
         double sa, pa, sb, pb;
         greater(-fabs(t0), sa, pa);
         less(fabs(t0), sb, pb);
         stat = (fabs(sb) < fabs(sa)) ? sb : sa;  // min(sa, sb, key=abs): first wins ties
         pv = (pb > pa) ? pb : pa;                // max(pa, pb)
-    } else if (prm.alt == 3) {
+    } else if (alt == 3) {
         greater(t0, stat, pv);
     } else {
         less(t0, stat, pv);
     }
+}
+
+// the per-gene algebra once M = X^T W X is known: H = (M + ridge)^-1, then the one contrast of `prm`
+template <int P>
+PDQ_HD void wald_finish(const Group& grp, const Sym<P>& M, const WaldParams<P>& prm, const double* lfc, double* p_out,
+                        double* stat_out, double* se_out, bool valid) {
+    Sym<P> H;
+    wald_inverse<P>(M, prm.ridge, H);
+    double pv, stat, se;
+    wald_contrast<P>(M, H, prm.contrast, prm.lfc_null, prm.alt, lfc, pv, stat, se);
     if (valid && grp.si == 0) {
         *p_out = pv;
         *stat_out = stat;
@@ -322,6 +336,47 @@ PDQ_HD void wald_gene(const Group& grp, const DesignS& d, const WaldParams<P>& p
     });
     group_sum_sym<P>(grp, M);
     wald_finish<P>(grp, M, prm, lfc, p_out, stat_out, se_out, valid);
+}
+
+// Wald tests of K contrasts from fitted coefficients (ds.py:303-360 once per contrast).  mu = sf * exp(x'beta) is built per
+// sample -- the reference's exp(X @ LFC.T) * sf, as k_mu_from_lfc writes it -- so no (N, G) array is read; X^T W X is summed over
+// the group and factored ONCE.  M and H are then replicated in every lane, so lane si evaluates contrasts si, si + T, ...: K
+// contrasts cost ceil(K / T) rounds instead of K.  `tab` (K, P + 2) row-major: contrast, lfc_null, alt.  Outputs (K, ld_out).
+template <int P>
+PDQ_HD void wald_contrasts_gene(const Group& grp, const DesignS& d, const double* ridge, double disp, const double* lfc, int K,
+                                const double* tab, double* p_out, double* stat_out, double* se_out, int64_t ld_out, bool valid) {
+    double b[P];
+PDQ_UNROLL_P
+    for (int j = 0; j < P; ++j) b[j] = lfc[j];
+    Sym<P> M;
+    sym_zero<P>(M);
+    for (int n = grp.si; n < d.N; n += grp.T) {
+        double x[P];
+        load_x<P>(d, n, x);
+        double eta = 0.0;
+PDQ_UNROLL_P
+        for (int j = 0; j < P; ++j) eta = fma(x[j], b[j], eta);
+        const double m = d.sf[n * d.RS] * exp(eta);
+        sym_rank1<P>(M, m / fma(m, disp, 1.0), x);
+    }
+    group_sum_sym<P>(grp, M);
+    Sym<P> H;
+    wald_inverse<P>(M, ridge, H);
+    // Every lane runs the same ceil(K / T) rounds and skips its slot when it has no contrast there.  A per-lane trip count
+    // (k = si; k < K; k += T) gave wrong results from the second round on in the wide units (p = 9..16, ptxas -O1) on an H100.
+    for (int k0 = 0; k0 < K; k0 += grp.T) {
+        const int k = k0 + grp.si;
+        if (!valid || k >= K) continue;
+        const double* row = tab + (int64_t)k * (P + 2);
+        double c[P];
+PDQ_UNROLL_P
+        for (int j = 0; j < P; ++j) c[j] = row[j];
+        double pv, stat, se;
+        wald_contrast<P>(M, H, c, row[P], (int)row[P + 1], b, pv, stat, se);
+        p_out[k * ld_out] = pv;
+        stat_out[k * ld_out] = stat;
+        se_out[k * ld_out] = se;
+    }
 }
 
 // =============================================================================================

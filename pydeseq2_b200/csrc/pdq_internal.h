@@ -62,6 +62,9 @@ int launch_alpha_mle(const LaunchCfg&, const DesignDev&, const int64_t* counts, 
 int launch_wald(const LaunchCfg&, const DesignDev&, const double* disp, const double* lfc, const double* mu,
                 int64_t ld_mu, int G, const double* ridge, const double* contrast, double lfc_null, int alt,
                 double* pv, double* stat, double* se);
+// K contrasts from fitted coefficients: `ridge` p x p (host), `tab` (K, p + 2) device rows [contrast | lfc_null | alt]
+int launch_wald_contrasts(const LaunchCfg&, const DesignDev&, const double* disp, const double* lfc, int G, const double* ridge, int K,
+                          const double* tab, double* pv, double* stat, double* se, int64_t ld_out);
 int launch_rough(const LaunchCfg&, const DesignDev&, const double* normed, int64_t ld, int G, double* alpha);
 int launch_moments(const LaunchCfg&, const DesignDev&, const double* normed, int64_t ld, int G, double* alpha,
                    double* all_zero);

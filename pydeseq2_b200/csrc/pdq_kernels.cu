@@ -361,6 +361,29 @@ __global__ void __launch_bounds__(kBlock) k_wald(const __grid_constant__ WaldArg
 }
 
 template <int P>
+struct WaldContrastsArgs {
+    DesignView dv;
+    double ridge[P * P];
+    const double* tab;  // (K, P + 2): contrast, lfc_null, alt
+    const double *disp, *lfc;
+    int G, lgT, K;
+    double *pv, *stat, *se;  // (K, ld_out)
+    int64_t ld_out;
+};
+
+template <int P>
+__global__ void __launch_bounds__(kBlock) k_wald_contrasts(const __grid_constant__ WaldContrastsArgs<P> a) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const DesignS d = stage_design(a.dv, P, smem);
+    Group grp;
+    int g;
+    bool valid;
+    map_lanes(a.lgT, a.G, grp, g, valid);
+    wald_contrasts_gene<P>(grp, d, a.ridge, a.disp[g], a.lfc + (int64_t)g * P, a.K, a.tab, a.pv + g, a.stat + g, a.se + g, a.ld_out,
+                           valid);
+}
+
+template <int P>
 struct MomArgs {
     DesignView dv;
     SmallMat<P> pinv;
@@ -1309,6 +1332,22 @@ int PDQ_TUFN(launch_wald)(const LaunchCfg& c, const DesignDev& d, const double* 
         a.pv = pv; a.stat = stat; a.se = se;
         if (int e = prep(k_wald<P>, d.smem_bytes)) return e;
         k_wald<P><<<grid_for(G, c.lgT), kBlock, d.smem_bytes, c.stream>>>(a);
+    });
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int PDQ_TUFN(launch_wald_contrasts)(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G,
+                                    const double* ridge, int K, const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
+    PDQ_DISPATCH_P(d.p, {
+        WaldContrastsArgs<P> a;
+        a.dv = DesignView{d.pack, d.N, d.staged ? (int)(d.smem_bytes - 16) : 0};
+        for (int i = 0; i < P * P; ++i) a.ridge[i] = ridge[i];
+        a.tab = tab;
+        a.disp = disp; a.lfc = lfc; a.G = G; a.lgT = c.lgT; a.K = K;
+        a.pv = pv; a.stat = stat; a.se = se; a.ld_out = ld_out;
+        if (int e = prep(k_wald_contrasts<P>, d.smem_bytes)) return e;
+        k_wald_contrasts<P><<<grid_for(G, c.lgT), kBlock, d.smem_bytes, c.stream>>>(a);
     });
     if (int e = check_launch()) return e;
     return 1;

@@ -157,6 +157,14 @@ class _CudaOps:
                                               G, as_f64p(ridge), as_f64p(contrast), lfc_null, alt, as_f64p(pv),
                                               as_f64p(stat), as_f64p(se)))
 
+    def wald_contrasts(self, X, sf, N, p, disp, lfc, G, ridge, K, contrasts, lfc_null, alt, pv, stat, se, ld_out):
+        """pdq_wald_contrasts: `alt` int32 (K,), outputs (K, ld_out)."""
+        self._io((X, sf, disp, lfc, contrasts), (pv, stat, se))
+        self.ctx.check(self.lib.pdq_wald_contrasts(self.ctx.h, as_f64p(X), as_f64p(sf), N, p, as_f64p(disp), as_f64p(lfc), G,
+                                                   as_f64p(ridge), K, as_f64p(contrasts), as_f64p(lfc_null),
+                                                   alt.ctypes.data_as(C.POINTER(C.c_int)), as_f64p(pv), as_f64p(stat), as_f64p(se),
+                                                   ld_out))
+
     def rough(self, normed, ld, N, G, X, p, out):
         self._io((normed, X), (out,))
         self.ctx.check(self.lib.pdq_fit_rough_dispersions(self.ctx.h, as_f64p(normed), ld, N, G, as_f64p(X), p, as_f64p(out)))
@@ -238,7 +246,7 @@ class B200Inference(_InferenceBase):
         Record every plugin call in ``self.trace`` (method, milliseconds, bytes requested host→device / device→host).
     """
 
-    _TRACED = ("lin_reg_mu", "irls", "alpha_mle", "wald_test", "fit_rough_dispersions", "fit_moments_dispersions",
+    _TRACED = ("lin_reg_mu", "irls", "alpha_mle", "wald_test", "wald_tests", "fit_rough_dispersions", "fit_moments_dispersions",
                "dispersion_trend_gamma_glm", "lfc_shrink_nbinom_glm", "size_factors", "calculate_cooks")
 
     def __init__(self, device: int = 0, n_cpus: int | None = None, lanes_per_gene: int = 0, _ops=None, trace: bool = False,
@@ -357,6 +365,55 @@ class B200Inference(_InferenceBase):
             self._ops.wald_test(X, N, p, disp, lfc, mu, ld_mu, G, ridge, contrast, float(np.asarray(lfc_null)),
                                 ALT_CODES[alt_hypothesis], pv, stat, se)
         return pv, stat, se
+
+    def wald_tests(self, design_matrix, size_factors, disp, lfc, contrasts, ridge_factor=None, lfc_null=0.0, alt_hypothesis=None):
+        """Wald tests of K contrasts on one fit -- ``DeseqStats.run_wald_test`` (ds.py:303-360) once per contrast -- in one call.
+        mu = size_factors * exp(X lfc) is built on the device, so only the coefficients and dispersions travel, and X^T W X is
+        factored once per gene.  ``contrasts`` (K, p), or (p,) for one contrast; ``lfc_null`` (natural log, as for
+        :meth:`wald_test`) and ``alt_hypothesis`` are scalars or length-K sequences; ``ridge_factor`` defaults to diag(1e-6).
+        Returns (pvalue, stat, se), each (K, G), or (G,) for a 1-D contrast.  Genes whose LFC row or dispersion is not finite are
+        not sent: their outputs are NaN, as NaN propagates through the reference's mu."""
+        X = np.ascontiguousarray(_f64(design_matrix, "design_matrix", 2))
+        sf = np.ascontiguousarray(_f64(size_factors, "size_factors", 1))
+        disp = np.ascontiguousarray(_f64(disp, "disp", 1))
+        lfc = np.ascontiguousarray(_f64(lfc, "lfc", 2))
+        cs = _f64(contrasts, "contrasts")
+        single = cs.ndim == 1
+        cs = np.ascontiguousarray(cs[None, :] if single else cs)
+        N, p = X.shape
+        G = lfc.shape[0]
+        self._check_design(X, N, sf)
+        if cs.ndim != 2 or cs.shape[1] != p or cs.shape[0] == 0:
+            raise ValueError(f"contrasts must be (K, {p}) or ({p},), got shape {np.shape(contrasts)}")
+        K = cs.shape[0]
+        if lfc.shape != (G, p) or disp.shape != (G,):
+            raise ValueError("wald_tests arguments disagree on the number of genes/coefficients")
+        ridge = np.diag(np.repeat(1e-6, p)) if ridge_factor is None else np.ascontiguousarray(_f64(ridge_factor, "ridge_factor", 2))
+        if ridge.shape != (p, p):
+            raise ValueError(f"ridge_factor must be ({p}, {p}), got shape {ridge.shape}")
+        alts = list(alt_hypothesis) if isinstance(alt_hypothesis, (list, tuple, np.ndarray)) else [alt_hypothesis] * K
+        nulls = np.asarray(lfc_null, dtype=np.float64)
+        if len(alts) != K or nulls.ndim > 1 or (nulls.ndim == 1 and nulls.shape[0] != K):
+            raise ValueError(f"lfc_null and alt_hypothesis must be scalars or have one entry per contrast ({K})")
+        for a in alts:
+            if a not in ALT_CODES:
+                raise KeyError(a)  # same failure mode as the dict lookup at utils.py:798-803
+        codes = np.array([ALT_CODES[a] for a in alts], dtype=np.int32)
+        nulls = np.ascontiguousarray(np.broadcast_to(nulls, (K,)))
+        ok = np.isfinite(disp) & np.isfinite(lfc).all(axis=1)
+        idx = None if ok.all() else np.flatnonzero(ok)
+        if idx is not None:
+            disp, lfc = np.ascontiguousarray(disp[idx]), np.ascontiguousarray(lfc[idx])
+        Gs = disp.shape[0]
+        outs = [self._ops.empty((K, Gs)) for _ in range(3)]
+        if Gs:
+            self._ops.wald_contrasts(X, sf, N, p, disp, lfc, Gs, ridge, K, cs, nulls, codes, *outs, Gs)
+        if idx is not None:
+            full = [np.full((K, G), np.nan) for _ in range(3)]
+            for f, o in zip(full, outs):
+                f[:, idx] = o
+            outs = full
+        return tuple(o[0] for o in outs) if single else tuple(outs)
 
     # ------------------------------------------------------------------ a5: inference.py:236-281
     def fit_rough_dispersions(self, normed_counts, design_matrix):  # noqa: D102

@@ -1,6 +1,6 @@
 """The wiring a PyDESeq2 maintainer adds for the steps that are NOT behind the ``Inference`` plugin API but have a device
-implementation here (SURVEY.md §8 f-1, f-2): Cook's distances, median-of-ratios size factors and the variance-stabilising
-transform (``vst()`` / ``vst_transform(counts)``).
+implementation here (SURVEY.md §8 f-1, f-2): Cook's distances, median-of-ratios size factors, the variance-stabilising
+transform (``vst()`` / ``vst_transform(counts)``) and the Wald test of a contrast from the fitted coefficients.
 
 ``pydeseq2`` is imported lazily -- this module is only usable where the reference package is installed::
 
@@ -102,3 +102,44 @@ def b200_dataset_class(all_size_factors=False):
             return inf.vst_transform(counts, sf, kind, coeffs)
 
     return B200DeseqDataSet
+
+
+def b200_stats_class():
+    """Returns a ``DeseqStats`` subclass whose ``run_wald_test`` (ds.py:303-360) sends the fit's coefficients, dispersions, size
+    factors and the contrast to ``inference.wald_tests``: mu is built on the device instead of as an (N, G) host array per
+    contrast.  The outputs and the override for genes whose replaced counts became all zero are the reference's.  A backend
+    without ``wald_tests``, or a dataset without size factors, runs the reference's own method::
+
+        DeseqStats = b200_stats_class()
+        for c in contrasts:                                  # one fit, any number of comparisons
+            ds = DeseqStats(dds, contrast=c, inference=B200Inference(device=0))
+            ds.summary()
+    """
+    import sys
+
+    import pandas as pd
+    from pydeseq2.ds import DeseqStats
+
+    class B200DeseqStats(DeseqStats):
+        def run_wald_test(self):  # ds.py:303-360
+            if not hasattr(self.inference, "wald_tests") or "size_factors" not in self.dds.obs:
+                return super().run_wald_test()
+            if self.shrunk_LFCs and not self.quiet:
+                print("Note: running Wald test on shrunk LFCs. Some sequencing datasets show better performance with the testing "
+                      "separated from the use of the LFC prior.", file=sys.stderr)
+            p = self.design_matrix.shape[1]
+            ridge = np.diag(1 / self.prior_LFC_var**2) if self.prior_LFC_var is not None else np.diag(np.repeat(1e-6, p))
+            pv, stat, se = self.inference.wald_tests(self.design_matrix.values, self.dds.obs["size_factors"].values,
+                                                     self.dds.var["dispersions"].values, self.LFC.values,
+                                                     np.asarray(self.contrast_vector, dtype=float), ridge,
+                                                     np.log(2) * self.lfc_null, self.alt_hypothesis)
+            self.p_values = pd.Series(pv, index=self.dds.var_names)
+            self.statistics = pd.Series(stat, index=self.dds.var_names)
+            self.SE = pd.Series(se, index=self.dds.var_names)
+            if self.dds.refit_cooks and self.dds.var["replaced"].sum() > 0:
+                self.SE.loc[self.dds.new_all_zeroes_genes] = 0.0
+                self.statistics.loc[self.dds.new_all_zeroes_genes] = 0.0
+                self.p_values.loc[self.dds.new_all_zeroes_genes] = 1.0
+            return None
+
+    return B200DeseqStats

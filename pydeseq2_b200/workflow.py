@@ -362,6 +362,91 @@ def _full(v, nz, G):
     return out
 
 
+# --------------------------------------------------------------------------------------- more contrasts on one fit
+def wald_tests_numpy(X, size_factors, disp, lfc, contrasts, ridge, lfc_null, alts):
+    """``utils.wald_test`` (utils.py:718-811) for every gene and each of K contrasts, with mu = sf * exp(X lfc) (ds.py:320-324),
+    for backends without ``wald_tests``.  ``lfc_null`` (K,) natural log, ``alts`` K alternatives.  Returns (K, G) p-values,
+    statistics and standard errors; genes with a non-finite LFC row or dispersion get NaN."""
+    from scipy.stats import norm
+
+    K, G = len(contrasts), lfc.shape[0]
+    pv, stat, se = (np.full((K, G), np.nan) for _ in range(3))
+    ok = np.isfinite(disp) & np.isfinite(lfc).all(axis=1)
+    b = lfc[ok]
+    mu = np.exp(X @ b.T) * size_factors[:, None]
+    W = mu / (1 + mu * disp[ok][None, :])
+    M = np.einsum("ni,ng,nj->gij", X, W, X)
+    H = np.linalg.inv(M + ridge)
+    for k, (c, t, alt) in enumerate(zip(contrasts, lfc_null, alts)):
+        Hc = H @ c
+        s = np.sqrt(np.einsum("gi,gij,gj->g", Hc, M, Hc))[:, None]
+        greater = lambda t: (np.fmax((b - t) / s, 0) @ c, norm.sf(np.fmax((b - t) / s, 0) @ c))  # noqa: E731
+        less = lambda t: (np.fmin((b - t) / s, 0) @ c, norm.sf(np.abs(np.fmin((b - t) / s, 0) @ c)))  # noqa: E731
+        if alt is None:
+            st = (b - t) @ c / s[:, 0]
+            p = 2 * norm.sf(np.abs(st))
+        elif alt == "greaterAbs":
+            st = (np.sign(b) * np.fmax((np.abs(b) - t) / s, 0)) @ c
+            p = 2 * norm.sf(np.abs(st))
+        elif alt == "lessAbs":
+            (sa, pa), (sb, pb) = greater(-abs(t)), less(abs(t))
+            st, p = np.where(np.abs(sb) < np.abs(sa), sb, sa), np.maximum(pa, pb)
+        elif alt == "greater":
+            st, p = greater(t)
+        else:
+            st, p = less(t)
+        pv[k, ok], stat[k, ok], se[k, ok] = p, st, s[:, 0]
+    return pv, stat, se
+
+
+def deseq2_stats(res: Deseq2Results, X, inference, contrasts, lfc_null=0.0, alt_hypothesis=None, cooks_filter=True,
+                 independent_filter=True, alpha=0.05, prior_lfc_var=None) -> list[Deseq2Results]:
+    """``DeseqStats(dds, contrast).summary()`` for each row of ``contrasts`` (K, p) -- or one (p,) contrast -- on the fit that
+    :func:`deseq2_results` or :func:`deseq2_results_resident` returned: the LFCs, dispersions, size factors, Cook's outliers and
+    the outlier refit are the fit's and are not recomputed; only the Wald test depends on the contrast (ds.py:303-360), and all K
+    run in ONE ``inference.wald_tests`` call (a numpy restatement for backends without it).  ``lfc_null`` (log2, as for the
+    drivers) and ``alt_hypothesis`` are scalars or one per contrast; ``prior_lfc_var`` (p,) sets the ridge diag(1 / var^2)
+    (ds.py:327-330).  Genes whose replaced counts became all zero get se 0, stat 0, p 1 (ds.py:355-360).  Returns one
+    :class:`Deseq2Results` per contrast, sharing every field but the results-table columns with ``res``."""
+    import dataclasses
+
+    if res.shrink_prior_scale is not None:
+        raise ValueError("deseq2_stats needs the fit's MLE LFCs; this result holds apeGLM-shrunk LFCs (shrink_coeff)")
+    X = np.ascontiguousarray(X, dtype=np.float64)
+    p = X.shape[1]
+    cs = np.asarray(contrasts, dtype=float)
+    cs = cs[None, :] if cs.ndim == 1 else cs
+    if cs.ndim != 2 or cs.shape[1] != p or cs.shape[0] == 0 or res.lfc.shape[1] != p:
+        raise ValueError(f"contrasts must be (K, {p}) or ({p},) for a fit with {res.lfc.shape[1]} coefficients, got shape {np.shape(contrasts)}")
+    K = cs.shape[0]
+    alts = list(alt_hypothesis) if isinstance(alt_hypothesis, (list, tuple, np.ndarray)) else [alt_hypothesis] * K
+    nulls = np.asarray(lfc_null, dtype=float)
+    if len(alts) != K or nulls.ndim > 1 or (nulls.ndim == 1 and nulls.shape[0] != K):
+        raise ValueError(f"lfc_null and alt_hypothesis must be scalars or have one entry per contrast ({K})")
+    nulls = np.broadcast_to(nulls, (K,))
+    for a, t in zip(alts, nulls):
+        if t < 0 and a in ("greaterAbs", "lessAbs"):
+            raise ValueError(f"The alternative hypothesis being {a}, please provide a positive lfc_null value (got {t}).")
+    ridge = np.diag(np.repeat(1e-6, p)) if prior_lfc_var is None else np.diag(1 / np.asarray(prior_lfc_var, dtype=float) ** 2)
+    if hasattr(inference, "wald_tests"):
+        pv, stat, se = inference.wald_tests(X, res.size_factors, res.dispersions, res.lfc, cs, ridge, LN2 * nulls, alts)
+    else:
+        for a in alts:
+            if a not in (None, "greaterAbs", "lessAbs", "greater", "less"):
+                raise KeyError(a)
+        pv, stat, se = wald_tests_numpy(X, res.size_factors, res.dispersions, res.lfc, cs, ridge, LN2 * nulls, alts)
+    new_zero = res.replaced & ~res.refitted
+    out = []
+    for k in range(K):
+        pk, sk, ek = np.array(pv[k]), np.array(stat[k]), np.array(se[k])
+        ek[new_zero], sk[new_zero], pk[new_zero] = 0.0, 0.0, 1.0
+        if cooks_filter:
+            pk[res.cooks_outlier] = np.nan
+        padj = _adjust(res.base_mean, pk, independent_filter, alpha)
+        out.append(dataclasses.replace(res, log2_fold_change=res.lfc @ cs[k] / LN2, lfc_se=ek / LN2, stat=sk, pvalue=pk, padj=padj))
+    return out
+
+
 # --------------------------------------------------------------------------------------- variance-stabilising transform
 _LEAK_WARNING = ("The size factors were fitted iteratively. They will be re-computed with the counts to be transformed. In a "
                  "train/test setting with a downstream task, this would result in a leak of data from test to train set.")
