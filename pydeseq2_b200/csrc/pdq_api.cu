@@ -467,7 +467,6 @@ extern "C" void pdq_graph_destroy(pdq_ctx* c, pdq_graph* g) {
 }
 
 // --------------------------------------------------------------------------------------------- design pack
-// `offsets`: `sf` holds LOG size factors (the apeGLM call receives them in that form, and exp/log is not the identity in FP64)
 static int design_create(pdq_ctx* c, const double* X, const double* sf, bool offsets, int N, int p, pdq_design** out) {
     if (!c || !X || !out || N <= 0 || p < 1) return fail(c, PDQ_ERR_INVALID, "pdq_design_create: bad arguments");
     if (p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
@@ -476,11 +475,13 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
     DesignDev& dd = d->d;
     dd.N = N;
     dd.p = p;
-    dd.RS = (p + 3) & ~1;  // row stride of the pack in doubles (design_row_stride, pdq_gene.cuh)
+    dd.RS = design_row_stride(p);
+    std::vector<double> pack;
+    dd.s_mean_inv = design_pack(X, sf, offsets, N, p, pack);
     // Staging limit: a pack of up to 40 KB leaves room for four blocks per SM next to the math table and the per-gene tables of
     // the two heavy kernels; larger packs (N > ~1 280 at p = 2, ~850 at p = 3) are read from global memory, where they live in
     // L1 / L2 (every warp walks the same rows), so the number of samples is not bounded by shared memory.
-    const size_t pack_bytes = (size_t)(N + 1) * dd.RS * 8;  // N sample rows + the row of column maxima
+    const size_t pack_bytes = pack.size() * 8;
     size_t stage_max = 40 * 1024;
     if (const char* e = getenv("PDQ_STAGE_MAX_BYTES")) stage_max = (size_t)atoll(e);  // tuning hook
     dd.staged = pack_bytes <= stage_max && pack_bytes + 16 <= kMaxDynSmem / 2;
@@ -501,21 +502,6 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
             return fail(c, PDQ_ERR_CUDA, "cudaMalloc/cudaMemcpy(cell plan) failed");
         }
     }
-    std::vector<double> pack((size_t)(N + 1) * dd.RS, 0.0);
-    double inv_sum = 0.0;
-    for (int n = 0; n < N; ++n) {
-        double* row = pack.data() + (size_t)n * dd.RS;
-        for (int j = 0; j < p; ++j) {
-            row[j] = X[(size_t)n * p + j];
-            double& mx = pack[(size_t)N * dd.RS + j];
-            mx = !(fabs(row[j]) <= mx) ? fabs(row[j]) : mx;  // NaN propagates into the bound
-        }
-        const double s = sf ? (offsets ? exp(sf[n]) : sf[n]) : 1.0;
-        row[p] = s;
-        row[p + 1] = (sf && offsets) ? sf[n] : log(s);
-        inv_sum += 1.0 / s;
-    }
-    dd.s_mean_inv = inv_sum / N;
     if (cudaMalloc((void**)&dd.pack, pack.size() * 8) != cudaSuccess) {
         cudaFree(dd.cell_plan);
         delete d;
@@ -1367,13 +1353,9 @@ extern "C" int pdq_wald_contrasts(pdq_ctx* c, const double* X, const double* sf,
         G <= 0 || K <= 0 || ld_out < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: bad arguments");
     if (p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
-    std::vector<double> tab((size_t)K * (p + 2));  // rows [contrast | lfc_null | alt] (wald_contrasts_gene)
-    for (int k = 0; k < K; ++k) {
-        if (alt[k] < 0 || alt[k] > 4) return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: unknown alternative %d (contrast %d)", alt[k], k);
-        memcpy(&tab[(size_t)k * (p + 2)], contrasts + (size_t)k * p, (size_t)p * 8);
-        tab[(size_t)k * (p + 2) + p] = lfc_null[k];
-        tab[(size_t)k * (p + 2) + p + 1] = (double)alt[k];
-    }
+    std::vector<double> tab((size_t)K * (p + 2));
+    if (const int k = wald_contrast_table(K, p, contrasts, lfc_null, alt, tab.data()); k >= 0)
+        return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: unknown alternative %d (contrast %d)", alt[k], k);
     pdq_design* d;
     if (int e = cached_design(c, X, sf, N, p, &d)) return e;
     const size_t kg = (size_t)K * G;

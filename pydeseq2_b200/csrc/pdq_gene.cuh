@@ -12,6 +12,7 @@
 #pragma once
 
 #include "pdq_fast.cuh"
+#include "pdq_host_linalg.h"
 #include "pdq_math.cuh"
 
 #ifndef PDQ_PREFETCH
@@ -107,11 +108,7 @@ struct Group {
     }
 };
 
-// staged design pack (shared memory on the device), ROW-major: row n = [ x_n0 .. x_n,p-1 | sf_n | log sf_n | pad ], RS doubles
-// per row (p + 2 rounded up to even, so every row is 16-byte aligned: a sample's design row + size factor is one or two
-// 128-bit shared-memory reads at immediate offsets from one walking pointer).  `sf` / `lsf` = X + p / X + p + 1, indexed [n * RS].
-// Row N (one past the samples) holds the column maxima max_n |x_nj| (used to bound |x'beta| once per sweep).
-constexpr int design_row_stride(int p) { return (p + 3) & ~1; }
+// staged design pack (shared memory on the device; layout: design_pack): `sf` / `lsf` = X + p / X + p + 1, indexed [n * RS]
 struct DesignS {
     const double* X;
     const double* sf;

@@ -1,5 +1,5 @@
-// pdq_host_linalg.h -- host-only design-matrix preprocessing (hoisted out of the per-gene work:
-// the reference recomputes matrix_rank / QR of the SAME X for every gene, utils.py:349-352).
+// pdq_host_linalg.h -- host-only design-matrix preprocessing and input packing, shared by the C ABI and the host emulator (hoisted
+// out of the per-gene work: the reference recomputes matrix_rank / QR of the SAME X for every gene, utils.py:349-352).
 #pragma once
 
 #include <math.h>
@@ -12,6 +12,41 @@
 #endif
 
 namespace pdq {
+
+// Design pack of X (N x p; DesignS, pdq_gene.cuh), ROW-major: row n = [ x_n0 .. x_n,p-1 | sf_n | log sf_n | pad ] of RS = p + 2
+// rounded up to even doubles (16-byte aligned rows: a sample's design row + size factor is one or two 128-bit shared-memory reads),
+// then row N of the column maxima max_n |x_nj| (to bound |x'beta| once per sweep).  `sf` NULL = all ones; `offsets`: `sf` holds LOG
+// size factors (the apeGLM call receives them so, and exp/log is not the identity in FP64).  Returns mean(1 / sf) (utils.py:880).
+constexpr int design_row_stride(int p) { return (p + 3) & ~1; }
+inline double design_pack(const double* X, const double* sf, bool offsets, int N, int p, std::vector<double>& pack) {
+    const int RS = design_row_stride(p);
+    pack.assign((size_t)(N + 1) * RS, 0.0);
+    double inv_sum = 0.0;
+    for (int n = 0; n < N; ++n) {
+        double* row = pack.data() + (size_t)n * RS;
+        for (int j = 0; j < p; ++j) {
+            row[j] = X[(size_t)n * p + j];
+            double& mx = pack[(size_t)N * RS + j];
+            mx = !(fabs(row[j]) <= mx) ? fabs(row[j]) : mx;  // NaN propagates into the bound
+        }
+        const double s = sf ? (offsets ? exp(sf[n]) : sf[n]) : 1.0;
+        row[p] = s;
+        row[p + 1] = (sf && offsets) ? sf[n] : log(s);
+        inv_sum += 1.0 / s;
+    }
+    return inv_sum / N;
+}
+
+// wald_contrasts_gene's (K, p + 2) rows [contrast | lfc_null | alt]; returns the first contrast whose alternative is not 0..4, or -1
+inline int wald_contrast_table(int K, int p, const double* contrasts, const double* lfc_null, const int* alt, double* tab) {
+    for (int k = 0; k < K; ++k) {
+        if (alt[k] < 0 || alt[k] > 4) return k;
+        memcpy(tab + (size_t)k * (p + 2), contrasts + (size_t)k * p, (size_t)p * 8);
+        tab[(size_t)k * (p + 2) + p] = lfc_null[k];
+        tab[(size_t)k * (p + 2) + p + 1] = (double)alt[k];
+    }
+    return -1;
+}
 
 // One-sided Jacobi SVD of X (N x p, p <= 8): the right singular vectors V and singular values give
 //   rank(X)   with numpy.linalg.matrix_rank's tolerance  s_max * max(N, p) * eps     (utils.py:349)

@@ -8,11 +8,8 @@
 
 namespace pdq {
 
-// Device-resident design pack (DESIGN.md §2):
-//   pack = N rows of [ x_n0 .. x_n,p-1 | sf_n | log sf_n | pad ]  float64, RS = p + 2 rounded up to even doubles per row,
-// so that rows are 16-byte aligned and `cp.async.bulk` (TMA 1-D bulk copy, 16-byte granularity) stages it into shared memory.
 struct DesignDev {
-    double* pack;       // device
+    double* pack;       // device; layout: design_pack (pdq_host_linalg.h), DESIGN.md §2
     int N, RS, p;
     int full_rank;      // np.linalg.matrix_rank(X) == p  (utils.py:349)
     int few_rows;       // X has at most 16 distinct rows (categorical design): k_irls reuses exp(x'beta) across equal rows

@@ -524,12 +524,7 @@ class B200Inference(_InferenceBase):
                 return counts / sf[:, None], sf
         sf = np.empty(N)
         logmeans = np.empty(G) if return_logmeans else None  # what deseq2_norm_fit returns (preprocessing.py:31-59)
-        try:
-            self._ops.size_factors(counts, ld, N, G, sf, logmeans)
-        except TypeError:  # an ops object without the logmeans output (test emulator)
-            self._ops.size_factors(counts, ld, N, G, sf)
-            with np.errstate(divide="ignore"):
-                logmeans = np.log(counts).mean(0) if return_logmeans else None
+        self._ops.size_factors(counts, ld, N, G, sf, logmeans)
         if not np.isfinite(sf).all():
             raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
         if return_logmeans:

@@ -7,7 +7,7 @@ OUT = os.path.join(HERE, "_build", "libpdq_emu.so")
 SRC = os.path.join(HERE, "pdq_emu.cpp")
 DEPS = [SRC] + [os.path.join(HERE, "..", "..", "pydeseq2_b200", "csrc", f)
                 for f in ("pdq_gene.cuh", "pdq_math.cuh", "pdq_host_linalg.h", "pdq_trend.cuh", "pdq_fast.cuh", "pdq_shrink.cuh",
-                          "pdq_tables.h")] + [os.path.join(HERE, "..", "gpu_probe", "math_ops.h")]
+                          "pdq_tables.h", "pdq_vst.cuh")] + [os.path.join(HERE, "..", "gpu_probe", "math_ops.h")]
 
 
 def build(force=False, defines=None):

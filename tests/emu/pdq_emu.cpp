@@ -1,9 +1,10 @@
 // pdq_emu.cpp -- HOST EMULATOR of the device per-gene routines.  TEST INFRASTRUCTURE ONLY.
 //
-// Compiles pydeseq2_b200/csrc/pdq_gene.cuh (the exact source the sm_90a kernels are built from)
-// with g++, one "lane" per gene (T = 1, Group::sum is the identity), so that the CPU test-suite can
+// Compiles pydeseq2_b200/csrc/pdq_gene.cuh, pdq_trend.cuh, pdq_shrink.cuh and pdq_vst.cuh (the exact sources the sm_90a kernels
+// are built from) with g++, one "lane" per gene (T = 1, Group::sum is the identity), so that the CPU test-suite can
 // check the algorithmic content of the kernels -- IRLS control flow, the bounded root search for
-// the dispersion, Cholesky algebra, special functions -- against the oracle without a GPU.
+// the dispersion, Cholesky algebra, special functions, size factors, the vst, Wald tests of K contrasts -- against the oracle
+// without a GPU.  The design pack and the contrast table are written by the product's own host code (pdq_host_linalg.h).
 // It is built by tests/emu/build.py into tests/emu/_build/ and loaded only by tests/; the product
 // (pydeseq2_b200) never loads it and has no CPU fallback.
 //
@@ -26,6 +27,7 @@ extern long g_emu_irls_sweeps;
 #include "../../pydeseq2_b200/csrc/pdq_host_linalg.h"
 #include "../../pydeseq2_b200/csrc/pdq_trend.cuh"
 #include "../../pydeseq2_b200/csrc/pdq_shrink.cuh"
+#include "../../pydeseq2_b200/csrc/pdq_vst.cuh"
 #include "../gpu_probe/math_ops.h"
 
 long g_emu_alpha_evals = 0;
@@ -129,26 +131,30 @@ struct Pack {
     double s_mean_inv;
 };
 
-Pack make_pack(const double* X, const double* sf, int N, int p) {
+// the pack of design_create (pdq_api.cu): `offsets` as there, for the apeGLM call
+Pack make_pack(const double* X, const double* sf, int N, int p, bool offsets = false) {
     Pack k;
-    const int RS = design_row_stride(p);
-    k.buf.assign((size_t)(N + 1) * RS, 0.0);
-    double inv = 0;
-    for (int n = 0; n < N; ++n) {
-        for (int j = 0; j < p; ++j) {
-            k.buf[(size_t)n * RS + j] = X[(size_t)n * p + j];
-            double& mx = k.buf[(size_t)N * RS + j];
-            mx = !(fabs(X[(size_t)n * p + j]) <= mx) ? fabs(X[(size_t)n * p + j]) : mx;
-        }
-        const double s = sf ? sf[n] : 1.0;
-        k.buf[(size_t)n * RS + p] = s;
-        k.buf[(size_t)n * RS + p + 1] = log(s);
-        inv += 1.0 / s;
-    }
-    k.s_mean_inv = inv / N;
-    k.d = DesignS{k.buf.data(), k.buf.data() + p, k.buf.data() + p + 1, N, RS, host_math_table()};
+    k.s_mean_inv = design_pack(X, sf, offsets, N, p, k.buf);
+    k.d = DesignS{k.buf.data(), k.buf.data() + p, k.buf.data() + p + 1, N, design_row_stride(p), host_math_table()};
     design_linear_algebra(X, N, p, k.pinv, &k.full_rank);
     return k;
+}
+
+// k_size_factor_median, one "thread": each sample's median of log ratios against the log means `lm` (a non-finite entry leaves
+// the gene out), exponentiated; `skip_zero` for poscounts
+void size_factor_medians(const int64_t* counts, int64_t ld, int N, int G, const double* lm, bool skip_zero, double* sf) {
+    std::vector<double> row((size_t)G);
+    unsigned hist[514];
+    SerialReducer red;
+    for (int n = 0; n < N; ++n) {
+        size_t cnt = 0;
+        for (int g = 0; g < G; ++g) {
+            bool keep;
+            row[g] = log_ratio_entry(counts[(size_t)n * ld + g], lm[g], keep, skip_zero);
+            cnt += keep;
+        }
+        sf[n] = exp(median_of(red, row.data(), (size_t)G, cnt, false, 0.0, hist));
+    }
 }
 
 template <int P>
@@ -282,8 +288,7 @@ int emu_alpha_mle_hint(const int64_t* counts, int64_t ld, int N, int G, const do
 int emu_lfc_shrink(const double* X, const int64_t* counts, int64_t ld, int N, int G, int p, const double* size, const double* offset,
                    double prior_no_shrink_scale, double prior_scale, int shrink_index, double* lfcs, double* inv_hessians, double* conv,
                    int* status, int force_grid) {
-    Pack k = make_pack(X, nullptr, N, p);
-    for (int n = 0; n < N; ++n) k.buf[(size_t)n * k.d.RS + p + 1] = offset[n];
+    Pack k = make_pack(X, offset, N, p, true);
     const ShrinkParams prm{1.0 / (prior_no_shrink_scale * prior_no_shrink_scale), prior_scale * prior_scale, shrink_index};
     EMU_DISPATCH(p, {
         for (int g = 0; g < G; ++g)
@@ -393,25 +398,63 @@ int emu_cooks(const int64_t* counts, int64_t ld, int N, int G, const double* sf,
     return 0;
 }
 
-// median-of-ratios size factors with the device's selection code (k_log_means + k_size_factor_median, one "thread")
-int emu_size_factors(const int64_t* counts, int64_t ld, int N, int G, double* sf) {
-    std::vector<double> lm((size_t)G), row((size_t)G);
+// pdq_size_factors_ex (k_log_means, k_size_factor_median, k_size_factor_geomean; one "thread"): `control` and `logmeans` (G,), the
+// raw log means, may be NULL; -2 (PDQ_ERR_INVALID) for an unknown kind
+int emu_size_factors_ex(const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control, double* sf, double* logmeans) {
+    if (kind != kSfRatio && kind != kSfPoscounts) return -2;
+    std::vector<double> lm((size_t)G), kept((size_t)G);
     for (int g = 0; g < G; ++g) {
         double s = 0.0;
-        for (int n = 0; n < N; ++n) s += log((double)counts[(size_t)n * ld + g]);
+        for (int n = 0; n < N; ++n) s += log_mean_term(counts[(size_t)n * ld + g], kind);
         lm[g] = s / (double)N;
+        kept[g] = kept_logmean(lm[g], kind, control == nullptr || control[g] != 0);
     }
-    unsigned hist[514];
-    SerialReducer red;
-    for (int n = 0; n < N; ++n) {
-        size_t cnt = 0;
-        for (int g = 0; g < G; ++g) {
-            const bool keep = fabs(lm[g]) <= 1.7976931348623157e308;
-            row[g] = keep ? log((double)counts[(size_t)n * ld + g]) - lm[g] : (0.0 / 0.0);
-            cnt += keep;
-        }
-        sf[n] = exp(median_of(red, row.data(), (size_t)G, cnt, false, 0.0, hist));
+    if (logmeans) memcpy(logmeans, lm.data(), (size_t)G * sizeof(double));
+    size_factor_medians(counts, ld, N, G, kept.data(), kind == kSfPoscounts, sf);
+    if (kind == kSfPoscounts) {
+        double s = 0.0;
+        for (int n = 0; n < N; ++n) s += log(sf[n]);
+        const double gm = exp(s / (double)N);
+        for (int n = 0; n < N; ++n) sf[n] = sf[n] / gm;
     }
+    return 0;
+}
+
+// pdq_size_factors: median of ratios over every gene
+int emu_size_factors(const int64_t* counts, int64_t ld, int N, int G, double* sf, double* logmeans) {
+    return emu_size_factors_ex(counts, ld, N, G, kSfRatio, nullptr, sf, logmeans);
+}
+
+// pdq_size_factors_from_logmeans: held-out samples against the caller's log means
+int emu_size_factors_from_logmeans(const int64_t* counts, int64_t ld, int N, int G, const double* lm, double* sf) {
+    size_factor_medians(counts, ld, N, G, lm, false, sf);
+    return 0;
+}
+
+int emu_vst_transform(const int64_t* counts, int64_t ld, int N, int G, const double* sf, int kind, double c0, double c1, double* out,
+                      int64_t ld_out) {
+    if (kind != kVstParametric && kind != kVstMean) return -2;
+    const VstParams prm{kind, c0, c1};
+    for (int n = 0; n < N; ++n)
+        for (int g = 0; g < G; ++g) out[(size_t)n * ld_out + g] = vst_value(counts[(size_t)n * ld + g], sf[n], prm);
+    return 0;
+}
+
+// pdq_wald_contrasts: K contrasts of fitted coefficients, mu built from them (wald_contrasts_gene); outputs (K, ld_out).
+// -2 (PDQ_ERR_INVALID) for K <= 0, ld_out < G or an unknown alternative, -3 for p > 16.
+int emu_wald_contrasts(const double* X, const double* sf, int N, int p, const double* disp, const double* lfc, int G, const double* ridge,
+                       int K, const double* contrasts, const double* lfc_null, const int* alt, double* pv, double* stat, double* se,
+                       int64_t ld_out) {
+    if (K <= 0 || ld_out < G) return -2;
+    std::vector<double> tab((size_t)K * (p + 2));
+    if (wald_contrast_table(K, p, contrasts, lfc_null, alt, tab.data()) >= 0) return -2;
+    Pack k = make_pack(X, sf, N, p);
+    EMU_DISPATCH(p, {
+        for (int g = 0; g < G; ++g)
+            with_lanes([&](const Group& grp) {
+                wald_contrasts_gene<P>(grp, k.d, ridge, disp[g], lfc + (size_t)g * P, K, tab.data(), pv + g, stat + g, se + g, ld_out, true);
+            });
+    });
     return 0;
 }
 

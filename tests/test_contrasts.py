@@ -14,18 +14,18 @@ from conftest import load_golden
 
 @pytest.fixture(scope="module")
 def emu():
-    from emu.contrast_ops import ContrastEmuOps
+    from emu.emu_ops import EmuOps
     from pydeseq2_b200.inference import B200Inference
 
-    return B200Inference(_ops=ContrastEmuOps())
+    return B200Inference(_ops=EmuOps())
 
 
 @pytest.fixture(scope="module")
 def emu8():
-    from emu.contrast_ops import ContrastEmuOps
+    from emu.emu_ops import EmuOps
     from pydeseq2_b200.inference import B200Inference
 
-    return B200Inference(_ops=ContrastEmuOps(lanes=8))
+    return B200Inference(_ops=EmuOps(lanes=8))
 
 
 @pytest.mark.parametrize("name", CT)
@@ -80,9 +80,9 @@ def test_wald_tests_argument_errors(emu):
 
 
 def test_emulator_entry_rejects_bad_tables():
-    from emu.contrast_ops import ContrastEmuOps
+    from emu.emu_ops import EmuOps
 
-    ops = ContrastEmuOps()
+    ops = EmuOps()
     X, sf, disp, lfc, cs = seeded_case(3, 20, 10, 2, seed=9)
     out = [np.empty((2, 10)) for _ in range(3)]
     args = (X, sf, 20, 3, disp, lfc, 10, np.eye(3) * 1e-6)

@@ -20,10 +20,10 @@ def inf():
 
 
 def emulated(X, sf, disp, lfc, cs, nulls, alts):
-    from emu.contrast_ops import ContrastEmuOps
+    from emu.emu_ops import EmuOps
     from pydeseq2_b200.inference import B200Inference
 
-    return B200Inference(_ops=ContrastEmuOps()).wald_tests(X, sf, disp, lfc, cs, None, nulls, alts)
+    return B200Inference(_ops=EmuOps()).wald_tests(X, sf, disp, lfc, cs, None, nulls, alts)
 
 
 @pytest.mark.parametrize("name", CT)

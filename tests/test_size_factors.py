@@ -2,7 +2,7 @@
 
 A numpy restatement of the reference (sf_cases.fit_size_factors) is pinned to the sf_* goldens of the real orchestrator
 (scripts/make_size_factor_golden.py); the device's per-entry functions and selection code run through the host emulator
-(tests/emu/sf_emu.cpp, the same source as
+(tests/emu/pdq_emu.cpp, the same source as
 k_log_means / k_size_factor_median / k_size_factor_geomean) and are compared with the same goldens, through `B200Inference`,
 `workflow.deseq2_results` / `vst` and the drop-in `DeseqDataSet` subclass."""
 import sys
@@ -22,9 +22,9 @@ from test_vst import assert_vst_close
 
 @pytest.fixture(scope="module")
 def ops():
-    from emu.sf_ops import SfEmuOps
+    from emu.emu_ops import EmuOps
 
-    return SfEmuOps()
+    return EmuOps()
 
 
 @pytest.fixture(scope="module")

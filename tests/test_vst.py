@@ -1,6 +1,6 @@
 """CPU suite: the variance-stabilising transform (DeseqDataSet.vst / vst_fit / vst_transform, dds.py:349-514).
 
-The kernels' per-element function and the held-out median selection run through the host emulator (tests/emu/vst_emu.cpp, the
+The kernels' per-element function and the held-out median selection run through the host emulator (tests/emu/pdq_emu.cpp, the
 same source as k_vst_transform / k_size_factor_median) and are compared with the reference's numpy expressions; `workflow.vst`
 and the `vst_transform` override of `integration.b200_dataset_class()` are compared with what the real orchestrator stored in
 the vst_* goldens (scripts/make_vst_golden.py)."""
@@ -53,9 +53,9 @@ def assert_vst_close(got, want, rel=1e-4):
 
 @pytest.fixture(scope="module")
 def ops():
-    from emu.vst_ops import VstEmuOps
+    from emu.emu_ops import EmuOps
 
-    return VstEmuOps()
+    return EmuOps()
 
 
 @pytest.fixture(scope="module")
