@@ -263,6 +263,24 @@ int pdq_irls_wald_dev(pdq_ctx* ctx, const pdq_design* design, const int64_t* cou
                       double* converged_out, int* n_fallback_dev, const double* ridge_host,
                       const double* contrast_host, double lfc_null, int alt, double* pvalue_out,
                       double* stat_out, double* se_out);
+/* The tail of a resident pass with a per-tile dependency: the MAP dispersion search (pdq_alpha_mle_hint_dev with cr_reg =
+ * prior_reg = 1, opened from `hint_in`, prior variance from `prior_var_dev` when set), pdq_select_dispersions_dev and
+ * pdq_irls_wald_dev.  The search kernel writes the final dispersions of a warp tile and publishes the tile; the fit kernel, a
+ * programmatic dependent launch that becomes resident while the last tiles of the search are still being worked on, waits per
+ * tile instead of for the whole grid (DESIGN.md §4).  Per-gene arithmetic is that of the three calls: results are bit-identical
+ * to issuing them in sequence, which is also what this call does when a warp has many tiles per launch and the hand-off would
+ * not pay.  Genes that need the grid fallback of the search or the optimiser branch of the fit take the same fallback
+ * kernels, behind the pair.  `outlier_out` may be NULL.  A hand-off wait that gives up (a logic error, never expected) is
+ * reported by pdq_map_irls_status after a stream synchronisation: 0, or 1 + the tile. */
+int pdq_map_irls_wald_dev(pdq_ctx* ctx, const pdq_design* design, const int64_t* counts, int64_t ld, int G,
+                          const double* mu, int64_t ld_mu, const double* fitted, const double* genewise,
+                          const double* hint_in, const double* trend_out16, double min_disp, double max_disp,
+                          double prior_disp_var, const double* prior_var_dev, double* map_out, double* map_converged_out,
+                          double* disp_out, double* outlier_out, double min_mu, double beta_tol, double min_beta,
+                          double max_beta, int maxiter, double* beta_out, double* mu_out, double* hat_out, int64_t ld_out,
+                          double* converged_out, const double* ridge_host, const double* contrast_host, double lfc_null,
+                          int alt, double* pvalue_out, double* stat_out, double* se_out);
+int pdq_map_irls_status(pdq_ctx* ctx, unsigned long long* status_out);
 int pdq_alpha_mle_dev(pdq_ctx* ctx, const pdq_design* design, const int64_t* counts, int64_t ld, int G,
                       const double* mu, int64_t ld_mu, const double* alpha_hat, double min_disp,
                       double max_disp, double prior_disp_var,

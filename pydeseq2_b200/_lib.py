@@ -83,6 +83,11 @@ _SIGNATURES = {
     "pdq_irls_wald_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, c_dptr, C.c_double, C.c_double, C.c_double,
                                     C.c_double, C.c_int, c_dptr, c_dptr, c_dptr, C.c_int64, c_dptr, c_dptr, f64p, f64p,
                                     C.c_double, C.c_int, c_dptr, c_dptr, c_dptr]),
+    "pdq_map_irls_wald_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, c_dptr, C.c_int64, c_dptr, c_dptr, c_dptr, c_dptr,
+                                        C.c_double, C.c_double, C.c_double, c_dptr, c_dptr, c_dptr, c_dptr, c_dptr, C.c_double,
+                                        C.c_double, C.c_double, C.c_double, C.c_int, c_dptr, c_dptr, c_dptr, C.c_int64, c_dptr, f64p,
+                                        f64p, C.c_double, C.c_int, c_dptr, c_dptr, c_dptr]),
+    "pdq_map_irls_status": (C.c_int, [c_ctx, C.POINTER(C.c_uint64)]),
     "pdq_alpha_mle_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, c_dptr, C.c_int64, c_dptr, C.c_double,
                                     C.c_double, C.c_double, c_dptr, C.c_int, C.c_int, c_dptr, c_dptr]),
     "pdq_alpha_mle_hint_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, c_dptr, C.c_int64, c_dptr, C.c_double,

@@ -149,7 +149,12 @@ struct pdq_ctx {
     cudaEvent_t stage_ev[2] = {nullptr, nullptr};
     bool stage_busy[2] = {false, false};
     int staging = 1;  // PDQ_STAGING=0 disables (plain cudaMemcpyAsync from pageable memory)
-    int* tickets = nullptr;  // device ints for the persistent kernels' tile counters (4 per stream slot)
+    int* tickets = nullptr;  // device ints for the persistent kernels' tile counters (4 per stream slot), then the control words of
+                             // the fused MAP -> LFC launch (launch_map_irls); zeroed once, here
+    unsigned* tile_done = nullptr;  // per-tile hand-off words of launch_map_irls (zeroed when allocated)
+    size_t tile_cap = 0;
+    unsigned long long* tail_err_host = nullptr;  // mapped page-locked word: non-zero after a tile wait of launch_map_irls gave up
+    unsigned long long* tail_err_dev = nullptr;
     void* grid_scratch = nullptr;  // accumulators of the grid-wide trend fit
     cudaStream_t pstream[2] = {nullptr, nullptr};  // gene-block pipeline of the host-buffer entry points
     cudaEvent_t pfork = nullptr, pjoin[2] = {nullptr, nullptr};
@@ -284,7 +289,7 @@ extern "C" int pdq_ctx_create(int device, pdq_ctx** out) {
     c->res_cap = c->prop.totalGlobalMem / 4;
     if (c->res_cap > ((size_t)16 << 30)) c->res_cap = (size_t)16 << 30;
     if (const char* s = getenv("PDQ_RESIDENCY_BYTES")) c->res_cap = (size_t)atoll(s);
-    if (cudaMalloc((void**)&c->tickets, 64) != cudaSuccess || cudaMalloc(&c->grid_scratch, kGridScratchBytes) != cudaSuccess || cudaStreamCreateWithFlags(&c->pstream[0], cudaStreamNonBlocking) != cudaSuccess ||
+    if (cudaMalloc((void**)&c->tickets, 128) != cudaSuccess || cudaMemsetAsync(c->tickets, 0, 128, c->stream) != cudaSuccess || cudaMalloc(&c->grid_scratch, kGridScratchBytes) != cudaSuccess || cudaStreamCreateWithFlags(&c->pstream[0], cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&c->pstream[1], cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->pfork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->pjoin[0], cudaEventDisableTiming) != cudaSuccess ||
@@ -311,6 +316,8 @@ extern "C" void pdq_ctx_destroy(pdq_ctx* c) {
     if (c->hash_dev) cudaFree(c->hash_dev);
     if (c->hash_host) cudaFreeHost(c->hash_host);
     if (c->tickets) cudaFree(c->tickets);
+    if (c->tile_done) cudaFree(c->tile_done);
+    if (c->tail_err_host) cudaFreeHost(c->tail_err_host);
     if (c->grid_scratch) cudaFree(c->grid_scratch);
     for (auto& st : c->pstream)
         if (st) cudaStreamDestroy(st);
@@ -636,6 +643,67 @@ extern "C" int pdq_alpha_mle_hint_dev(pdq_ctx* c, const pdq_design* d, const int
                                       const double* hint_in, double* hint_out) {
     return alpha_mle_dev(c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_disp_var, prior_var_dev, cr_reg, prior_reg, alpha,
                          conv, hint_in, hint_out);
+}
+
+extern "C" int pdq_map_irls_wald_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, const double* mu,
+                                     int64_t ld_mu, const double* fitted, const double* genewise, const double* hint_in,
+                                     const double* trend_out16, double min_disp, double max_disp, double prior_disp_var,
+                                     const double* prior_var_dev, double* map, double* map_conv, double* disp, double* outlier,
+                                     double min_mu, double beta_tol, double min_beta, double max_beta, int maxiter, double* beta,
+                                     double* mu_out, double* hat, int64_t ld_out, double* conv, const double* ridge,
+                                     const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
+    CHECK_CTX(c);
+    if (!d || !counts || !mu || !fitted || !genewise || !hint_in || !trend_out16 || !map || !map_conv || !disp || !beta || !mu_out ||
+        !hat || !conv || G <= 0 || ld < G || ld_mu < G || ld_out < G || !ridge || !contrast || !pv || !stat || !se || alt < 0 || alt > 4)
+        return fail(c, PDQ_ERR_INVALID, "pdq_map_irls_wald_dev: bad arguments");
+    if (!prior_var_dev && !(prior_disp_var > 0.0)) return fail(c, PDQ_ERR_INVALID, "pdq_map_irls_wald_dev: needs prior_disp_var > 0");
+    // The hand-off pays where a warp works on few tiles per launch, so that the drained end of the search and the ramp-up of the
+    // fit are a visible share of both: measured on H100 it gains 3-7 % up to ~10 tiles per resident warp of the search (12 per SM)
+    // and loses 2.5 % at 20 (DESIGN.md §5).  Above 12 the three stages run as the three launches.
+    const LaunchCfg lcfg = cfg(c, G, d->d.N);
+    const int gpw = 32 >> lcfg.lgT;
+    if ((int64_t)(G + gpw - 1) / gpw > (int64_t)12 * 12 * lcfg.sm_count) {
+        if (int e = alpha_mle_dev(c, d, counts, ld, G, mu, ld_mu, fitted, min_disp, max_disp, prior_disp_var, prior_var_dev, 1, 1, map,
+                                  map_conv, hint_in, nullptr))
+            return e;
+        if (int e = done(c, launch_select_disp(lcfg, genewise, map, fitted, trend_out16, (size_t)G, min_disp, max_disp, disp, outlier),
+                         "select_dispersions"))
+            return e;
+        return pdq_irls_wald_dev(c, d, counts, ld, G, disp, min_mu, beta_tol, min_beta, max_beta, maxiter, beta, mu_out, hat, ld_out, conv,
+                                 nullptr, ridge, contrast, lfc_null, alt, pv, stat, se);
+    }
+    void* status;
+    if (int e = ensure(c, kBufStatus, 2 * (size_t)G * sizeof(int), &status)) return e;
+    if ((size_t)G > c->tile_cap) {  // one word per gene covers every tile size
+        if (c->tile_done) {
+            CU(c, cudaFree(c->tile_done));
+            ++c->buf_epoch;
+        }
+        c->tile_done = nullptr;
+        c->tile_cap = 0;
+        const size_t want = (size_t)G + (size_t)G / 8 + 64;
+        CU(c, cudaMalloc((void**)&c->tile_done, want * sizeof(unsigned)));
+        CU(c, cudaMemsetAsync(c->tile_done, 0, want * sizeof(unsigned), c->stream));
+        c->tile_cap = want;
+    }
+    if (!c->tail_err_host) {
+        CU(c, cudaHostAlloc((void**)&c->tail_err_host, 8, cudaHostAllocMapped));
+        *c->tail_err_host = 0;
+        CU(c, cudaHostGetDevicePointer((void**)&c->tail_err_dev, c->tail_err_host, 0));
+    }
+    const TailHost t{mu, ld_mu, fitted, genewise, hint_in, trend_out16, min_disp, max_disp, prior_disp_var, prior_var_dev, map, map_conv,
+                     disp, outlier, beta, mu_out, hat, conv, ld_out, (int*)status, (int*)status + G, c->tile_done, c->tail_err_dev};
+    const IrlsHost h{min_mu, beta_tol, min_beta, max_beta, maxiter};
+    const WaldHost w{ridge, contrast, lfc_null, alt, pv, stat, se};
+    return done(c, launch_map_irls(lcfg, d->d, counts, ld, G, t, h, w), "map+irls+wald");
+}
+
+// 0 while every tile hand-off of pdq_map_irls_wald_dev completed; 1 + tile after a wait gave up (valid after a stream synchronisation)
+extern "C" int pdq_map_irls_status(pdq_ctx* c, unsigned long long* status_out) {
+    CHECK_CTX(c);
+    if (!status_out) return fail(c, PDQ_ERR_INVALID, "pdq_map_irls_status: bad arguments");
+    *status_out = c->tail_err_host ? *(volatile unsigned long long*)c->tail_err_host : 0ULL;
+    return PDQ_OK;
 }
 
 extern "C" int pdq_wald_test_dev(pdq_ctx* c, const pdq_design* d, const double* disp, const double* lfc, const double* mu,

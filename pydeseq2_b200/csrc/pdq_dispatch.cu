@@ -51,7 +51,15 @@ int launch_alpha_mle(const LaunchCfg& c, const DesignDev& d, const int64_t* coun
               prior_reg, alpha, conv, status, hint_in, hint_out)
 }
 
-#define DECL_WALD(sfx)                                                                                                          \
+#define DECL_TAIL(sfx) \
+    int launch_map_irls##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, const TailHost&, const IrlsHost&, const WaldHost&);
+PDQ_UNITS(DECL_TAIL)
+int launch_map_irls(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const TailHost& t, const IrlsHost& prm,
+                    const WaldHost& wald) {
+    PDQ_ROUTE(launch_map_irls, d.p, c, d, counts, ld, G, t, prm, wald)
+}
+
+#define DECL_WALD(sfx)                                                                                                         \
     int launch_wald##sfx(const LaunchCfg&, const DesignDev&, const double*, const double*, const double*, int64_t, int, const double*, \
                          const double*, double, int, double*, double*, double*);
 PDQ_UNITS(DECL_WALD)

@@ -1405,6 +1405,17 @@ PDQ_HD void alpha_grid_gene(const Group& grp, const DesignS& d, double lo, doubl
     if (valid && grp.si == 0) *alpha_out = exp(bestf);
 }
 
+// final dispersion of one gene (dds.py:918-932): the clipped MAP estimate, but a gene whose genewise estimate lies more than
+// 2 sd of the log residuals above the trend keeps its (clipped) genewise value.  The one statement of the rule: the elementwise
+// kernel and the fused MAP -> LFC launch both call it.
+PDQ_HD double select_disp(double gw, double mp, double fitted, double squared_logres, double lo, double hi, bool& outlier) {
+    double g = gw, m = mp;
+    g = (g < lo) ? lo : ((g > hi) ? hi : g);
+    m = (m < lo) ? lo : ((m > hi) ? hi : m);
+    outlier = log(g) > log(fitted) + 2.0 * sqrt(squared_logres);
+    return outlier ? g : m;
+}
+
 // =============================================================================================
 // (a5) fit_rough_dispersions (utils.py:814-853) / fit_moments_dispersions (utils.py:856-885)
 // `Y` abstracts where normalised counts come from: a float64 (N,G) array (the plugin call) or raw

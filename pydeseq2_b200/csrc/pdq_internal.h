@@ -56,6 +56,25 @@ int launch_alpha_mle(const LaunchCfg&, const DesignDev&, const int64_t* counts, 
                      int64_t ld_mu, const double* alpha_hat, double min_disp, double max_disp, double prior_var,
                      const double* prior_var_dev, int cr_reg, int prior_reg, double* alpha, double* conv, int* status,
                      const double* hint_in = nullptr, double* hint_out = nullptr);
+// MAP dispersion search -> final dispersions -> LFC fit + Wald test as one persistent launch (k_map_irls): device pointers of the
+// stages' inputs and outputs, everything but the counts and the small host parameters (IrlsHost, WaldHost)
+struct TailHost {
+    const double* mu;          // (N, G) means the dispersion search runs on
+    int64_t ld_mu;
+    const double *fitted, *gw, *hint_in;  // trend values, genewise dispersions, [G][2] hints of the genewise search
+    const double* trend16;     // trend record (TrendOut)
+    double min_disp, max_disp, prior_var;
+    const double* prior_var_dev;  // overrides prior_var when set
+    double *map, *map_conv, *disp, *outlier;
+    double *beta, *mu_out, *hat, *conv;
+    int64_t ld_out;
+    int *status_map, *status_irls;  // G ints each
+    unsigned* tile_done;       // >= number of warp tiles words, zeroed when allocated and owned by these launches since
+    unsigned long long* err;   // device address of a mapped host word: non-zero after a tile wait gave up
+};
+// LaunchCfg::tickets must hold 32 ints, all zero when the context is created (ints 16.. are the launch's control words)
+int launch_map_irls(const LaunchCfg&, const DesignDev&, const int64_t* counts, int64_t ld, int G, const TailHost&, const IrlsHost&,
+                    const WaldHost&);
 int launch_wald(const LaunchCfg&, const DesignDev&, const double* disp, const double* lfc, const double* mu,
                 int64_t ld_mu, int G, const double* ridge, const double* contrast, double lfc_null, int alt,
                 double* pv, double* stat, double* se);

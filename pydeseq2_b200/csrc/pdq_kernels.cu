@@ -338,6 +338,219 @@ __global__ void __launch_bounds__(kBlock) k_alpha_grid(const __grid_constant__ A
     }
 }
 
+// ---- MAP dispersion search -> final dispersion -> LFC fit + Wald test with a per-tile dependency (DESIGN.md §4) ----------------
+// The LFC fit of a gene needs that gene's final dispersion only, and the final dispersion is an elementwise function of the
+// gene's MAP estimate: the dependency between the two heavy stages is per gene tile, not per grid.  k_map_irls<.., 0> is the MAP
+// search (alpha_gene as in k_alpha_mle, then select_disp per gene); it publishes every warp tile with a release store of the pass
+// number into tile_done[tile].  k_map_irls<.., 1> is the LFC fit (irls_gene as in k_irls); before a tile it waits for that word.
+// The second kernel is a programmatic dependent launch: its blocks become resident as soon as every block of the first has
+// started and an SM has room, i.e. while the last MAP tiles are still being worked on, where two ordinary launches would drain,
+// run the elementwise kernel and ramp up again.  Two kernels rather than one so that each body keeps its own register budget
+// (3 resident blocks per SM for the search, 4 for the fit).
+//
+// Control words (device ints, LaunchCfg::tickets + kTailWords), kept consistent by the kernels themselves so that the pair
+// replays inside a CUDA graph without memset nodes: the last block of each kernel zeroes its ticket counter and moves its
+// flagged-gene count to the word the fallback kernel behind the pair reads; the last block of the fit bumps the pass number.
+// tile_done holds (pass << 1) | deferred: words of earlier passes never match, so the array is zeroed once, when it is allocated.
+constexpr int kTailWords = 16;  // offset of the control words in LaunchCfg::tickets
+enum { kTailTicket = 0, kTailPass = 1, kTailBlocks = 2, kTailGridCnt = 3, kTailOptCnt = 4, kTailTicket2 = 5, kTailGridOut = 6, kTailOptOut = 7,
+       kTailBlocks2 = 8 };  // ...2: ticket counter and finished blocks of the LFC kernel
+
+template <int P>
+struct TailArgs {
+    AlphaArgs<P> al;  // MAP search: al.alpha = MAP estimates, al.alpha_hat = trend values
+    IrlsArgs<P> ir;   // LFC fit + Wald test: ir.disp = the final dispersions written by the MAP tickets
+                      // (al.ticket / ir.ticket serve k_alpha_grid / k_irls_optimizer behind the launch: ticket[1] = flagged genes)
+    const double* gw;       // genewise dispersions
+    const TrendOut* trend;  // device record of the trend fit (squared_logres)
+    double min_disp, max_disp;
+    double *disp, *outlier;
+    int* words;               // control words above
+    unsigned* tile_done;      // one word per warp tile
+    unsigned long long* err;  // mapped host word: 1 + tile when a wait gave up
+    unsigned long long timeout_ns;
+};
+
+__device__ __forceinline__ void tile_lanes(int lgT, int G, int tile, Group& grp, int& gene, bool& valid) {
+    const int lane = threadIdx.x & 31;
+    grp.T = 1 << lgT;
+    grp.gpw = 32 >> lgT;
+    grp.si = lane >> (5 - lgT);
+    const int gidx = tile * grp.gpw + (lane & (grp.gpw - 1));
+    valid = gidx < G;
+    gene = valid ? gidx : (G - 1);
+}
+__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
+    unsigned v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release_gpu(unsigned* p, unsigned v) {
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long tail_timer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+// the LFC fit of one tile and its bookkeeping, shared by k_map_irls and k_irls_deferred
+template <int P>
+__device__ __forceinline__ void tail_irls_tile(const TailArgs<P>& a, const Group& grp, const DesignS& d, int g, bool valid, double disp,
+                                               double* lg_tab, const double* logfact, int* flagged) {
+    const IrlsArgs<P>& r = a.ir;
+    int st = 0;
+    irls_gene<P>(grp, d, r.pinv, r.prm, r.counts + g, r.ld, disp, r.beta + (int64_t)g * P, r.mu + g, r.hat + g, r.ld_out,
+                 r.conv + g, &st, valid, lg_tab, logfact, r.with_wald ? &r.wald : nullptr, r.wald_p + g, r.wald_stat + g,
+                 r.wald_se + g);
+    if (valid && grp.si == 0) {
+        if (r.force) st = kIrlsNeedsOptimizer;
+        r.status[g] = st;
+        if (st != kIrlsOk) atomicAdd(flagged, 1);
+    }
+}
+
+template <int P, bool STAGED, int PHASE>
+__global__ void __launch_bounds__(kBlock, PHASE ? PDQ_IRLS_MINB : PDQ_ALPHA_MINB) k_map_irls(const __grid_constant__ TailArgs<P> a) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    // both kernels read the pass number before any block of the LFC kernel exists (the MAP blocks read it before they allow the
+    // dependent launch), and only the LFC kernel's last block changes it
+    const unsigned pass = (unsigned)*reinterpret_cast<volatile const int*>(a.words + kTailPass) + 1u;
+    if (PHASE == 0) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    const DesignS d = stage_design_t<true, STAGED ? 1 : 0>(a.al.dv, P, smem);
+    // scratch behind the design pack, its mbarrier and the math table: the block's log(k!) table, then one slot of 2 * kPsiK doubles
+    // per gene of the warp's tile -- psi / psi' tables in the MAP kernel, the lgamma(r + k) table in the LFC kernel
+    double* logfact = reinterpret_cast<double*>(smem + scratch_off(a.al.dv, true));
+    if (PHASE == 1) {
+        if (threadIdx.x < kPsiK) logfact[threadIdx.x] = kLogFact[threadIdx.x];
+        __syncthreads();
+    }
+    const int lane = threadIdx.x & 31, gpw = 32 >> a.al.lgT;
+    double* slot = logfact + kPsiK + (size_t)((threadIdx.x >> 5) * gpw + (lane & (gpw - 1))) * (2 * kPsiK);
+    const int G = a.al.G, ntiles = (G + gpw - 1) >> (5 - a.al.lgT);
+    int* ticket = a.words + (PHASE ? kTailTicket2 : kTailTicket);
+    Group grp;
+    int g;
+    bool valid;
+    int ahead = draw_ticket(ticket);
+    if (PHASE == 0) {
+        AlphaParams prm = a.al.prm;
+        if (a.al.prior_var_dev) prm.prior_var = *a.al.prior_var_dev;
+        const double sq_logres = a.trend->squared_logres;
+        for (;;) {
+            const int t = __shfl_sync(0xffffffffu, ahead, 0);
+            if (t >= ntiles) break;
+            ahead = draw_ticket(ticket);  // the next ticket's round trip to L2 hides behind this tile
+            tile_lanes(a.al.lgT, G, t, grp, g, valid);
+            alpha_gene<P>(grp, d, prm, a.al.counts + g, a.al.ld, a.al.mu + g, a.al.ld_mu, a.al.alpha_hat[g], a.al.alpha + g,
+                          a.al.conv + g, a.al.status + g, valid, slot, a.al.hint_in ? a.al.hint_in + 2 * (int64_t)g : nullptr,
+                          nullptr);
+            bool defer = false;
+            if (valid && grp.si == 0) {
+                if (a.al.force) {
+                    a.al.status[g] = kAlphaNeedsGrid;
+                    a.al.conv[g] = 0.0;
+                }
+                if (a.al.status[g] == kAlphaNeedsGrid) {
+                    atomicAdd(a.words + kTailGridCnt, 1);
+                    defer = true;
+                } else {
+                    bool out;
+                    a.disp[g] = select_disp(a.gw[g], a.al.alpha[g], a.al.alpha_hat[g], sq_logres, a.min_disp, a.max_disp, out);
+                    if (a.outlier) a.outlier[g] = out ? 1.0 : 0.0;
+                }
+            }
+            // a tile with a gene left to the grid fallback is published as deferred: the LFC kernel skips it, and k_alpha_grid +
+            // k_irls_deferred behind the pair finish it
+            defer = __any_sync(0xffffffffu, defer);
+            __threadfence();
+            __syncwarp();  // every lane's stores of the tile are ordered before lane 0's release
+            if (lane == 0) st_release_gpu(a.tile_done + t, (pass << 1) | (defer ? 1u : 0u));
+        }
+    } else {
+        for (;;) {
+            const int tile = __shfl_sync(0xffffffffu, ahead, 0);
+            if (tile >= ntiles) break;
+            ahead = draw_ticket(ticket);
+            // Every wait ends: a block of this kernel exists only after every block of the MAP kernel has started (programmatic
+            // dependent launch), so every MAP block is resident or done; MAP tiles never wait and their tickets are drawn by running
+            // warps only, so every tile is published.  Both kernels walk the tiles in increasing order, so the wait is short.  The
+            // time limit only turns a logic error into a reported failure (pdq_map_irls_status) instead of a hung device.
+            unsigned v = 0;
+            if (lane == 0) {
+                v = ld_acquire_gpu(a.tile_done + tile);
+                if ((v >> 1) != pass) {
+                    const unsigned long long t0 = tail_timer_ns();
+                    do {
+                        __nanosleep(200);
+                        v = ld_acquire_gpu(a.tile_done + tile);
+                    } while ((v >> 1) != pass && tail_timer_ns() - t0 <= a.timeout_ns);
+                    if ((v >> 1) != pass) {
+                        *a.err = 1ULL + (unsigned long long)tile;
+                        __threadfence_system();
+                    }
+                }
+            }
+            v = __shfl_sync(0xffffffffu, v, 0);
+            __syncwarp();
+            if ((v >> 1) != pass || (v & 1u)) continue;
+            tile_lanes(a.al.lgT, G, tile, grp, g, valid);
+            tail_irls_tile<P>(a, grp, d, g, valid, __ldcg(a.ir.disp + g), slot, logfact, a.words + kTailOptCnt);
+        }
+        // the MAP kernel has completed and its writes (the count of flagged genes, its control words) are visible before this
+        // kernel completes: what follows in the stream is ordered behind both
+        asm volatile("griddepcontrol.wait;" ::: "memory");
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        if (atomicAdd(a.words + (PHASE ? kTailBlocks2 : kTailBlocks), 1) == (int)gridDim.x - 1) {  // the kernel's last block
+            if (PHASE == 0) {
+                a.words[kTailGridOut] = atomicExch(a.words + kTailGridCnt, 0);
+                a.words[kTailTicket] = 0;
+                a.words[kTailBlocks] = 0;
+            } else {
+                a.words[kTailOptOut] = atomicExch(a.words + kTailOptCnt, 0);
+                a.words[kTailTicket2] = 0;
+                a.words[kTailBlocks2] = 0;
+                a.words[kTailPass] = (int)pass;
+            }
+        }
+    }
+}
+
+// The tiles the MAP kernel published as deferred, behind k_alpha_grid (which has replaced the MAP estimate of their flagged genes):
+// final dispersions of the tile's genes, then the LFC fit.  Normally no tile is deferred: one wave of blocks that read the count
+// of flagged genes and exit.
+template <int P>
+__global__ void __launch_bounds__(kBlock) k_irls_deferred(const __grid_constant__ TailArgs<P> a) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    if (*reinterpret_cast<volatile const int*>(a.words + kTailGridOut) == 0) return;
+    const DesignS d = stage_design_t<true, -1>(a.al.dv, P, smem);
+    double* logfact = reinterpret_cast<double*>(smem + scratch_off(a.al.dv, true));
+    if (threadIdx.x < kPsiK) logfact[threadIdx.x] = kLogFact[threadIdx.x];
+    __syncthreads();
+    const unsigned mark = ((unsigned)a.words[kTailPass] << 1) | 1u;  // the pass number the pair left behind is its own
+    const double sq_logres = a.trend->squared_logres;
+    const int lane = threadIdx.x & 31, gpw = 32 >> a.al.lgT;
+    double* slot = logfact + kPsiK + (size_t)((threadIdx.x >> 5) * gpw + (lane & (gpw - 1))) * (2 * kPsiK);
+    const int G = a.al.G, ntiles = (G + gpw - 1) >> (5 - a.al.lgT);
+    for (int tile = blockIdx.x * kWarps + (threadIdx.x >> 5); tile < ntiles; tile += gridDim.x * kWarps) {
+        if (a.tile_done[tile] != mark) continue;
+        Group grp;
+        int g;
+        bool valid;
+        tile_lanes(a.al.lgT, G, tile, grp, g, valid);
+        bool out;
+        const double disp = select_disp(a.gw[g], a.al.alpha[g], a.al.alpha_hat[g], sq_logres, a.min_disp, a.max_disp, out);
+        if (valid && grp.si == 0) {
+            a.disp[g] = disp;
+            if (a.outlier) a.outlier[g] = out ? 1.0 : 0.0;
+        }
+        tail_irls_tile<P>(a, grp, d, g, valid, disp, slot, logfact, a.words + kTailOptOut);
+    }
+}
+
 template <int P>
 struct WaldArgs {
     DesignView dv;
@@ -1013,17 +1226,13 @@ __global__ void k_trend_eval(const double* __restrict__ means, size_t n, const T
     if (i < n) fitted[i] = c->c0 + c->c1 / means[i];
 }
 
-// final dispersions (dds.py:918-932): clip the MAP estimate, but genes whose genewise estimate lies more than
-// 2 sd of the log residuals above the trend keep their (clipped) genewise value
+// final dispersions (dds.py:918-932), elementwise: select_disp (pdq_gene.cuh) per gene
 __global__ void k_select_disp(const double* __restrict__ gw, const double* __restrict__ mp, const double* __restrict__ fitted,
                               const TrendOut* __restrict__ c, size_t n, double lo, double hi, double* disp, double* outlier) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    double g = gw[i], m = mp[i];
-    g = (g < lo) ? lo : ((g > hi) ? hi : g);
-    m = (m < lo) ? lo : ((m > hi) ? hi : m);
-    const bool out = log(g) > log(fitted[i]) + 2.0 * sqrt(c->squared_logres);
-    disp[i] = out ? g : m;
+    bool out;
+    disp[i] = select_disp(gw[i], mp[i], fitted[i], c->squared_logres, lo, hi, out);
     if (outlier) outlier[i] = out ? 1.0 : 0.0;
 }
 
@@ -1091,6 +1300,26 @@ int persistent_grid(K kernel, size_t smem, int sm_count, int G, int lgT) {
     const int need = grid_for(G, lgT);
     const int fit = per_sm * sm_count;
     return need < fit ? need : fit;
+}
+
+// the MAP kernel, then the LFC kernel as its programmatic dependent (see k_map_irls)
+template <int P, bool STAGED>
+int launch_tail_pair(const LaunchCfg& c, const TailArgs<P>& a, size_t smem, int G) {
+    if (int e = prep(k_map_irls<P, STAGED, 0>, smem)) return e;
+    if (int e = prep(k_map_irls<P, STAGED, 1>, smem)) return e;
+    k_map_irls<P, STAGED, 0><<<persistent_grid(k_map_irls<P, STAGED, 0>, smem, c.sm_count, G, c.lgT), kBlock, smem, c.stream>>>(a);
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = dim3((unsigned)persistent_grid(k_map_irls<P, STAGED, 1>, smem, c.sm_count, G, c.lgT));
+    lc.blockDim = dim3(kBlock);
+    lc.dynamicSmemBytes = smem;
+    lc.stream = c.stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    lc.attrs = at;
+    lc.numAttrs = 1;
+    if (cudaLaunchKernelEx(&lc, k_map_irls<P, STAGED, 1>, a) != cudaSuccess) return PDQ_ERR_CUDA;
+    return 0;
 }
 
 template <int P>
@@ -1316,6 +1545,47 @@ int PDQ_TUFN(launch_alpha_mle)(const LaunchCfg& c, const DesignDev& d, const int
     });
     if (int e = check_launch()) return e;
     return 2;
+}
+
+int PDQ_TUFN(launch_map_irls)(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const TailHost& t,
+                              const IrlsHost& h, const WaldHost& w) {
+    PDQ_DISPATCH_P(d.p, {
+        TailArgs<P> a;
+        const DesignView dv{d.pack, d.N, d.staged ? (int)(d.smem_bytes - 16) : 0};
+        int* words = c.tickets + kTailWords;
+        // the fallback kernels read the count of flagged genes at ticket[1]: the words the last blocks of k_map_irls fill
+        a.al = AlphaArgs<P>{dv, AlphaParams{log(t.min_disp), log(t.max_disp), t.prior_var, 1, 1}, counts, ld, G, c.lgT, t.mu, t.ld_mu,
+                            t.fitted, t.map, t.map_conv, t.status_map, t.prior_var_dev, words + kTailGridOut - 1,
+                            (c.debug & PDQ_DEBUG_FORCE_ALPHA_GRID) ? 1 : 0, t.hint_in, nullptr, 0};
+        a.ir.dv = dv;
+        a.ir.pinv = pinv_of<P>(d);
+        a.ir.prm = IrlsParams{h.min_mu, h.beta_tol, h.min_beta, h.max_beta, h.maxiter, d.full_rank, d.few_rows,
+                              (c.debug & PDQ_DEBUG_FAIL_IRLS_OPTIMIZER) ? 1 : 0};
+        a.ir.counts = counts; a.ir.ld = ld; a.ir.G = G; a.ir.lgT = c.lgT; a.ir.disp = t.disp;
+        a.ir.beta = t.beta; a.ir.mu = t.mu_out; a.ir.hat = t.hat; a.ir.conv = t.conv; a.ir.ld_out = t.ld_out;
+        a.ir.status = t.status_irls; a.ir.n_fallback = nullptr; a.ir.ticket = words + kTailOptOut - 1;
+        a.ir.force = (c.debug & PDQ_DEBUG_FORCE_IRLS_OPTIMIZER) ? 1 : 0;
+        a.ir.with_wald = 1;
+        for (int i = 0; i < P * P; ++i) a.ir.wald.ridge[i] = w.ridge[i];
+        for (int i = 0; i < P; ++i) a.ir.wald.contrast[i] = w.contrast[i];
+        a.ir.wald.lfc_null = w.lfc_null;
+        a.ir.wald.alt = w.alt;
+        a.ir.wald_p = w.pv; a.ir.wald_stat = w.stat; a.ir.wald_se = w.se;
+        a.gw = t.gw; a.trend = reinterpret_cast<const TrendOut*>(t.trend16);
+        a.min_disp = t.min_disp; a.max_disp = t.max_disp; a.disp = t.disp; a.outlier = t.outlier;
+        a.words = words; a.tile_done = t.tile_done; a.err = t.err; a.timeout_ns = 20000000000ULL;
+        const size_t smem_tail = d.smem_bytes + kMathTabBytes + (size_t)(1 + 2 * kWarps * (32 >> c.lgT)) * kPsiK * sizeof(double);
+        if (int e = prep(k_alpha_grid<P>, d.smem_bytes)) return e;
+        if (int e = prep(k_irls_deferred<P>, smem_tail)) return e;
+        if (int e = prep(k_irls_optimizer<P>, d.smem_bytes)) return e;
+        if (int e = d.staged ? launch_tail_pair<P, true>(c, a, smem_tail, G) : launch_tail_pair<P, false>(c, a, smem_tail, G)) return e;
+        const int wave = fallback_grid(c.sm_count, G, c.lgT);
+        k_alpha_grid<P><<<wave, kBlock, d.smem_bytes, c.stream>>>(a.al);
+        k_irls_deferred<P><<<wave, kBlock, smem_tail, c.stream>>>(a);
+        k_irls_optimizer<P><<<wave, kBlock, d.smem_bytes, c.stream>>>(a.ir);
+    });
+    if (int e = check_launch()) return e;
+    return 5;
 }
 
 int PDQ_TUFN(launch_wald)(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu,

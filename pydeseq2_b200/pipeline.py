@@ -395,6 +395,11 @@ class ResidentFit:
         self.fuse_wald = True         # Wald test inside the LFC-fit launch (False: the two plugin-shaped calls in sequence)
         self.gather = comm is not None  # end the pass with the all-gather of the result tables of all gene shards
         self.use_hint = True          # MAP dispersion search opened from the genewise optimum + curvature (pdq_alpha_mle_hint_dev)
+        # MAP search, final dispersions and LFC fit + Wald test with a per-tile dependency instead of three grid-wide ones
+        # (pdq_map_irls_wald_dev; needs fuse_wald and use_hint): the fit's kernel becomes resident while the search's last tiles
+        # run.  Bit-identical results; the entry point keeps the three launches where a warp has many tiles per launch.  False: the
+        # three launches always (the reference of tests/test_gpu_fused_tail.py and scripts/tail_bench.py)
+        self.fuse_tail = True
         # how gene shards exchange: "peer" = one kernel per exchange storing into every peer's HBM over NVLink (sharding.PeerWindow),
         # "nccl" = grouped NCCL all-gathers, "auto" = peer when the ranks can map each other's memory (one node), else NCCL
         self.exchange = os.environ.get("PDQ_EXCHANGE", "auto")
@@ -748,7 +753,7 @@ class ResidentFit:
                 begin("trend_prior")
                 check(L.pdq_trend_fit_dev(h, c_d(d_means_all), c_d(d_gw_all), n_all, self.min_disp, self.max_disp, trigamma_c,
                                           c_d(d_t16), c_d(d_fit_all)))
-                self._tail(d_fitted, d_t16, d_t16 + 9 * 8, 0.0, contrast, ridge, lfc_null, alt_hypothesis, begin, check)
+                self._tail(d_fitted, d_t16, d_t16 + 9 * 8, 0.0, contrast, ridge, lfc_null, alt_hypothesis, begin, check, profile)
                 if self._perm is not None:
                     begin("to_caller_order")
                     self._to_caller_order()
@@ -766,7 +771,7 @@ class ResidentFit:
         # The pass is ~20 launches + copies with no host synchronisation in between: after one eager pass (which allocates
         # every buffer) the identical sequence is captured into a CUDA graph and replayed with a single call.
         key = (fit_type, contrast.tobytes(), float(lfc_null), alt_hypothesis, G, self.with_cooks, n_all, self.fuse_wald, self.use_hint,
-               self.gather, win is not None)
+               self.fuse_tail, self.gather, win is not None)
         # a captured pass holds pointers into context-owned scratch (per-gene status words, trend scratch); host-buffer calls on the
         # same context may have re-allocated it since: the context counts re-allocations, a stale graph is dropped and re-captured
         if events:
@@ -794,6 +799,7 @@ class ResidentFit:
         ctx.sync()  # the only host synchronisation of the pass
         if win is not None:
             win.check()
+        self._check_tail()
         t16 = H["t16"]
         if fit_type == "parametric" and t16[2] == 0.0:
             trend = TrendFit("parametric", np.array([t16[0], t16[1]]), None, int(t16[3]))
@@ -818,12 +824,13 @@ class ResidentFit:
             fit_all[:] = trend.coeffs[0]
             ctx.h2d(d_t16, rec)
             ctx.h2d(d_fit_all, fit_all)
-            self._tail(d_fitted, d_t16, None, prior_var, contrast, ridge, lfc_null, alt_hypothesis, begin, check)
+            self._tail(d_fitted, d_t16, None, prior_var, contrast, ridge, lfc_null, alt_hypothesis, begin, check, profile)
             self._to_caller_order()
             if self.comm is not None:
                 exchange_tables()
             ctx.d2h(self._h_slab, self.d_slab_out)
             ctx.sync()
+            self._check_tail()
         gw = np.clip(H["gw"], self.min_disp, self.max_disp)
         means = H["means"]
         if trend.kind == "parametric":
@@ -989,11 +996,43 @@ class ResidentFit:
         se_o[self._perm], conv_o[self._perm] = se_s, conv_s
         return ShrinkResult(lfc, se_o, conv_o, float(prior_scale), prior_var)
 
-    def _tail(self, d_fitted, d_t16, d_prior_var, prior_var, contrast, ridge, lfc_null, alt_hypothesis, begin, check):
+    def _check_tail(self):
+        """After a stream synchronisation: raise when a tile hand-off of the fused tail launch gave up waiting."""
+        st = C.c_uint64(0)
+        self.ctx.check(self.lib.pdq_map_irls_status(self.ctx.h, C.byref(st)))
+        if st.value:
+            raise RuntimeError(f"MAP -> LFC hand-off: the LFC fit of tile {st.value - 1} never saw its dispersions")
+
+    def _cooks(self, begin, check):
+        """Optional: Cook's distances from the resident mu / hat (dds.py:986-1040); only per-gene results leave the device."""
+        if self.with_cooks:
+            from scipy.stats import f as _f
+
+            L, h, d, G = self.lib, self.ctx.h, self.design, self.G
+            c_d = self._lib_mod.c_dptr
+            begin("cooks")
+            check(L.pdq_cooks_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu), c_d(self.d_hat), G,
+                                  float(_f.ppf(0.99, self.p, self.N - self.p)), None, G, c_d(self.d_robust_disp),
+                                  c_d(self.d_cooks_outlier), c_d(self.d_cooks_replaced)))
+
+    def _tail(self, d_fitted, d_t16, d_prior_var, prior_var, contrast, ridge, lfc_null, alt_hypothesis, begin, check, profile=False):
         """MAP dispersions -> final dispersions -> LFC fit -> Wald, all enqueued without host synchronisation."""
         L, ctx, h, d, G = self.lib, self.ctx, self.ctx.h, self.design, self.G
         c_d = self._lib_mod.c_dptr
         H = self._h
+        if self.fuse_tail and self.fuse_wald and self.use_hint and not profile:
+            # steps 5-7 below with a per-tile dependency: the LFC fit of a gene tile starts when that tile's final dispersions are
+            # written.  Stage timings (profile=True) keep the three launches: overlapping kernels have no stage boundaries to time.
+            check(L.pdq_map_irls_wald_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu_hat), G, c_d(d_fitted), c_d(self.d_gw),
+                                          c_d(self.d_hint), c_d(d_t16), self.min_disp, self.max_disp,
+                                          prior_var if d_prior_var is None else 1.0,
+                                          c_d(d_prior_var) if d_prior_var is not None else None, c_d(self.d_map), c_d(self.d_map_conv),
+                                          c_d(self.d_disp), c_d(self.d_outlier), self.min_mu, self.beta_tol, -30.0, 30.0, 250,
+                                          c_d(self.d_beta), c_d(self.d_mu), c_d(self.d_hat), G, c_d(self.d_conv),
+                                          self._lib_mod.as_f64p(ridge), self._lib_mod.as_f64p(contrast), LN2 * lfc_null,
+                                          self._lib_mod.ALT_CODES[alt_hypothesis], c_d(self.d_pv), c_d(self.d_stat), c_d(self.d_se)))
+            self._cooks(begin, check)
+            return
         # 5. MAP dispersions (dds.py:886-935); the prior variance is read from device memory (written by the trend kernel)
         begin("alpha_mle_map")
         check(L.pdq_alpha_mle_hint_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu_hat), G, c_d(d_fitted), self.min_disp,
@@ -1020,11 +1059,5 @@ class ResidentFit:
             check(L.pdq_wald_test_dev(h, d, c_d(self.d_disp), c_d(self.d_beta), c_d(self.d_mu), G, G,
                                       self._lib_mod.as_f64p(ridge), self._lib_mod.as_f64p(contrast), LN2 * lfc_null,
                                       self._lib_mod.ALT_CODES[alt_hypothesis], c_d(self.d_pv), c_d(self.d_stat), c_d(self.d_se)))
-        # 8. optional: Cook's distances from the resident mu / hat (dds.py:986-1040); only per-gene results leave the device
-        if self.with_cooks:
-            from scipy.stats import f as _f
-
-            begin("cooks")
-            check(L.pdq_cooks_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu), c_d(self.d_hat), G,
-                                  float(_f.ppf(0.99, self.p, self.N - self.p)), None, G, c_d(self.d_robust_disp),
-                                  c_d(self.d_cooks_outlier), c_d(self.d_cooks_replaced)))
+        # 8. optional: Cook's distances
+        self._cooks(begin, check)
