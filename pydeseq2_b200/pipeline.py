@@ -18,6 +18,7 @@ import os
 import time
 import warnings
 from dataclasses import dataclass, field
+from types import SimpleNamespace
 
 import numpy as np
 from scipy.special import polygamma
@@ -119,12 +120,31 @@ class TrendFit:
     fitted: np.ndarray        # fitted dispersion per gene
     n_iter: int = 0
 
+    def at(self, means: np.ndarray) -> np.ndarray:
+        """The trend at the normalised means ``means`` (dds.py:1267-1275); the mean trend is flat."""
+        if self.kind == "parametric":
+            return self.coeffs[0] + self.coeffs[1] / means
+        return np.full(len(means), self.coeffs[0])
+
+
+def mean_dispersion(genewise: np.ndarray, min_disp: float) -> float:
+    """The mean-type trend: trimmed mean of the genewise dispersions above 10 * min_disp (dds.py:1277-1299, :503-505)."""
+    g = np.asarray(genewise, dtype=float)
+    return float(trim_mean(g[g > 10 * min_disp], proportiontocut=0.001))
+
+
+def default_contrast(contrast, p: int) -> np.ndarray:
+    """``contrast`` as a float64 vector; None selects the last coefficient."""
+    if contrast is None:
+        contrast = np.zeros(p)
+        contrast[-1] = 1.0
+    return np.ascontiguousarray(contrast, dtype=np.float64)
+
 
 def fit_trend(inference, normed_means: np.ndarray, genewise: np.ndarray, min_disp: float, fit_type="parametric") -> TrendFit:
     """Dispersion trend (dds.py:799-831): parametric gamma-GLM loop (:1199-1275) or trimmed mean (:1277-1299)."""
     def mean_trend():
-        sel = genewise > 10 * min_disp
-        m = float(trim_mean(genewise[sel], proportiontocut=0.001))
+        m = mean_dispersion(genewise, min_disp)
         return TrendFit("mean", np.array([m, np.nan]), np.full_like(genewise, m))
 
     if fit_type == "mean":
@@ -149,6 +169,18 @@ def fit_trend(inference, normed_means: np.ndarray, genewise: np.ndarray, min_dis
         idx = idx[~((ratio < 1e-4) | (ratio >= 15))]
     fitted = coeffs[0] + coeffs[1] / normed_means
     return TrendFit("parametric", coeffs, fitted, n_iter)
+
+
+def _device_trend(t16: np.ndarray, fit_type: str) -> TrendFit | None:
+    """The parametric trend of the device's trend record ``t16``, or None -- the caller falls back to the mean trend -- for
+    ``fit_type="mean"`` and, after the reference's warning, when the fit did not converge (dds.py:1243-1252)."""
+    if fit_type != "parametric":
+        return None
+    if t16[2] == 0.0:
+        return TrendFit("parametric", np.array([t16[0], t16[1]]), None, int(t16[3]))
+    warnings.warn("The dispersion trend curve fitting did not converge. Switching to a mean-based dispersion trend.",
+                  UserWarning, stacklevel=3)
+    return None
 
 
 def fit_prior_var(genewise: np.ndarray, fitted: np.ndarray, N: int, p: int, min_disp: float):
@@ -192,14 +224,20 @@ def _expand(v, nz, G_all):
     return out
 
 
-def genewise_stage(counts, X, inference, sf, normed, normed_means, min_mu, min_disp, max_disp, beta_tol, fresh=None, timed=None):
+def _as_is(a):
+    return a
+
+
+def _untimed(key, fn, *a, **k):
+    return fn(*a, **k)
+
+
+def genewise_stage(counts, X, inference, sf, normed, normed_means, min_mu, min_disp, max_disp, beta_tol, fresh=_as_is, timed=_untimed):
     """``fit_genewise_dispersions`` (dds.py:713-797) after the size factors: all-zero mask, method-of-moments start values
     (dds.py:1140-1162), initial mu_hat by ``lin_reg_mu`` or ``irls``, genewise ``alpha_mle``.  ``max_disp`` is the caller's
     ``max(max_disp, N)``.  Returns ``(non_zero, counts of the non-zero genes, their normalised means, mom, mu_hat,
-    initial-fit converged flags, genewise dispersions (clipped), genewise converged flags)``.  Shared by :func:`fit_host` and
-    ``workflow.vst``."""
-    fresh = fresh if fresh is not None else (lambda a: a)
-    timed = timed if timed is not None else (lambda key, fn, *a, **k: fn(*a, **k))
+    initial-fit converged flags, genewise dispersions (clipped), genewise converged flags)``.  Shared by :func:`fit_host`, the
+    outlier refit and ``workflow.vst``."""
     # dds.py:729-731 `~(X == 0).all(0)`.  Counts are non-negative, so a gene is all-zero exactly when the mean of its normalised
     # counts is 0: with var["_normed_means"] at hand (dds.py:708) the mask costs O(G) instead of a pass over the (N, G) matrix.
     normed_means = normed.mean(0) if normed_means is None else np.asarray(normed_means)
@@ -221,6 +259,21 @@ def genewise_stage(counts, X, inference, sf, normed, normed_means, min_mu, min_d
     gw, gw_conv = timed("alpha_mle_genewise", inference.alpha_mle, fresh(c), X, fresh(mu_hat), mom, min_disp, max_disp)
     gw = np.clip(gw, min_disp, max_disp)                 # dds.py:792-794
     return nz, c, normed_means, mom, mu_hat, init_conv, gw, gw_conv
+
+
+def map_lfc_stage(c, X, inference, sf, mu_hat, gw, fitted, prior_var, sq, min_mu, min_disp, max_disp, beta_tol, fresh=_as_is,
+                  timed=_untimed):
+    """After the trend, on the genes of :func:`genewise_stage`: MAP dispersions, final dispersions (dds.py:886-935) and the LFC
+    fit (dds.py:937-984).  ``fitted``: the trend at the genes' means.  Returns ``(map, map converged, final dispersions, lfc, mu,
+    hat diagonals, lfc converged)``.  Shared by :func:`fit_host` and the outlier refit."""
+    mp, mp_conv = timed("alpha_mle_map", inference.alpha_mle, fresh(c), X, fresh(mu_hat), fitted, min_disp, max_disp,
+                        prior_disp_var=prior_var, cr_reg=True, prior_reg=True)
+    mp = np.clip(mp, min_disp, max_disp)
+    disp = mp.copy()
+    outlier = np.log(gw) > np.log(fitted) + 2 * np.sqrt(sq)   # dds.py:926-932
+    disp[outlier] = gw[outlier]
+    lfc, mu_lfc, hat, lfc_conv = timed("irls_lfc", inference.irls, fresh(c), sf, X, disp, min_mu, beta_tol)
+    return mp, mp_conv, disp, lfc, mu_lfc, hat, lfc_conv
 
 
 def fit_host(counts, X, inference, contrast=None, size_factors=None, min_mu=0.5, min_disp=1e-8, max_disp=10.0,
@@ -261,9 +314,7 @@ def fit_host(counts, X, inference, contrast=None, size_factors=None, min_mu=0.5,
     N, G_all = counts.shape
     p = X.shape[1]
     max_disp = max(max_disp, N)  # dds.py:312
-    if contrast is None:
-        contrast = np.zeros(p)
-        contrast[-1] = 1.0
+    contrast = default_contrast(contrast, p)
     if size_factors is None:
         normed, sf = timed("size_factors", median_of_ratios, counts)
     else:
@@ -289,15 +340,9 @@ def fit_host(counts, X, inference, contrast=None, size_factors=None, min_mu=0.5,
         trend = timed("trend", fit_trend, inference, means_all, gw_all, min_disp, fit_type)
         sq, prior_var = timed("prior", fit_prior_var, gw_all, trend.fitted, N, p, min_disp)
     if comm is not None:
-        local = (trend.coeffs[0] + trend.coeffs[1] / normed_means) if trend.kind == "parametric" else np.full_like(gw, trend.coeffs[0])
-        trend = TrendFit(trend.kind, trend.coeffs, local, trend.n_iter)
-    mp, mp_conv = timed("alpha_mle_map", inference.alpha_mle, fresh(c), X, fresh(mu_hat), trend.fitted, min_disp, max_disp,
-                        prior_disp_var=prior_var, cr_reg=True, prior_reg=True)
-    mp = np.clip(mp, min_disp, max_disp)
-    disp = mp.copy()
-    outlier = np.log(gw) > np.log(trend.fitted) + 2 * np.sqrt(sq)   # dds.py:926-932
-    disp[outlier] = gw[outlier]
-    lfc, mu_lfc, hat, lfc_conv = timed("irls_lfc", inference.irls, fresh(c), sf, X, disp, min_mu, beta_tol)
+        trend = TrendFit(trend.kind, trend.coeffs, trend.at(normed_means), trend.n_iter)
+    mp, mp_conv, disp, lfc, mu_lfc, hat, lfc_conv = map_lfc_stage(c, X, inference, sf, mu_hat, gw, trend.fitted, prior_var, sq, min_mu,
+                                                                  min_disp, max_disp, beta_tol, fresh, timed)
 
     # Wald stage on ALL genes, all-zero genes carry NaN (ds.py:320-347)
     lfc_all = _expand(np.asarray(lfc), nz, G_all)
@@ -311,8 +356,8 @@ def fit_host(counts, X, inference, contrast=None, size_factors=None, min_mu=0.5,
         mu_w = np.exp(X @ lfc_all.T) * sf[:, None]
     T["wald_mu_host"] = T.get("wald_mu_host", 0.0) + time.perf_counter() - t0
     ridge = np.diag(np.repeat(1e-6, p))
-    pv, st, se = timed("wald_test", inference.wald_test, X, disp_all, lfc_all, fresh(mu_w), ridge, np.asarray(contrast, float),
-                       LN2 * lfc_null, alt_hypothesis)
+    pv, st, se = timed("wald_test", inference.wald_test, X, disp_all, lfc_all, fresh(mu_w), ridge, contrast, LN2 * lfc_null,
+                       alt_hypothesis)
     return FitResult(sf, nz, mom, gw, np.asarray(gw_conv), trend, prior_var, sq, mp, np.asarray(mp_conv), disp_all,
                      lfc_all, np.asarray(lfc_conv), np.asarray(pv), np.asarray(st), np.asarray(se), T,
                      np.asarray(init_conv, dtype=float), mu_lfc, hat, normed_means)
@@ -392,13 +437,11 @@ class ResidentFit:
         self.comm = comm
         self.with_cooks = with_cooks  # also compute Cook's distances (per-gene outlier flags) after the LFC fit
         self.use_graph = True         # replay the pass as one CUDA graph after the first eager pass
-        self.fuse_wald = True         # Wald test inside the LFC-fit launch (False: the two plugin-shaped calls in sequence)
         self.gather = comm is not None  # end the pass with the all-gather of the result tables of all gene shards
-        self.use_hint = True          # MAP dispersion search opened from the genewise optimum + curvature (pdq_alpha_mle_hint_dev)
         # MAP search, final dispersions and LFC fit + Wald test with a per-tile dependency instead of three grid-wide ones
-        # (pdq_map_irls_wald_dev; needs fuse_wald and use_hint): the fit's kernel becomes resident while the search's last tiles
-        # run.  Bit-identical results; the entry point keeps the three launches where a warp has many tiles per launch.  False: the
-        # three launches always (the reference of tests/test_gpu_fused_tail.py and scripts/tail_bench.py)
+        # (pdq_map_irls_wald_dev): the fit's kernel becomes resident while the search's last tiles run.  Bit-identical results; the
+        # entry point keeps the three launches where a warp has many tiles per launch.  False: the three launches always (the
+        # reference of tests/test_gpu_fused_tail.py and scripts/tail_bench.py)
         self.fuse_tail = True
         # how gene shards exchange: "peer" = one kernel per exchange storing into every peer's HBM over NVLink (sharding.PeerWindow),
         # "nccl" = grouped NCCL all-gathers, "auto" = peer when the ranks can map each other's memory (one node), else NCCL
@@ -443,7 +486,7 @@ class ResidentFit:
         sf = np.empty(self.N)
         ctl = control_mask(self.control_genes, self.G)
         if kind == "ratio" and ctl is None:
-            self.ctx.check(self.lib.pdq_size_factors_dev(self.ctx.h, c_d(self.d_counts), self.G, self.N, self.G, c_d(d_sf), None))
+            self.ctx.check(self.lib.pdq_size_factors_dev(self.ctx.h, c_d(self._main.counts), self.G, self.N, self.G, c_d(d_sf), None))
             self.ctx.d2h(sf, d_sf)
             self.ctx.sync()
             if not np.isfinite(sf).all():
@@ -456,7 +499,7 @@ class ResidentFit:
             d_ctl = self._dev("sf_control", self.G)
             self.ctx.h2d(d_ctl, ctl.astype(np.uint8))
         d_lm = self._dev("sf_logmeans", self.G * 8)
-        self.ctx.check(self.lib.pdq_size_factors_ex_dev(self.ctx.h, c_d(self.d_counts), self.G, self.N, self.G, size_factor_kind(kind),
+        self.ctx.check(self.lib.pdq_size_factors_ex_dev(self.ctx.h, c_d(self._main.counts), self.G, self.N, self.G, size_factor_kind(kind),
                                                         c_d(d_ctl) if d_ctl else None, c_d(d_sf), c_d(d_lm)))
         lm = np.empty(self.G)
         self.ctx.d2h(sf, d_sf)
@@ -466,7 +509,7 @@ class ResidentFit:
             raise ValueError("Every gene contains at least one zero, cannot compute log geometric means.")
         if not np.isfinite(sf).all():  # the error path only: the counts come back to name the samples
             counts = np.empty((self.N, self.G), dtype=np.int64)
-            self.ctx.d2h(counts, self.d_counts)
+            self.ctx.d2h(counts, self._main.counts)
             self.ctx.sync()
             check_size_factors(sf, counts, lm, kind, ctl)
         self._set_size_factors(sf)
@@ -480,6 +523,15 @@ class ResidentFit:
                 self.ctx.free(cur[0])
             self._bufs[name] = (self.ctx.malloc(nbytes), nbytes)
         return self._bufs[name][0]
+
+    def _gene_set(self, prefix: str, G: int, d_vec: int, stride: int, names) -> SimpleNamespace:
+        """Device pointers of one gene set, what the stages of a pass read and write: the (N, G) ``counts``, ``mu_hat``, ``mu`` and
+        ``hat`` diagonals, the MAP search's ``hint`` and the IRLS start values ``beta0`` in buffers named ``prefix + name``; the
+        per-gene vectors ``names``, then the (G, p) LFCs ``beta``, ``stride`` doubles apart from ``d_vec``."""
+        ng = self.N * G * 8
+        return SimpleNamespace(G=G, **{k: self._dev(prefix + k, ng) for k in ("counts", "mu_hat", "mu", "hat")},
+                               hint=self._dev(prefix + "hint", 2 * G * 8), beta0=self._dev(prefix + "beta0", G * self.p * 8),
+                               beta=d_vec + len(names) * stride * 8, **{k: d_vec + i * stride * 8 for i, k in enumerate(names)})
 
     def upload(self, counts: np.ndarray):
         """H2D of this shard's counts (genes that are all-zero must already be dropped, dds.py:729-731)."""
@@ -507,10 +559,6 @@ class ResidentFit:
         self.G = G
         G, N, p = self.G, self.N, self.p
         ng = N * G * 8
-        self.d_counts = self._dev("counts", ng)
-        self.d_mu_hat = self._dev("mu_hat", ng)
-        self.d_mu = self._dev("mu", ng)
-        self.d_hat = self._dev("hat", ng)
         # every per-gene result lives in ONE device slab mirrored by one page-locked host block: a pass ends with a single
         # device-to-host copy instead of a dozen small ones.  With gene shards every vector is laid out with the LARGEST shard's
         # length `Gs` and NaN behind this shard's last gene (written here, once): the slab then is directly the send
@@ -521,25 +569,23 @@ class ResidentFit:
         assert Gs >= G
         total = self._slab_len = len(per_gene) * Gs + Gs * p + 16
         self.d_slab = self._dev("slab", total * 8)
+        gs = self._main = self._gene_set("", G, self.d_slab, Gs, per_gene)
         self._h_slab = self.ctx.pinned_empty((total,))
         self._h_slab[:] = np.nan
         self._h = {}
         self._slab_off = {}
         off = 0
         for name in per_gene:
-            setattr(self, "d_" + name, self.d_slab + off * 8)
             self._h[name] = self._h_slab[off:off + G]
             self._slab_off[name] = (off, 1)
             off += Gs
-        self.d_beta, self._h["beta"] = self.d_slab + off * 8, self._h_slab[off:off + G * p].reshape(G, p)
+        self._h["beta"] = self._h_slab[off:off + G * p].reshape(G, p)
         self._slab_off["beta"] = (off, p)
         off += Gs * p
         self.d_t16, self._h["t16"] = self.d_slab + off * 8, self._h_slab[off:off + 16]
         self._off_beta, self._off_t16, self._n_vec = off - Gs * p, off, len(per_gene)
         self._h_slab[off:off + 16] = 0.0
         self.ctx.h2d(self.d_slab, self._h_slab)  # NaN pads (and zeros) land on the device once
-        for name, n in (("fitted", G), ("beta0", G * p), ("hint", 2 * G)):
-            setattr(self, "d_" + name, self._dev(name, n * 8))
         self.d_nfb = self._dev("nfb", 64)
         c_d = self._lib_mod.c_dptr
         self._perm = self._inv = None
@@ -560,18 +606,17 @@ class ResidentFit:
                 self.d_perm = self._dev("perm", G * 4)
                 self.ctx.h2d(self.d_perm, perm)
                 # 8-byte words are moved as they are: the same gather serves int64 counts and float64 arrays
-                self.ctx.check(self.lib.pdq_gather_columns_dev(self.ctx.h, c_d(d_raw), G, N, c_d(self.d_perm), G, c_d(self.d_counts), G))
+                self.ctx.check(self.lib.pdq_gather_columns_dev(self.ctx.h, c_d(d_raw), G, N, c_d(self.d_perm), G, c_d(gs.counts), G))
                 self.ctx.sync()
             finally:
                 self.ctx.free(d_raw)
             self.d_slab_out = self._dev("slab_out", total * 8)  # the results in the caller's gene order
             self.ctx.h2d(self.d_slab_out, self._h_slab)
         else:
-            fill(self.d_counts)
+            fill(gs.counts)
         self.ctx.sync()
         if self.design is None:
             self.device_size_factors()
-        self._h["fitted"] = self.ctx.pinned_empty((G,))
 
     def _to_caller_order(self):
         """Enqueue the scatter of the pass' per-gene results from the device's gene order into the caller's (no-op when unsorted)."""
@@ -624,40 +669,39 @@ class ResidentFit:
             self.design = None
 
     # -- one pass ----------------------------------------------------------------------------------
-    def _enqueue_genewise(self, check, begin):
-        """Steps 1-3 of a pass (``fit_genewise_dispersions``, dds.py:713-797), enqueued without synchronising."""
-        L, h, d, G = self.lib, self.ctx.h, self.design, self.G
+    def _enqueue_genewise(self, gs, check, begin):
+        """Steps 1-3 of a pass (``fit_genewise_dispersions``, dds.py:713-797) on the gene set ``gs``, enqueued without
+        synchronising."""
+        L, h, d, G = self.lib, self.ctx.h, self.design, gs.G
         c_d = self._lib_mod.c_dptr
         # 1. method-of-moments start values + normalised means (dds.py:1140-1162, :708)
         begin("mom_dispersions")
         #    -- and, on the lin_reg_mu branch (dds.py:747-756), the initial mu_hat from the same projection
-        check(L.pdq_mom_dispersions_dev(h, d, c_d(self.d_counts), G, G, self.min_disp, self.max_disp, c_d(self.d_mom),
-                                        c_d(self.d_means), self.min_mu, c_d(self.d_mu_hat) if self.lin_branch else None, G))
+        check(L.pdq_mom_dispersions_dev(h, d, c_d(gs.counts), G, G, self.min_disp, self.max_disp, c_d(gs.mom),
+                                        c_d(gs.means), self.min_mu, c_d(gs.mu_hat) if self.lin_branch else None, G))
         # 2. initial mu_hat by IRLS otherwise (dds.py:757-765)
         if not self.lin_branch:
             begin("irls_init")
-            check(L.pdq_irls_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mom), self.min_mu, self.beta_tol, -30.0, 30.0,
-                                 250, c_d(self.d_beta0), c_d(self.d_mu_hat), c_d(self.d_hat), G, c_d(self.d_conv),
-                                 c_d(self.d_nfb)))
+            check(L.pdq_irls_dev(h, d, c_d(gs.counts), G, G, c_d(gs.mom), self.min_mu, self.beta_tol, -30.0, 30.0,
+                                 250, c_d(gs.beta0), c_d(gs.mu_hat), c_d(gs.hat), G, c_d(gs.conv), c_d(self.d_nfb)))
         # 3. genewise dispersions (dds.py:778-797)
         begin("alpha_mle_genewise")
         #    (its optimum and curvature per gene are kept on the device: the MAP search of step 5 opens from them)
-        check(L.pdq_alpha_mle_hint_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu_hat), G, c_d(self.d_mom), self.min_disp,
-                                       self.max_disp, 1.0, None, 1, 0, c_d(self.d_gw), c_d(self.d_gw_conv), None,
-                                       c_d(self.d_hint) if self.use_hint else None))
+        check(L.pdq_alpha_mle_hint_dev(h, d, c_d(gs.counts), G, G, c_d(gs.mu_hat), G, c_d(gs.mom), self.min_disp,
+                                       self.max_disp, 1.0, None, 1, 0, c_d(gs.gw), c_d(gs.gw_conv), None, c_d(gs.hint)))
 
     def vst_dispersions(self, fit_type="parametric"):
         """The fit stage of ``vst_fit`` (dds.py:384-436) on the resident counts: steps 1-3 of :meth:`run` and the dispersion
         trend (dds.py:1199-1299), then stop.  Returns ``(kind, coeffs, genewise)``: the final kind (``"mean"`` also after a
         parametric trend that did not converge, with the reference's warning), ``(a0, a1)`` or ``(mean_disp,)``, and the clipped
         genewise dispersions in the uploaded gene order.  Only per-gene vectors come back; :meth:`run`'s graph is left alone."""
-        ctx, c_d = self.ctx, self._lib_mod.c_dptr
-        self._enqueue_genewise(ctx.check, lambda name: None)
+        ctx, c_d, gs = self.ctx, self._lib_mod.c_dptr, self._main
+        self._enqueue_genewise(gs, ctx.check, lambda name: None)
         if fit_type == "parametric":
-            ctx.check(self.lib.pdq_trend_fit_dev(ctx.h, c_d(self.d_means), c_d(self.d_gw), self.G, self.min_disp, self.max_disp,
+            ctx.check(self.lib.pdq_trend_fit_dev(ctx.h, c_d(gs.means), c_d(gs.gw), self.G, self.min_disp, self.max_disp,
                                                  float(polygamma(1, (self.N - self.p) / 2)), c_d(self.d_t16), None))
         gw = ctx.pinned_empty((self.G,))
-        ctx.d2h(gw, self.d_gw)
+        ctx.d2h(gw, gs.gw)
         t16 = ctx.pinned_empty((16,))
         ctx.d2h(t16, self.d_t16)
         ctx.sync()
@@ -666,13 +710,10 @@ class ResidentFit:
             out = np.empty_like(gw)
             out[self._perm] = gw
             gw = out
-        if fit_type == "parametric" and t16[2] == 0.0:
-            return "parametric", np.array([t16[0], t16[1]]), gw
-        if fit_type == "parametric":
-            warnings.warn("The dispersion trend curve fitting did not converge. Switching to a mean-based dispersion trend.",
-                          UserWarning, stacklevel=2)
-        sel = gw > 10 * self.min_disp
-        return "mean", np.array([float(trim_mean(gw[sel], proportiontocut=0.001))]), gw
+        trend = _device_trend(t16, fit_type)
+        if trend is not None:
+            return "parametric", trend.coeffs, gw
+        return "mean", np.array([mean_dispersion(gw, self.min_disp)]), gw
 
     def run(self, contrast=None, lfc_null=0.0, alt_hypothesis=None, fit_type="parametric", profile=False, copy=True, events=None):
         """One pass of the hot path.  Every stage is enqueued on the context's stream back to back -- the trend and
@@ -700,11 +741,9 @@ class ResidentFit:
                 ctx.sync()
                 ctx.record(2)
 
-        if contrast is None:
-            contrast = np.zeros(p)
-            contrast[-1] = 1.0
-        contrast = np.ascontiguousarray(contrast, dtype=np.float64)
-        ridge = np.ascontiguousarray(np.diag(np.repeat(1e-6, p)))
+        gs = self._main
+        contrast = default_contrast(contrast, p)
+        fused = self.fuse_tail and not profile  # stage timings need the three launches: overlapping kernels have no boundaries
         trigamma_c = float(polygamma(1, (N - p) / 2))
         W = self.comm.world if self.comm is not None else 1
         rank = self.comm.rank if self.comm is not None else 0
@@ -720,14 +759,14 @@ class ResidentFit:
             d_gw_all, d_means_all = self._dev("gw_all", n_all * 8), self._dev("means_all", n_all * 8)
             d_table_all = self._dev("table_all", W * self._slab_len * 8) if self.gather else None
         else:
-            d_gw_all, d_means_all, d_table_all = self.d_gw, self.d_means, None
+            d_gw_all, d_means_all, d_table_all = gs.gw, gs.means, None
         self._d_table_all = d_table_all
 
         def exchange_vectors():
             if win is not None:
-                win.push([(self.d_gw, off_gw), (self.d_means, off_means)], m)
+                win.push([(gs.gw, off_gw), (gs.means, off_means)], m)
             else:
-                self.comm.allgather_dev([(self.d_gw, d_gw_all), (self.d_means, d_means_all)], m)
+                self.comm.allgather_dev([(gs.gw, d_gw_all), (gs.means, d_means_all)], m)
 
         def exchange_tables():
             if win is not None:  # without a table exchange the pass still ends with the barrier: a fast rank must not store the
@@ -740,7 +779,7 @@ class ResidentFit:
         d_fitted = d_fit_all + rank * m * 8  # this shard's slice of the fitted curve
 
         def enqueue():
-            self._enqueue_genewise(check, begin)  # steps 1-3
+            self._enqueue_genewise(gs, check, begin)  # steps 1-3
             # 4. trend + prior: global over ALL genes of ALL shards (dds.py:799-884).  With gene shards the per-gene
             #    vectors are exchanged first, device to device (peer-memory push kernel or grouped NCCL all-gathers); the fit itself
             #    is one launch (a thread-block cluster, or a cooperative grid from 65 536 genes).
@@ -753,7 +792,8 @@ class ResidentFit:
                 begin("trend_prior")
                 check(L.pdq_trend_fit_dev(h, c_d(d_means_all), c_d(d_gw_all), n_all, self.min_disp, self.max_disp, trigamma_c,
                                           c_d(d_t16), c_d(d_fit_all)))
-                self._tail(d_fitted, d_t16, d_t16 + 9 * 8, 0.0, contrast, ridge, lfc_null, alt_hypothesis, begin, check, profile)
+                self._tail(gs, d_fitted, d_t16 + 9 * 8, 0.0, contrast, lfc_null, alt_hypothesis, begin, check, fused)
+                self._cooks(begin, check)
                 if self._perm is not None:
                     begin("to_caller_order")
                     self._to_caller_order()
@@ -770,8 +810,8 @@ class ResidentFit:
 
         # The pass is ~20 launches + copies with no host synchronisation in between: after one eager pass (which allocates
         # every buffer) the identical sequence is captured into a CUDA graph and replayed with a single call.
-        key = (fit_type, contrast.tobytes(), float(lfc_null), alt_hypothesis, G, self.with_cooks, n_all, self.fuse_wald, self.use_hint,
-               self.fuse_tail, self.gather, win is not None)
+        key = (fit_type, contrast.tobytes(), float(lfc_null), alt_hypothesis, G, self.with_cooks, n_all, self.fuse_tail, self.gather,
+               win is not None)
         # a captured pass holds pointers into context-owned scratch (per-gene status words, trend scratch); host-buffer calls on the
         # same context may have re-allocated it since: the context counts re-allocations, a stale graph is dropped and re-captured
         if events:
@@ -801,14 +841,11 @@ class ResidentFit:
             win.check()
         self._check_tail()
         t16 = H["t16"]
-        if fit_type == "parametric" and t16[2] == 0.0:
-            trend = TrendFit("parametric", np.array([t16[0], t16[1]]), None, int(t16[3]))
+        trend = _device_trend(t16, fit_type)
+        if trend is not None:
             sq, prior_var = float(t16[8]), float(t16[9])
         else:
             # dds.py:1243-1252 / fit_type="mean": trimmed-mean trend on the host (global, G-length), then the tail again
-            if fit_type == "parametric":
-                warnings.warn("The dispersion trend curve fitting did not converge. Switching to a mean-based dispersion trend.",
-                              UserWarning, stacklevel=2)
             A = ctx.pinned_empty((2, n_all))
             ctx.d2h(A[0], d_gw_all)
             ctx.d2h(A[1], d_means_all)
@@ -824,7 +861,8 @@ class ResidentFit:
             fit_all[:] = trend.coeffs[0]
             ctx.h2d(d_t16, rec)
             ctx.h2d(d_fit_all, fit_all)
-            self._tail(d_fitted, d_t16, None, prior_var, contrast, ridge, lfc_null, alt_hypothesis, begin, check, profile)
+            self._tail(gs, d_fitted, None, prior_var, contrast, lfc_null, alt_hypothesis, begin, check, fused)
+            self._cooks(begin, check)
             self._to_caller_order()
             if self.comm is not None:
                 exchange_tables()
@@ -833,11 +871,9 @@ class ResidentFit:
             self._check_tail()
         gw = np.clip(H["gw"], self.min_disp, self.max_disp)
         means = H["means"]
+        fitted = trend.at(means)
         if trend.kind == "parametric":
-            fitted = trend.coeffs[0] + trend.coeffs[1] / means
             trend = TrendFit("parametric", trend.coeffs, fitted, trend.n_iter)
-        else:
-            fitted = np.full(G, trend.coeffs[0])
         # the slab is reused by the next pass: hand out copies (a result dict must survive later run() calls)
         cp = np.array if copy else (lambda v: v)
         return {"mom": cp(H["mom"]), "genewise": gw, "genewise_converged": cp(H["gw_conv"]), "trend": trend, "prior_var": prior_var,
@@ -872,10 +908,7 @@ class ResidentFit:
             out[key] = full.reshape(-1, w) if w > 1 else full
         out["genewise"] = np.clip(out["genewise"], self.min_disp, self.max_disp)
         out["map"] = np.clip(out["map"], self.min_disp, self.max_disp)
-        if result["trend"].kind == "parametric":
-            out["fitted"] = result["trend"].coeffs[0] + result["trend"].coeffs[1] / out["normed_means"]
-        else:
-            out["fitted"] = np.full(len(out["normed_means"]), result["trend"].coeffs[0])
+        out["fitted"] = result["trend"].at(out["normed_means"])
         for k in ("cooks_outlier", "cooks_replaced"):
             if k in out and k in names:
                 out[k] = out[k] == 1.0
@@ -894,7 +927,7 @@ class ResidentFit:
             return out
         d_idx, d_out = self._dev("gather_idx", R * 4), self._dev("gather_out", self.N * R * 8)
         self.ctx.h2d(d_idx, idx)
-        src = {"mu": self.d_mu, "hat": self.d_hat}[which]
+        src = {"mu": self._main.mu, "hat": self._main.hat}[which]
         c_d = self._lib_mod.c_dptr
         self.ctx.check(self.lib.pdq_gather_columns_dev(self.ctx.h, c_d(src), self.G, self.N, c_d(d_idx), R, c_d(d_out), R))
         self.ctx.d2h(out, d_out)
@@ -902,59 +935,34 @@ class ResidentFit:
         return out
 
     def refit_subset(self, sub_counts: np.ndarray, trend: "TrendFit", prior_var: float, contrast=None, lfc_null=0.0, alt_hypothesis=None):
-        """``_refit_without_outliers`` (dds.py:1393-1458) for a few genes whose outlier counts were replaced: the same kernels as
+        """``_refit_without_outliers`` (dds.py:1393-1458) for a few genes whose outlier counts were replaced: the stages of
         :meth:`run` on the compact (N, R) matrix -- genewise dispersions from scratch, the main fit's trend FUNCTION and prior
         (neither is re-estimated; the trend record of the last pass is still on the device), MAP dispersions, LFCs, Wald test.
-        Returns R-length per-gene results."""
-        L, ctx, h, d = self.lib, self.ctx, self.ctx.h, self.design
-        c_d = self._lib_mod.c_dptr
+        The tail always takes the three launches.  Returns R-length per-gene results."""
+        ctx = self.ctx
         sub = np.ascontiguousarray(sub_counts, dtype=np.int64)
-        N, p = self.N, self.p
         R = sub.shape[1]
-        assert sub.shape[0] == N and R > 0
-        if contrast is None:
-            contrast = np.zeros(p)
-            contrast[-1] = 1.0
-        contrast = np.ascontiguousarray(contrast, dtype=np.float64)
-        ridge = np.ascontiguousarray(np.diag(np.repeat(1e-6, p)))
-        ng = N * R * 8
-        dv = lambda name, nbytes: self._dev("refit_" + name, nbytes)  # noqa: E731
-        d_c, d_muhat, d_mu, d_hat = dv("counts", ng), dv("mu_hat", ng), dv("mu", ng), dv("hat", ng)
-        names = ("mom", "means", "gw", "gw_conv", "fitted", "map", "map_conv", "disp", "outl", "conv", "pv", "stat", "se")
-        d_vec = dv("vec", (len(names) + p) * R * 8)
-        dptr = {k: d_vec + i * R * 8 for i, k in enumerate(names)}
-        d_beta = d_vec + len(names) * R * 8
-        d_beta0 = dv("beta0", R * p * 8)
-        ctx.h2d(d_c, sub)
-        check = ctx.check
-        check(L.pdq_mom_dispersions_dev(h, d, c_d(d_c), R, R, self.min_disp, self.max_disp, c_d(dptr["mom"]), c_d(dptr["means"]),
-                                        self.min_mu, c_d(d_muhat) if self.lin_branch else None, R))
-        if not self.lin_branch:
-            check(L.pdq_irls_dev(h, d, c_d(d_c), R, R, c_d(dptr["mom"]), self.min_mu, self.beta_tol, -30.0, 30.0, 250, c_d(d_beta0),
-                                 c_d(d_muhat), c_d(d_hat), R, c_d(dptr["conv"]), c_d(self.d_nfb)))
-        d_hint = dv("hint", 2 * R * 8)
-        check(L.pdq_alpha_mle_hint_dev(h, d, c_d(d_c), R, R, c_d(d_muhat), R, c_d(dptr["mom"]), self.min_disp, self.max_disp, 1.0, None, 1, 0,
-                                       c_d(dptr["gw"]), c_d(dptr["gw_conv"]), None, c_d(d_hint)))
+        assert sub.shape[0] == self.N and R > 0
+        names = ("mom", "means", "gw", "gw_conv", "fitted", "map", "map_conv", "disp", "outlier", "conv", "pv", "stat", "se")
+        d_vec = self._dev("refit_vec", (len(names) + self.p) * R * 8)
+        gs = self._gene_set("refit_", R, d_vec, R, names)
+        ctx.h2d(gs.counts, sub)
+        no_stage = lambda name: None  # noqa: E731
+        self._enqueue_genewise(gs, ctx.check, no_stage)
         means = np.empty(R)
-        ctx.d2h(means, dptr["means"])
+        ctx.d2h(means, gs.means)
         ctx.sync()
         with np.errstate(divide="ignore"):
-            fitted = (trend.coeffs[0] + trend.coeffs[1] / means) if trend.kind == "parametric" else np.full(R, trend.coeffs[0])
-        ctx.h2d(dptr["fitted"], np.ascontiguousarray(fitted))
-        check(L.pdq_alpha_mle_hint_dev(h, d, c_d(d_c), R, R, c_d(d_muhat), R, c_d(dptr["fitted"]), self.min_disp, self.max_disp,
-                                       float(prior_var), None, 1, 1, c_d(dptr["map"]), c_d(dptr["map_conv"]), c_d(d_hint), None))
-        check(L.pdq_select_dispersions_dev(h, c_d(dptr["gw"]), c_d(dptr["map"]), c_d(dptr["fitted"]), c_d(self.d_t16), R, self.min_disp,
-                                           self.max_disp, c_d(dptr["disp"]), c_d(dptr["outl"])))
-        check(L.pdq_irls_wald_dev(h, d, c_d(d_c), R, R, c_d(dptr["disp"]), self.min_mu, self.beta_tol, -30.0, 30.0, 250, c_d(d_beta),
-                                  c_d(d_mu), c_d(d_hat), R, c_d(dptr["conv"]), c_d(self.d_nfb), self._lib_mod.as_f64p(ridge),
-                                  self._lib_mod.as_f64p(contrast), LN2 * lfc_null, self._lib_mod.ALT_CODES[alt_hypothesis],
-                                  c_d(dptr["pv"]), c_d(dptr["stat"]), c_d(dptr["se"])))
-        host = np.empty((len(names) + p) * R)
+            fitted = trend.at(means)
+        ctx.h2d(gs.fitted, np.ascontiguousarray(fitted))
+        self._tail(gs, gs.fitted, None, float(prior_var), default_contrast(contrast, self.p), lfc_null, alt_hypothesis, no_stage,
+                   ctx.check, False)
+        host = np.empty((len(names) + self.p) * R)
         ctx.d2h(host, d_vec)
         ctx.sync()
         v = {k: host[i * R:(i + 1) * R] for i, k in enumerate(names)}
         return {"normed_means": means, "genewise": np.clip(v["gw"], self.min_disp, self.max_disp), "fitted": fitted, "disp": v["disp"],
-                "lfc": host[len(names) * R:].reshape(R, p), "pvalue": v["pv"], "stat": v["stat"], "se": v["se"]}
+                "lfc": host[len(names) * R:].reshape(R, self.p), "pvalue": v["pv"], "stat": v["stat"], "se": v["se"]}
 
     # -- apeGLM shrinkage on the resident counts ----------------------------------------------------------
     def lfc_shrink(self, result, coeff_idx: int, adapt: bool = True, se=None, prior_scale=None):
@@ -982,7 +990,7 @@ class ResidentFit:
         d_size, d_out = self._dev("shrink_size", G * 8), self._dev("shrink_out", G * (p + p * p + 1) * 8)
         d_status = self._dev("shrink_status", G * 4)
         ctx.h2d(d_size, size)
-        ctx.check(L.pdq_lfc_shrink_dev(h, self.design, c_d(self.d_counts), G, G, c_d(d_size), 15.0, float(prior_scale), int(coeff_idx),
+        ctx.check(L.pdq_lfc_shrink_dev(h, self.design, c_d(self._main.counts), G, G, c_d(d_size), 15.0, float(prior_scale), int(coeff_idx),
                                        c_d(d_out), c_d(d_out + G * p * 8), c_d(d_out + G * (p + p * p) * 8), c_d(d_status)))
         ctx.d2h(host[G:], d_out)
         ctx.sync()
@@ -1008,56 +1016,41 @@ class ResidentFit:
         if self.with_cooks:
             from scipy.stats import f as _f
 
-            L, h, d, G = self.lib, self.ctx.h, self.design, self.G
+            L, h, d, G, gs = self.lib, self.ctx.h, self.design, self.G, self._main
             c_d = self._lib_mod.c_dptr
             begin("cooks")
-            check(L.pdq_cooks_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu), c_d(self.d_hat), G,
-                                  float(_f.ppf(0.99, self.p, self.N - self.p)), None, G, c_d(self.d_robust_disp),
-                                  c_d(self.d_cooks_outlier), c_d(self.d_cooks_replaced)))
+            check(L.pdq_cooks_dev(h, d, c_d(gs.counts), G, G, c_d(gs.mu), c_d(gs.hat), G,
+                                  float(_f.ppf(0.99, self.p, self.N - self.p)), None, G, c_d(gs.robust_disp),
+                                  c_d(gs.cooks_outlier), c_d(gs.cooks_replaced)))
 
-    def _tail(self, d_fitted, d_t16, d_prior_var, prior_var, contrast, ridge, lfc_null, alt_hypothesis, begin, check, profile=False):
-        """MAP dispersions -> final dispersions -> LFC fit -> Wald, all enqueued without host synchronisation."""
-        L, ctx, h, d, G = self.lib, self.ctx, self.ctx.h, self.design, self.G
-        c_d = self._lib_mod.c_dptr
-        H = self._h
-        if self.fuse_tail and self.fuse_wald and self.use_hint and not profile:
+    def _tail(self, gs, d_fitted, d_prior_var, prior_var, contrast, lfc_null, alt_hypothesis, begin, check, fused):
+        """MAP dispersions -> final dispersions -> LFC fit -> Wald on the gene set ``gs``, enqueued without host synchronisation.
+        The prior variance is read from ``d_prior_var`` on the device, or is ``prior_var`` when that is None.  ``fused``: the
+        kernel pair of ``pdq_map_irls_wald_dev`` instead of the three launches."""
+        L, h, d, G = self.lib, self.ctx.h, self.design, gs.G
+        c_d, f64p = self._lib_mod.c_dptr, self._lib_mod.as_f64p
+        ridge = np.ascontiguousarray(np.diag(np.repeat(1e-6, self.p)))
+        prior = (prior_var, None) if d_prior_var is None else (1.0, c_d(d_prior_var))
+        wald = (f64p(ridge), f64p(contrast), LN2 * lfc_null, self._lib_mod.ALT_CODES[alt_hypothesis], c_d(gs.pv), c_d(gs.stat),
+                c_d(gs.se))
+        if fused:
             # steps 5-7 below with a per-tile dependency: the LFC fit of a gene tile starts when that tile's final dispersions are
-            # written.  Stage timings (profile=True) keep the three launches: overlapping kernels have no stage boundaries to time.
-            check(L.pdq_map_irls_wald_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu_hat), G, c_d(d_fitted), c_d(self.d_gw),
-                                          c_d(self.d_hint), c_d(d_t16), self.min_disp, self.max_disp,
-                                          prior_var if d_prior_var is None else 1.0,
-                                          c_d(d_prior_var) if d_prior_var is not None else None, c_d(self.d_map), c_d(self.d_map_conv),
-                                          c_d(self.d_disp), c_d(self.d_outlier), self.min_mu, self.beta_tol, -30.0, 30.0, 250,
-                                          c_d(self.d_beta), c_d(self.d_mu), c_d(self.d_hat), G, c_d(self.d_conv),
-                                          self._lib_mod.as_f64p(ridge), self._lib_mod.as_f64p(contrast), LN2 * lfc_null,
-                                          self._lib_mod.ALT_CODES[alt_hypothesis], c_d(self.d_pv), c_d(self.d_stat), c_d(self.d_se)))
-            self._cooks(begin, check)
+            # written
+            check(L.pdq_map_irls_wald_dev(h, d, c_d(gs.counts), G, G, c_d(gs.mu_hat), G, c_d(d_fitted), c_d(gs.gw), c_d(gs.hint),
+                                          c_d(self.d_t16), self.min_disp, self.max_disp, *prior, c_d(gs.map), c_d(gs.map_conv),
+                                          c_d(gs.disp), c_d(gs.outlier), self.min_mu, self.beta_tol, -30.0, 30.0, 250, c_d(gs.beta),
+                                          c_d(gs.mu), c_d(gs.hat), G, c_d(gs.conv), *wald))
             return
-        # 5. MAP dispersions (dds.py:886-935); the prior variance is read from device memory (written by the trend kernel)
+        # 5. MAP dispersions (dds.py:886-935), opened from the genewise optimum and curvature
         begin("alpha_mle_map")
-        check(L.pdq_alpha_mle_hint_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_mu_hat), G, c_d(d_fitted), self.min_disp,
-                                       self.max_disp, prior_var if d_prior_var is None else 1.0,
-                                       c_d(d_prior_var) if d_prior_var is not None else None, 1, 1, c_d(self.d_map), c_d(self.d_map_conv),
-                                       c_d(self.d_hint) if self.use_hint else None, None))
+        check(L.pdq_alpha_mle_hint_dev(h, d, c_d(gs.counts), G, G, c_d(gs.mu_hat), G, c_d(d_fitted), self.min_disp, self.max_disp,
+                                       *prior, 1, 1, c_d(gs.map), c_d(gs.map_conv), c_d(gs.hint), None))
         # final dispersions: clip(MAP), outlier genes keep the genewise value (dds.py:918-932)
         begin("select_dispersions")
-        check(L.pdq_select_dispersions_dev(h, c_d(self.d_gw), c_d(self.d_map), c_d(d_fitted), c_d(d_t16), G, self.min_disp,
-                                           self.max_disp, c_d(self.d_disp), c_d(self.d_outlier)))
+        check(L.pdq_select_dispersions_dev(h, c_d(gs.gw), c_d(gs.map), c_d(d_fitted), c_d(self.d_t16), G, self.min_disp,
+                                           self.max_disp, c_d(gs.disp), c_d(gs.outlier)))
         # 6. + 7. LFC fit (dds.py:937-984: beta, mu (unclamped), hat diagonal stay on the device) and the Wald test of its
         #    coefficients (ds.py:303-360) in ONE launch: the test's X^T W X is the last IRLS sweep's, so mu is not read again
-        begin("irls_lfc_wald" if self.fuse_wald else "irls_lfc")
-        if self.fuse_wald:
-            check(L.pdq_irls_wald_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_disp), self.min_mu, self.beta_tol, -30.0, 30.0, 250,
-                                      c_d(self.d_beta), c_d(self.d_mu), c_d(self.d_hat), G, c_d(self.d_conv), c_d(self.d_nfb),
-                                      self._lib_mod.as_f64p(ridge), self._lib_mod.as_f64p(contrast), LN2 * lfc_null,
-                                      self._lib_mod.ALT_CODES[alt_hypothesis], c_d(self.d_pv), c_d(self.d_stat), c_d(self.d_se)))
-        else:
-            check(L.pdq_irls_dev(h, d, c_d(self.d_counts), G, G, c_d(self.d_disp), self.min_mu, self.beta_tol, -30.0, 30.0, 250,
-                                 c_d(self.d_beta), c_d(self.d_mu), c_d(self.d_hat), G, c_d(self.d_conv), c_d(self.d_nfb)))
-            # mu = sf * exp(X beta) is exactly the mu the LFC fit just wrote (unclamped)
-            begin("wald_test")
-            check(L.pdq_wald_test_dev(h, d, c_d(self.d_disp), c_d(self.d_beta), c_d(self.d_mu), G, G,
-                                      self._lib_mod.as_f64p(ridge), self._lib_mod.as_f64p(contrast), LN2 * lfc_null,
-                                      self._lib_mod.ALT_CODES[alt_hypothesis], c_d(self.d_pv), c_d(self.d_stat), c_d(self.d_se)))
-        # 8. optional: Cook's distances
-        self._cooks(begin, check)
+        begin("irls_lfc_wald")
+        check(L.pdq_irls_wald_dev(h, d, c_d(gs.counts), G, G, c_d(gs.disp), self.min_mu, self.beta_tol, -30.0, 30.0, 250,
+                                  c_d(gs.beta), c_d(gs.mu), c_d(gs.hat), G, c_d(gs.conv), c_d(self.d_nfb), *wald))

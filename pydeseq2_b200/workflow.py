@@ -21,10 +21,9 @@ from math import ceil, floor
 import warnings
 
 import numpy as np
-from scipy.stats import trim_mean
 
-from .pipeline import (LN2, FitResult, check_size_factors, filtered_genes, fit_host, fit_shrink_prior_var, fit_trend, genewise_stage,
-                       lin_mu_branch, size_factor_kind, size_factors_numpy)
+from .pipeline import (LN2, FitResult, check_size_factors, default_contrast, filtered_genes, fit_host, fit_shrink_prior_var, fit_trend,
+                       genewise_stage, map_lfc_stage, mean_dispersion, size_factor_kind, size_factors_numpy)
 
 
 def n_or_more_replicates(X: np.ndarray, min_replicates: int) -> np.ndarray:
@@ -148,12 +147,7 @@ def deseq2_results(counts, X, inference, contrast=None, size_factors=None, refit
     X = np.ascontiguousarray(X, dtype=np.float64)
     N, G = counts.shape
     p = X.shape[1]
-    if contrast is None:
-        contrast = np.zeros(p)
-        contrast[-1] = 1.0
-    contrast = np.asarray(contrast, dtype=float)
-    if lfc_null < 0 and alt_hypothesis in ("greaterAbs", "lessAbs"):
-        raise ValueError(f"The alternative hypothesis being {alt_hypothesis}, please provide a positive lfc_null value (got {lfc_null}).")
+    contrast = _test_arguments(contrast, p, lfc_null, alt_hypothesis)
     if comm is not None and size_factors is None:
         raise ValueError("gene shards: size factors are per sample and global over genes -- pass them in")
     if size_factors is None and (size_factors_fit_type != "ratio" or control_genes is not None):
@@ -167,6 +161,7 @@ def deseq2_results(counts, X, inference, contrast=None, size_factors=None, refit
     base_mean = np.zeros(G)
     base_mean[nz] = fit.normed_means                     # all-zero genes have mean 0
     pv, stat, se = fit.pvalue.copy(), fit.stat.copy(), fit.se.copy()
+    tables = dict(normed_means=base_mean, lfc=lfc, genewise=genewise, fitted=fitted, disp=disp, pvalue=pv, stat=stat, se=se)
 
     # ---- Cook's distances (dds.py:986-1040) on the non-zero genes
     c_nz = counts if nz.all() else np.ascontiguousarray(counts[:, nz])
@@ -184,39 +179,20 @@ def deseq2_results(counts, X, inference, contrast=None, size_factors=None, refit
         if replaceable.any():
             replaced = above.any(axis=0)
         if replaced.any():
-            sub = counts[:, replaced].copy()
-            base = trimmed_mean_rows(sub / sf[:, None], 0.2)
-            repl = (base[None, :] * sf[:, None]).astype(int)   # truncation towards zero, like DataFrame.astype(int)
-            mask = replaceable[:, None] & above[:, replaced]
-            sub[mask] = repl[mask]
-            zero_now = (sub == 0).all(axis=0)
+            new, zero_now = _replace_counts(counts[:, replaced], sf, replaceable[:, None] & above[:, replaced])
             ridx = np.flatnonzero(replaced)
             new_zero[ridx[zero_now]] = True
             refitted[ridx[~zero_now]] = True
-            base_mean[new_zero] = 0.0
-            lfc[new_zero] = 0.0
+            r = None
             if refitted.any():
-                r = _refit_subset(np.ascontiguousarray(sub[:, ~zero_now]), X, sf, inference, fit, min_mu, min_disp, max_disp, beta_tol)
-                base_mean[refitted], lfc[refitted] = r["normed_means"], r["lfc"]
-                genewise[refitted], fitted[refitted], disp[refitted] = r["genewise"], r["fitted"], r["disp"]
+                r = _refit_subset(np.ascontiguousarray(new[:, ~zero_now]), X, sf, inference, fit, contrast, lfc_null, alt_hypothesis,
+                                  min_mu, min_disp, max_disp, beta_tol)
                 replace_cooks = cooks.copy()
                 replace_cooks[np.ix_(replaceable, refitted)] = 0.0
-                # Wald statistics of the refitted genes (per-gene independent: same as re-running run_wald_test on every gene)
-                mu_r = np.exp(X @ r["lfc"].T) * sf[:, None]
-                pv[refitted], stat[refitted], se[refitted] = inference.wald_test(
-                    X, r["disp"], r["lfc"], mu_r, np.diag(np.repeat(1e-6, p)), contrast, LN2 * lfc_null, alt_hypothesis)
-            if new_zero.any():
-                # run_wald_test (ds.py:355-360) on genes whose replacement made them all-zero
-                se[new_zero], stat[new_zero], pv[new_zero] = 0.0, 0.0, 1.0
+            _merge_refit(tables, refitted, new_zero, r)
 
     # ---- which genes lose their p-value (dds.py:1066-1110)
-    use_for_max = n_or_more_replicates(X, 3)
-    src = replace_cooks if (refit_cooks and refitted.any() and replace_cooks is not None) else cooks
-    outlier = (src[use_for_max] > cutoff).any(axis=0)
-    if outlier.any():
-        pos = cooks[:, outlier].argmax(0)
-        top = counts[:, outlier][pos, np.arange(len(pos))]
-        outlier[outlier] = (counts[:, outlier] > top).sum(0) < 3
+    outlier = _cooks_outlier(cooks if replace_cooks is None else replace_cooks, cooks, counts, X, cutoff)
     if cooks_filter:
         pv[outlier] = np.nan
 
@@ -239,6 +215,48 @@ def deseq2_results(counts, X, inference, contrast=None, size_factors=None, refit
         se[nz] = np.sqrt(np.abs(np.asarray(ih)[:, k, k]))
         res.lfc, res.log2_fold_change, res.lfc_se, res.shrink_prior_scale = lfc, lfc[:, k] / LN2, se / LN2, scale
     return res
+
+
+def _test_arguments(contrast, p, lfc_null, alt_hypothesis) -> np.ndarray:
+    """The drivers' contrast (default: the last coefficient); raises for a negative ``lfc_null`` with an ``*Abs`` alternative."""
+    contrast = default_contrast(contrast, p)
+    if lfc_null < 0 and alt_hypothesis in ("greaterAbs", "lessAbs"):
+        raise ValueError(f"The alternative hypothesis being {alt_hypothesis}, please provide a positive lfc_null value (got {lfc_null}).")
+    return contrast
+
+
+def _replace_counts(sub, sf, mask):
+    """``_replace_outliers`` (dds.py:1301-1358) on the (N, R) counts of the replaced genes: the entries of ``mask`` become the
+    gene's trimmed mean of normalised counts times the sample's size factor.  Returns (new counts, genes now all zero)."""
+    base = trimmed_mean_rows(sub / sf[:, None], 0.2)
+    repl = (base[None, :] * sf[:, None]).astype(int)   # truncation towards zero, like DataFrame.astype(int)
+    new = sub.copy()
+    new[mask] = repl[mask]
+    return new, (new == 0).all(axis=0)
+
+
+def _cooks_outlier(flag_cooks, cooks, counts, X, cutoff):
+    """``cooks_outlier`` (dds.py:1066-1110): genes with a Cook's distance of ``flag_cooks`` above ``cutoff`` in a sample of a
+    design cell with at least 3 replicates, unless fewer than 3 samples have more counts than the sample of the gene's largest
+    distance in ``cooks``."""
+    outlier = (flag_cooks[n_or_more_replicates(X, 3)] > cutoff).any(axis=0)
+    if outlier.any():
+        pos = cooks[:, outlier].argmax(0)
+        c = counts[:, outlier]
+        outlier[outlier] = (c > c[pos, np.arange(len(pos))]).sum(0) < 3
+    return outlier
+
+
+def _merge_refit(tables, refitted, new_zero, refit):
+    """Write an outlier refit over ``tables`` (G-length arrays under the keys of the refit's result, changed in place): the rows of
+    the ``refitted`` genes from ``refit`` (None when no gene was refitted), and for genes that the replacement made all zero base
+    mean 0, LFC 0 and the test of an all-zero gene, se 0, stat 0, p 1 (ds.py:355-360)."""
+    if refit is not None:
+        for k, v in tables.items():
+            v[refitted] = refit[k]
+    tables["normed_means"][new_zero] = 0.0
+    tables["lfc"][new_zero] = 0.0
+    tables["se"][new_zero], tables["stat"][new_zero], tables["pvalue"][new_zero] = 0.0, 0.0, 1.0
 
 
 def _adjust(base_mean, pv, independent_filter, alpha, comm=None):
@@ -272,12 +290,7 @@ def deseq2_results_resident(rf, contrast=None, refit_cooks=True, min_replicates=
 
     X, N, p, G = rf.X, rf.N, rf.p, rf.G
     sf = rf.sf
-    if contrast is None:
-        contrast = np.zeros(p)
-        contrast[-1] = 1.0
-    contrast = np.asarray(contrast, dtype=float)
-    if lfc_null < 0 and alt_hypothesis in ("greaterAbs", "lessAbs"):
-        raise ValueError(f"The alternative hypothesis being {alt_hypothesis}, please provide a positive lfc_null value (got {lfc_null}).")
+    contrast = _test_arguments(contrast, p, lfc_null, alt_hypothesis)
     was = rf.with_cooks
     rf.with_cooks = True
     try:
@@ -288,6 +301,7 @@ def deseq2_results_resident(rf, contrast=None, refit_cooks=True, min_replicates=
     lfc, disp = np.array(r["lfc"]), np.array(r["dispersions"])
     genewise, fitted = np.array(r["genewise"]), np.array(r["fitted"])
     pv, stat, se = np.array(r["pvalue"]), np.array(r["stat"]), np.array(r["se"])
+    tables = dict(normed_means=base_mean, lfc=lfc, genewise=genewise, fitted=fitted, disp=disp, pvalue=pv, stat=stat, se=se)
     outlier = np.array(r["cooks_outlier"], dtype=bool)
     cutoff = f_dist.ppf(0.99, p, N - p)
     replaced, refitted, new_zero = np.zeros(G, bool), np.zeros(G, bool), np.zeros(G, bool)
@@ -297,43 +311,25 @@ def deseq2_results_resident(rf, contrast=None, refit_cooks=True, min_replicates=
             replaced = np.array(r["cooks_replaced"], dtype=bool)
         if replaced.any():
             ridx = np.flatnonzero(replaced)
-            counts = rf._h_counts
-            sub = np.ascontiguousarray(counts[:, ridx])
+            sub = np.ascontiguousarray(rf._h_counts[:, ridx])
             mu, hat = rf.gather_columns("mu", ridx), rf.gather_columns("hat", ridx)
             # Cook's distances of the replaced genes (dds.py:1022-1036) from the resident mu / hat and the device's robust dispersions
             a = np.asarray(r["robust_dispersions"])[ridx]
             V = mu + a[None, :] * mu**2
             ck = (sub - mu) ** 2 / V / p * (hat / (1 - hat) ** 2)
-            above = ck > cutoff
-            base = trimmed_mean_rows(sub / sf[:, None], 0.2)
-            repl = (base[None, :] * sf[:, None]).astype(int)   # truncation towards zero, like DataFrame.astype(int)
-            mask = replaceable[:, None] & above
-            new = sub.copy()
-            new[mask] = repl[mask]
-            zero_now = (new == 0).all(axis=0)
+            new, zero_now = _replace_counts(sub, sf, replaceable[:, None] & (ck > cutoff))
             new_zero[ridx[zero_now]] = True
             refitted[ridx[~zero_now]] = True
-            base_mean[new_zero] = 0.0
-            lfc[new_zero] = 0.0
+            q = None
             if refitted.any():
                 q = rf.refit_subset(np.ascontiguousarray(new[:, ~zero_now]), r["trend"], r["prior_var"], contrast, lfc_null, alt_hypothesis)
-                base_mean[refitted], lfc[refitted] = q["normed_means"], q["lfc"]
-                genewise[refitted], fitted[refitted], disp[refitted] = q["genewise"], q["fitted"], q["disp"]
-                pv[refitted], stat[refitted], se[refitted] = q["pvalue"], q["stat"], q["se"]
                 # which refitted genes still lose their p-value (dds.py:1066-1110 on `replace_cooks`: distances of the replaceable
                 # samples are zeroed for refitted genes): samples in cells of 3..min_replicates-1 replicates can still flag them
-                use_for_max = n_or_more_replicates(X, 3)
                 keep = ~zero_now
                 ck_r = ck[:, keep].copy()
                 ck_r[replaceable] = 0.0
-                out_r = (ck_r[use_for_max] > cutoff).any(axis=0)
-                if out_r.any():
-                    pos = ck[:, keep][:, out_r].argmax(0)
-                    top = sub[:, keep][:, out_r][pos, np.arange(len(pos))]
-                    out_r[out_r] = (sub[:, keep][:, out_r] > top).sum(0) < 3
-                outlier[ridx[keep]] = out_r
-            if new_zero.any():
-                se[new_zero], stat[new_zero], pv[new_zero] = 0.0, 0.0, 1.0   # ds.py:355-360
+                outlier[ridx[keep]] = _cooks_outlier(ck_r, ck[:, keep], sub[:, keep], X, cutoff)
+            _merge_refit(tables, refitted, new_zero, q)
     if cooks_filter:
         pv[outlier] = np.nan
     nz = np.ones(G, bool)
@@ -500,12 +496,6 @@ def _fit_size_factors(counts, inference, fit_type="ratio", control_genes=None):
     return normed, sf, lm
 
 
-def mean_dispersion(genewise: np.ndarray, min_disp: float) -> float:
-    """Dispersion of the ``"mean"`` transform: trimmed mean of the genewise dispersions above 10 * min_disp (dds.py:503-505)."""
-    g = np.asarray(genewise, dtype=float)
-    return float(trim_mean(g[g > 10 * min_disp], proportiontocut=0.001))
-
-
 def vst(counts, X, inference, fit_type="parametric", use_design=False, size_factors=None, logmeans=None, min_mu=0.5, min_disp=1e-8,
         max_disp=10.0, beta_tol=1e-8, transform=True, size_factors_fit_type="ratio", control_genes=None) -> VstFit:
     """``DeseqDataSet.vst(use_design, fit_type)`` (dds.py:349-436) on bare arrays: median-of-ratios size factors unless
@@ -617,23 +607,16 @@ def vst_resident(inference, counts, X, fit_type="parametric", use_design=False, 
     return VstFit(sf, logmeans, filtered, kind, coeffs, _full(gw, nz, G), nz, out, inference)
 
 
-def _refit_subset(sub, X, sf, inference, fit: FitResult, min_mu, min_disp, max_disp, beta_tol):
-    """``_refit_without_outliers`` (dds.py:1393-1458) on the replaced counts: genewise dispersions from scratch, the SAME trend
-    function and prior as the main fit (neither is re-estimated), MAP dispersions, LFCs."""
-    normed = sub / sf[:, None]
-    mom = np.clip(np.minimum(inference.fit_rough_dispersions(normed, X), inference.fit_moments_dispersions(normed, sf)), min_disp, max_disp)
-    if lin_mu_branch(X):
-        mu_hat = inference.lin_reg_mu(sub, sf, X, min_mu)
-    else:
-        mu_hat = inference.irls(sub, sf, X, mom, min_mu, beta_tol)[1]
-    mu_hat = np.ascontiguousarray(mu_hat)
-    gw = np.clip(inference.alpha_mle(sub, X, mu_hat, mom, min_disp, max_disp)[0], min_disp, max_disp)
-    means = normed.mean(0)
-    co = fit.trend.coeffs
-    fitted = (co[0] + co[1] / means) if fit.trend.kind == "parametric" else np.full(len(means), co[0])
-    mp = inference.alpha_mle(sub, X, mu_hat, fitted, min_disp, max_disp, prior_disp_var=fit.prior_var, cr_reg=True, prior_reg=True)[0]
-    disp = np.clip(mp, min_disp, max_disp)
-    keep_gw = np.log(gw) > np.log(fitted) + 2 * np.sqrt(fit.squared_logres)
-    disp[keep_gw] = gw[keep_gw]
-    lfc = np.asarray(inference.irls(sub, sf, X, disp, min_mu, beta_tol)[0])
-    return {"normed_means": means, "genewise": gw, "fitted": fitted, "disp": disp, "lfc": lfc}
+def _refit_subset(sub, X, sf, inference, fit: FitResult, contrast, lfc_null, alt_hypothesis, min_mu, min_disp, max_disp, beta_tol):
+    """``_refit_without_outliers`` (dds.py:1393-1458) on the replaced counts, through the main fit's stages: genewise dispersions
+    from scratch, the SAME trend function and prior as the main fit (neither is re-estimated), MAP dispersions, LFCs, then the
+    Wald test of the refitted genes (per-gene independent: the same as re-running run_wald_test on every gene)."""
+    _, c, means, _, mu_hat, _, gw, _ = genewise_stage(sub, X, inference, sf, sub / sf[:, None], None, min_mu, min_disp, max_disp,
+                                                      beta_tol)
+    fitted = fit.trend.at(means)
+    disp, lfc = map_lfc_stage(c, X, inference, sf, mu_hat, gw, fitted, fit.prior_var, fit.squared_logres, min_mu, min_disp, max_disp,
+                              beta_tol)[2:4]
+    lfc = np.asarray(lfc)
+    mu = np.exp(X @ lfc.T) * sf[:, None]
+    pv, stat, se = inference.wald_test(X, disp, lfc, mu, np.diag(np.repeat(1e-6, X.shape[1])), contrast, LN2 * lfc_null, alt_hypothesis)
+    return {"normed_means": means, "genewise": gw, "fitted": fitted, "disp": disp, "lfc": lfc, "pvalue": pv, "stat": stat, "se": se}
