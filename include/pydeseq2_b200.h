@@ -236,6 +236,24 @@ int pdq_size_factors_from_logmeans(pdq_ctx* ctx, const int64_t* counts, int64_t 
 int pdq_vst_transform(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, const double* size_factors, int kind, double c0,
                       double c1, double* out, int64_t ld_out);
 
+/* Multiple testing -- DeseqStats._independent_filtering / _p_value_adjustment (ds.py:486-542) for K rows of p-values on one set
+ * of base means.  `pvalues` (K, G) with row pitch ld, each entry in [0, 1] or NaN (NaN = not tested); an entry outside [0, 1]
+ * fails the call with PDQ_ERR_INVALID, as scipy.stats.false_discovery_control raises.  Every result is numpy's / scipy's bit
+ * for bit: each row is sorted by p once on the device, and the BH value of rank r in a set of m tested genes is p * (m / r).
+ *
+ * pdq_padj_rejections: `cutoffs_out` (n_theta,) = np.quantile(base_mean, theta) (method "linear"); `num_rej_out` (K, n_theta)
+ * = the number of genes of row k whose BH-adjusted p-value over {g : base_mean[g] >= cutoff[i], p[k, g] not NaN} is below alpha.
+ * 1 <= n_theta <= 64.
+ * pdq_padj_bh: `padj_out` (K, ld_out) = the BH-adjusted p-values of row k over {g : base_mean[g] >= cutoff[k], p not NaN}, NaN
+ * outside that set; cutoff[k] = -inf is plain BH over every tested gene, whatever its base mean.
+ *
+ * A NaN base mean makes every quantile NaN, as in numpy, so no gene passes any cutoff.  K <= 0, G <= 0, ld < G or ld_out < G:
+ * PDQ_ERR_INVALID. */
+int pdq_padj_rejections(pdq_ctx* ctx, const double* base_mean, int G, const double* pvalues, int64_t ld, int K, const double* theta,
+                        int n_theta, double alpha, double* cutoffs_out, int* num_rej_out);
+int pdq_padj_bh(pdq_ctx* ctx, const double* base_mean, int G, const double* pvalues, int64_t ld, int K, const double* cutoff,
+                double* padj_out, int64_t ld_out);
+
 /* Cook's distances -- DeseqDataSet.calculate_cooks (dds.py:986-1040) with the trimmed-moments dispersion
  * (utils.py:914-960; cells = identical design rows with >= 3 replicates) -- and the two per-gene decisions derived from them:
  * `outlier_out` = the p-value filter of cooks_outlier() (dds.py:1066-1110, no prior refit), `replaced_out` = any distance above

@@ -115,6 +115,9 @@ _SIGNATURES = {
                                     C.c_int64]),
     "pdq_vst_transform_dev": (C.c_int, [c_ctx, c_dptr, C.c_int64, C.c_int, C.c_int, c_dptr, C.c_int, C.c_double, C.c_double,
                                         c_dptr, C.c_int64]),
+    "pdq_padj_rejections": (C.c_int, [c_ctx, f64p, C.c_int, f64p, C.c_int64, C.c_int, f64p, C.c_int, C.c_double, f64p,
+                                       C.POINTER(C.c_int)]),
+    "pdq_padj_bh": (C.c_int, [c_ctx, f64p, C.c_int, f64p, C.c_int64, C.c_int, f64p, f64p, C.c_int64]),
     "pdq_dispersion_trend_gamma_glm": (C.c_int, [c_ctx, f64p, f64p, C.c_size_t, f64p, f64p, C.POINTER(C.c_int)]),
     "pdq_trend_prior": (C.c_int, [c_ctx, f64p, f64p, C.c_size_t, C.c_double, C.c_double, C.c_double, f64p, f64p]),
     "pdq_trend_fit_dev": (C.c_int, [c_ctx, c_dptr, c_dptr, C.c_size_t, C.c_double, C.c_double, C.c_double, c_dptr, c_dptr]),

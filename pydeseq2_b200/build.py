@@ -13,11 +13,11 @@ OUT = os.path.join(HERE, "libpydeseq2_b200.so")
 # translation units: (source, object tag, extra defines).  pdq_kernels.cu is compiled once for p = 1..8 and once per wide design
 # width p = 9..16 (see the note at its top); the units are independent and compile in parallel.
 WIDE_P = tuple(range(9, 17))
-UNITS = [("pdq_api.cu", "pdq_api", ()), ("pdq_dispatch.cu", "pdq_dispatch", ()), ("pdq_io.cpp", "pdq_io", ()), ("pdq_kernels.cu", "pdq_kernels_p1to8", ())] + \
+UNITS = [("pdq_api.cu", "pdq_api", ()), ("pdq_dispatch.cu", "pdq_dispatch", ()), ("pdq_io.cpp", "pdq_io", ()), ("pdq_padj.cu", "pdq_padj", ()), ("pdq_kernels.cu", "pdq_kernels_p1to8", ())] + \
         [("pdq_kernels.cu", f"pdq_kernels_p{p}", (f"-DPDQ_TU_P={p}", "-Xptxas", "-O1")) for p in WIDE_P]
 # (ptxas -O1 for the wide widths: 12 s instead of 85 s per unit; their kernels keep the small matrices in local memory anyway)
 SOURCES = sorted({u[0] for u in UNITS})
-HEADERS = ["pdq_math.cuh", "pdq_fast.cuh", "pdq_tables.h", "pdq_trend.cuh", "pdq_gene.cuh", "pdq_shrink.cuh", "pdq_vst.cuh", "pdq_internal.h",
+HEADERS = ["pdq_math.cuh", "pdq_fast.cuh", "pdq_tables.h", "pdq_trend.cuh", "pdq_gene.cuh", "pdq_shrink.cuh", "pdq_vst.cuh", "pdq_padj.cuh", "pdq_internal.h",
            "pdq_host_linalg.h", os.path.join("..", "..", "include", "pydeseq2_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-fopenmp", "--expt-relaxed-constexpr"]

@@ -19,6 +19,7 @@
 
 #include "pdq_internal.h"
 #include "pdq_host_linalg.h"
+#include "pdq_padj.cuh"
 
 using namespace pdq;
 
@@ -122,7 +123,7 @@ struct NcclApi {
 };
 static const int kNcclFloat64 = 8;  // ncclDataType_t::ncclFloat64 (stable across NCCL 2.x)
 
-enum { kBufCounts, kBufA, kBufB, kBufC, kBufD, kBufE, kBufF, kBufG, kBufStatus, kBufMisc, kBufKeep, kBufRes, kNumBufs };
+enum { kBufCounts, kBufA, kBufB, kBufC, kBufD, kBufE, kBufF, kBufG, kBufStatus, kBufMisc, kBufKeep, kBufRes, kBufPadj, kNumBufs };
 
 struct DesignCacheEntry {
     pdq_design* d = nullptr;
@@ -1720,6 +1721,59 @@ extern "C" int pdq_trend_prior(pdq_ctx* c, const double* means, const double* ge
     if (fitted_out) CU(c, cudaMemcpyAsync(fitted_out, df, n * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     return PDQ_OK;
+}
+
+// --------------------------------------------------------------------------------------------- multiple testing (ds.py:486-542)
+// Host vectors in and out; the device scratch is one context buffer of its own (pdq_padj.cu, padj_layout).
+static int padj_begin(pdq_ctx* c, const double* base_mean, int G, const double* pvalues, int64_t ld, int K, int n_theta, PadjScratch* s) {
+    void* base;
+    if (int e = ensure(c, kBufPadj, padj_layout(G, K, n_theta, nullptr, s), &base)) return e;
+    padj_layout(G, K, n_theta, base, s);
+    if (int e = vec_h2d(c, s->bm, base_mean, (size_t)G * 8)) return e;
+    return h2d_2d(c, s->keys_in, pvalues, ld, K, G, 8);
+}
+
+static int padj_end(pdq_ctx* c, const PadjScratch& s, int K, const char* what) {
+    int bad = 0;
+    CU(c, cudaMemcpyAsync(&bad, s.counters + K, sizeof bad, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    if (bad) return fail(c, PDQ_ERR_INVALID, "%s: %d p-value(s) outside [0, 1]", what, bad);
+    return PDQ_OK;
+}
+
+extern "C" int pdq_padj_rejections(pdq_ctx* c, const double* base_mean, int G, const double* pvalues, int64_t ld, int K,
+                                   const double* theta, int n_theta, double alpha, double* cutoffs_out, int* num_rej_out) {
+    CHECK_CTX(c);
+    if (!base_mean || !pvalues || !theta || !cutoffs_out || !num_rej_out || G <= 0 || K <= 0 || ld < G || n_theta <= 0 ||
+        n_theta > kPadjMaxTheta)
+        return fail(c, PDQ_ERR_INVALID, "pdq_padj_rejections: bad arguments (G=%d, K=%d, ld=%lld, n_theta=%d)", G, K, (long long)ld,
+                    n_theta);
+    PadjScratch s;
+    if (int e = padj_begin(c, base_mean, G, pvalues, ld, K, n_theta, &s)) return e;
+    if (int e = vec_h2d(c, s.theta, theta, (size_t)n_theta * 8)) return e;
+    if (int e = done(c, launch_padj_rejections(c->stream, s, G, K, n_theta, alpha), "padj_rejections")) return e;
+    if (int e = vec_d2h(c, cutoffs_out, s.cutoffs, (size_t)n_theta * 8)) return e;
+    if (int e = vec_d2h(c, num_rej_out, s.num_rej, (size_t)K * n_theta * sizeof(int))) return e;
+    return padj_end(c, s, K, "pdq_padj_rejections");
+}
+
+extern "C" int pdq_padj_bh(pdq_ctx* c, const double* base_mean, int G, const double* pvalues, int64_t ld, int K, const double* cutoff,
+                           double* padj_out, int64_t ld_out) {
+    CHECK_CTX(c);
+    if (!base_mean || !pvalues || !cutoff || !padj_out || G <= 0 || K <= 0 || ld < G || ld_out < G)
+        return fail(c, PDQ_ERR_INVALID, "pdq_padj_bh: bad arguments (G=%d, K=%d, ld=%lld, ld_out=%lld)", G, K, (long long)ld,
+                    (long long)ld_out);
+    PadjScratch s;
+    if (int e = padj_begin(c, base_mean, G, pvalues, ld, K, 1, &s)) return e;
+    if (int e = vec_h2d(c, s.row_cutoff, cutoff, (size_t)K * 8)) return e;
+    double* d_out = (double*)s.keys_in;  // free once the rows are sorted
+    if (int e = done(c, launch_padj_bh(c->stream, s, G, K, d_out, G), "padj_bh")) return e;
+    if (ld_out == G) {
+        if (int e = copy_d2h(c, padj_out, d_out, (size_t)K * G * 8)) return e;
+    } else {
+        CU(c, cudaMemcpy2DAsync(padj_out, (size_t)ld_out * 8, d_out, (size_t)G * 8, (size_t)G * 8, K, cudaMemcpyDeviceToHost, c->stream));
+    }
+    return padj_end(c, s, K, "pdq_padj_bh");
 }
 
 // --------------------------------------------------------------------------------------------- NCCL gene-shard exchange

@@ -115,6 +115,28 @@ int launch_vst_transform(const LaunchCfg&, const int64_t* counts, int64_t ld, in
 int launch_select_disp(const LaunchCfg&, const double* gw, const double* mp, const double* fitted, const double* out16,
                        size_t n, double lo, double hi, double* disp, double* outlier);
 
+// multiple testing (pdq_padj.cu): device scratch of one call over K rows of G p-values, carved by padj_layout from one buffer
+struct PadjScratch {
+    uint64_t *keys_in, *keys;  // (K, G): the p-values as uploaded, then the sort keys; sorted.  keys_in takes pdq_padj_bh's output
+    int *vals_in, *vals;       // (K, G) gene indices, sorted with the keys
+    double *bm, *bm_sorted;    // (G,) base means
+    uint64_t* masks;           // (G,) bit i: base mean >= cutoff i
+    int* counters;             // K set sizes, then the count of p-values outside [0, 1]
+    double *theta, *cutoffs;   // kPadjMaxTheta each
+    double* row_cutoff;        // (K,) pdq_padj_bh's cutoffs
+    int *num_rej, *totals;     // (K, n_theta)
+    int* chunk_counts;         // (K, n_theta, chunks)
+    double *chunk_min, *suffix;  // (K, chunks)
+    void* temp;                // cub's temporary storage
+    size_t temp_bytes;
+};
+// bytes of the scratch (base may be NULL: sizes only); fills `s` with pointers into `base`
+size_t padj_layout(int G, int K, int n_theta, void* base, PadjScratch* s);
+// inputs in s.bm, s.keys_in (raw p-values), s.theta; outputs s.cutoffs, s.num_rej, s.counters[K] (p-values outside [0, 1])
+int launch_padj_rejections(cudaStream_t, const PadjScratch& s, int G, int K, int n_theta, double alpha);
+// inputs in s.bm, s.keys_in, s.row_cutoff; output `padj` (K, ld_out) device, which may be s.keys_in
+int launch_padj_bh(cudaStream_t, const PadjScratch& s, int G, int K, double* padj, int64_t ld_out);
+
 // largest dynamic shared memory a kernel of this library may ask for (H100: 227 KB per CTA)
 constexpr size_t kMaxDynSmem = 227 * 1024;
 

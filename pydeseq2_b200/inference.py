@@ -112,8 +112,8 @@ def _rows(a, dtype, name):
 class _CudaOps:
     """Raw ops on numpy buffers through the C ABI (host-buffer entry points)."""
 
-    def __init__(self, device=0, lanes_per_gene=0, pinned_outputs=True):
-        self.ctx = _lib.Context(device)
+    def __init__(self, device=0, lanes_per_gene=0, pinned_outputs=True, ctx=None):
+        self.ctx = ctx if ctx is not None else _lib.Context(device)  # ctx: share an existing context (its device and stream)
         self.lib = self.ctx.lib
         self.pinned_outputs = pinned_outputs
         self.h2d_bytes = 0  # bytes the calls below asked the library to copy in / out (bench.py `e2e`)
@@ -220,6 +220,16 @@ class _CudaOps:
         return coeffs, pred, bool(ok.value)
 
 
+    def padj_rejections(self, base_mean, G, pv, ld, K, theta, n_theta, alpha, cutoffs, num_rej):
+        """pdq_padj_rejections: `num_rej` int32 (K, n_theta)."""
+        self._io((base_mean, pv, theta), (cutoffs, num_rej))
+        self.ctx.check(self.lib.pdq_padj_rejections(self.ctx.h, as_f64p(base_mean), G, as_f64p(pv), ld, K, as_f64p(theta), n_theta, alpha,
+                                                    as_f64p(cutoffs), num_rej.ctypes.data_as(C.POINTER(C.c_int))))
+
+    def padj_bh(self, base_mean, G, pv, ld, K, cutoff, padj, ld_out):
+        self._io((base_mean, pv, cutoff), (padj,))
+        self.ctx.check(self.lib.pdq_padj_bh(self.ctx.h, as_f64p(base_mean), G, as_f64p(pv), ld, K, as_f64p(cutoff), as_f64p(padj), ld_out))
+
     def trend_prior(self, means, genewise, min_disp, max_disp, trigamma_c):
         n = len(means)
         out16, fitted = np.empty(16), np.empty(n)
@@ -247,7 +257,7 @@ class B200Inference(_InferenceBase):
     """
 
     _TRACED = ("lin_reg_mu", "irls", "alpha_mle", "wald_test", "wald_tests", "fit_rough_dispersions", "fit_moments_dispersions",
-               "dispersion_trend_gamma_glm", "lfc_shrink_nbinom_glm", "size_factors", "calculate_cooks")
+               "dispersion_trend_gamma_glm", "lfc_shrink_nbinom_glm", "size_factors", "calculate_cooks", "adjust_pvalues")
 
     def __init__(self, device: int = 0, n_cpus: int | None = None, lanes_per_gene: int = 0, _ops=None, trace: bool = False,
                  pinned_outputs: bool = True):
@@ -530,6 +540,46 @@ class B200Inference(_InferenceBase):
         if return_logmeans:
             return counts / sf[:, None], sf, logmeans
         return counts / sf[:, None], sf
+
+    def adjust_pvalues(self, base_mean, pvalues, alpha=0.05, independent_filter=True, lowess=None):
+        """Adjusted p-values of ``DeseqStats.summary()`` (ds.py:486-542) for one row of p-values (G,) or K rows (K, G) on the same
+        base means, each row as the reference adjusts one contrast's ``p_values``: with ``independent_filter`` the mean-count
+        filter that maximises the rejections (``_independent_filtering``), else BH over the tested genes
+        (``_p_value_adjustment``).  NaN p-values are not tested and get NaN.
+
+        The device computes the 50 base-mean cutoffs (``np.quantile``), the rejection count of every (row, cutoff) pair and the BH
+        values, all bit for bit as numpy / scipy; the host fits the lowess to each row's 50 counts and picks the cutoff
+        (:func:`workflow.filter_threshold`).  ``lowess`` replaces that smoother (default :func:`workflow.lowess`; the drop-in
+        class passes the reference's own).  Raises ``ValueError`` for a p-value outside [0, 1], as scipy does.  Returns None when
+        the backend's ops cannot run the two entry points (the callers then keep their host restatement), like
+        :meth:`trend_and_prior`."""
+        from . import workflow
+
+        if not hasattr(self._ops, "padj_bh"):
+            return None
+        bm = np.ascontiguousarray(_f64(base_mean, "base_mean", 1))
+        pv = _f64(pvalues, "pvalues")
+        single = pv.ndim == 1
+        pv = np.ascontiguousarray(pv[None, :] if single else pv)
+        G = bm.shape[0]
+        if pv.ndim != 2 or pv.shape[1] != G or pv.shape[0] == 0:
+            raise ValueError(f"pvalues must be ({G},) or (K, {G}) for {G} base means, got shape {np.shape(pvalues)}")
+        K = pv.shape[0]
+        if not G:
+            return np.empty((K, 0)) if not single else np.empty(0)
+        bad = ~np.isnan(pv) & ((pv < 0) | (pv > 1))
+        if bad.any():
+            raise ValueError("All values in `ps` must lie between 0. and 1.")  # scipy.stats.false_discovery_control's message
+        cut = np.full(K, -np.inf)
+        if independent_filter:
+            theta = workflow.filter_theta(bm)
+            cutoffs, num_rej = np.empty(len(theta)), np.empty((K, len(theta)), dtype=np.int32)
+            self._ops.padj_rejections(bm, G, pv, G, K, theta, len(theta), float(alpha), cutoffs, num_rej)
+            for k in range(K):
+                cut[k] = cutoffs[workflow.filter_threshold(theta, num_rej[k].astype(int), lowess or workflow.lowess)]
+        padj = self._ops.empty((K, G))
+        self._ops.padj_bh(bm, G, pv, G, K, cut, padj, G)
+        return padj[0] if single else padj
 
     def vst_transform(self, counts, size_factors, kind, coeffs):
         """Variance-stabilised counts (``DeseqDataSet.vst_transform``, dds.py:438-514) from RAW counts and size factors, one

@@ -1,6 +1,7 @@
 """The wiring a PyDESeq2 maintainer adds for the steps that are NOT behind the ``Inference`` plugin API but have a device
 implementation here (SURVEY.md §8 f-1, f-2): Cook's distances, median-of-ratios size factors, the variance-stabilising
-transform (``vst()`` / ``vst_transform(counts)``) and the Wald test of a contrast from the fitted coefficients.
+transform (``vst()`` / ``vst_transform(counts)``), the Wald test of a contrast from the fitted coefficients and the adjusted
+p-values (independent filtering / Benjamini-Hochberg).
 
 ``pydeseq2`` is imported lazily -- this module is only usable where the reference package is installed::
 
@@ -108,7 +109,11 @@ def b200_stats_class():
     """Returns a ``DeseqStats`` subclass whose ``run_wald_test`` (ds.py:303-360) sends the fit's coefficients, dispersions, size
     factors and the contrast to ``inference.wald_tests``: mu is built on the device instead of as an (N, G) host array per
     contrast.  The outputs and the override for genes whose replaced counts became all zero are the reference's.  A backend
-    without ``wald_tests``, or a dataset without size factors, runs the reference's own method::
+    without ``wald_tests``, or a dataset without size factors, runs the reference's own method.
+
+    ``_independent_filtering`` and ``_p_value_adjustment`` (ds.py:486-542) go through ``inference.adjust_pvalues``: the cutoffs,
+    the rejection counts and the BH values come from the device, bit for bit those of numpy and scipy, and the cutoff is chosen
+    with the reference's own ``pydeseq2.utils.lowess``.  A backend without ``adjust_pvalues`` runs the reference's methods::
 
         DeseqStats = b200_stats_class()
         for c in contrasts:                                  # one fit, any number of comparisons
@@ -141,5 +146,30 @@ def b200_stats_class():
                 self.statistics.loc[self.dds.new_all_zeroes_genes] = 0.0
                 self.p_values.loc[self.dds.new_all_zeroes_genes] = 1.0
             return None
+
+        def _independent_filtering(self):  # ds.py:486-528
+            if not self._device_padj(True):
+                return super()._independent_filtering()
+            return None
+
+        def _p_value_adjustment(self):  # ds.py:529-542
+            if not self._device_padj(False):
+                return super()._p_value_adjustment()
+            return None
+
+        def _device_padj(self, independent_filter):
+            """Sets self.padj through the backend; False when it has no adjust_pvalues or cannot run it."""
+            if not hasattr(self.inference, "adjust_pvalues"):
+                return False
+            from pydeseq2.utils import lowess
+
+            if not hasattr(self, "p_values"):
+                self.run_wald_test()
+            padj = self.inference.adjust_pvalues(np.asarray(self.base_mean, dtype=float), np.asarray(self.p_values, dtype=float),
+                                                 self.alpha, independent_filter, lowess=lowess)
+            if padj is None:
+                return False
+            self.padj = pd.Series(padj, index=self.dds.var_names)
+            return True
 
     return B200DeseqStats

@@ -77,11 +77,31 @@ def bh_adjust(p: np.ndarray) -> np.ndarray:
     return out
 
 
-def independent_filtering(base_mean: np.ndarray, pvalues: np.ndarray, alpha: float = 0.05) -> np.ndarray:
-    """Adjusted p-values with the mean-count filter chosen to maximise rejections (ds.py:486-528)."""
+def filter_theta(base_mean: np.ndarray) -> np.ndarray:
+    """The 50 quantile levels of the independent filter's base-mean cutoffs (ds.py:495-502)."""
     lower = float(np.mean(base_mean == 0))
     upper = 0.95 if lower < 0.95 else 1.0
-    theta = np.linspace(lower, upper, 50)
+    return np.linspace(lower, upper, 50)
+
+
+def filter_threshold(theta: np.ndarray, num_rej: np.ndarray, lowess=lowess) -> int:
+    """Index of the cutoff the independent filter keeps (ds.py:515-525): the first whose rejection count exceeds the lowess fit's
+    maximum less the root mean square residual of the non-zero counts; 0 when no count exceeds 10.  ``lowess`` is the smoother
+    (the project's restatement, or the reference's own ``pydeseq2.utils.lowess``)."""
+    fit = lowess(theta, num_rej, frac=1 / 5)
+    j = 0
+    if num_rej.max() > 10:
+        resid = num_rej[num_rej > 0] - fit[num_rej > 0]
+        thresh = fit.max() - np.sqrt(np.mean(resid**2))
+        above = np.where(num_rej > thresh)[0]
+        if above.size:
+            j = int(above[0])
+    return j
+
+
+def independent_filtering(base_mean: np.ndarray, pvalues: np.ndarray, alpha: float = 0.05) -> np.ndarray:
+    """Adjusted p-values with the mean-count filter chosen to maximise rejections (ds.py:486-528)."""
+    theta = filter_theta(base_mean)
     cutoffs = np.quantile(base_mean, theta)
     G = len(pvalues)
     padj = np.full((G, len(theta)), np.nan)
@@ -91,15 +111,7 @@ def independent_filtering(base_mean: np.ndarray, pvalues: np.ndarray, alpha: flo
         if use.any():
             padj[use, i] = bh_adjust(pvalues[use])
     num_rej = (padj < alpha).sum(0).astype(int)
-    fit = lowess(theta, num_rej, frac=1 / 5)
-    j = 0
-    if num_rej.max() > 10:
-        resid = num_rej[num_rej > 0] - fit[num_rej > 0]
-        thresh = fit.max() - np.sqrt(np.mean(resid**2))
-        above = np.where(num_rej > thresh)[0]
-        if above.size:
-            j = int(above[0])
-    return padj[:, j]
+    return padj[:, filter_threshold(theta, num_rej)]
 
 
 @dataclass
@@ -196,7 +208,7 @@ def deseq2_results(counts, X, inference, contrast=None, size_factors=None, refit
     if cooks_filter:
         pv[outlier] = np.nan
 
-    padj = _adjust(base_mean, pv, independent_filter, alpha, comm)
+    padj = _adjust(base_mean, pv, independent_filter, alpha, comm, inference)
 
     res = Deseq2Results(base_mean, lfc @ contrast / LN2, se / LN2, stat, pv, padj, lfc, disp, genewise, fitted, sf, nz, replaced, refitted,
                         outlier, cooks if keep_cooks else None, fit)
@@ -259,8 +271,13 @@ def _merge_refit(tables, refitted, new_zero, refit):
     tables["se"][new_zero], tables["stat"][new_zero], tables["pvalue"][new_zero] = 0.0, 0.0, 1.0
 
 
-def _adjust(base_mean, pv, independent_filter, alpha, comm=None):
-    """Multiple testing (ds.py:486-542): global over the genes of all shards."""
+def _adjust(base_mean, pv, independent_filter, alpha, comm=None, inference=None):
+    """Multiple testing (ds.py:486-542): global over the genes of all shards.  Through ``inference.adjust_pvalues`` when the
+    backend has it and the genes are not sharded, else the host restatement below."""
+    if comm is None and hasattr(inference, "adjust_pvalues"):
+        padj = inference.adjust_pvalues(base_mean, pv, alpha, independent_filter)
+        if padj is not None:
+            return padj
     bm_all, pv_all = base_mean, pv
     if comm is not None:
         g = comm.allgather_table({"bm": base_mean, "pv": pv})
@@ -347,9 +364,16 @@ def deseq2_results_resident(rf, contrast=None, refit_cooks=True, min_replicates=
         pv, stat, se = full(pv, np.nan), full(stat, np.nan), full(se, np.nan)
         replaced, refitted, outlier = full(replaced, False), full(refitted, False), full(outlier, False)
     # adjust=False stops where deseq2() + run_wald_test() + the Cook's filter stop (no independent filtering / BH: `padj` is NaN)
-    padj = _adjust(base_mean, pv, independent_filter, alpha, None) if adjust else np.full(len(pv), np.nan)
+    padj = _adjust(base_mean, pv, independent_filter, alpha, None, _context_inference(rf.ctx)) if adjust else np.full(len(pv), np.nan)
     return Deseq2Results(base_mean, lfc @ contrast / LN2, se / LN2, stat, pv, padj, lfc, disp, genewise, fitted, sf, nz, replaced, refitted,
                          outlier, None, None)
+
+
+def _context_inference(ctx):
+    """A ``B200Inference`` on an existing context (the resident drivers' own), for the backend calls that follow a resident pass."""
+    from .inference import B200Inference, _CudaOps
+
+    return B200Inference(_ops=_CudaOps(ctx=ctx))
 
 
 def _full(v, nz, G):
@@ -400,7 +424,8 @@ def deseq2_stats(res: Deseq2Results, X, inference, contrasts, lfc_null=0.0, alt_
     """``DeseqStats(dds, contrast).summary()`` for each row of ``contrasts`` (K, p) -- or one (p,) contrast -- on the fit that
     :func:`deseq2_results` or :func:`deseq2_results_resident` returned: the LFCs, dispersions, size factors, Cook's outliers and
     the outlier refit are the fit's and are not recomputed; only the Wald test depends on the contrast (ds.py:303-360), and all K
-    run in ONE ``inference.wald_tests`` call (a numpy restatement for backends without it).  ``lfc_null`` (log2, as for the
+    run in ONE ``inference.wald_tests`` call (a numpy restatement for backends without it), and their p-values are adjusted in ONE
+    ``inference.adjust_pvalues`` call when the backend has it.  ``lfc_null`` (log2, as for the
     drivers) and ``alt_hypothesis`` are scalars or one per contrast; ``prior_lfc_var`` (p,) sets the ridge diag(1 / var^2)
     (ds.py:327-330).  Genes whose replaced counts became all zero get se 0, stat 0, p 1 (ds.py:355-360).  Returns one
     :class:`Deseq2Results` per contrast, sharing every field but the results-table columns with ``res``."""
@@ -432,15 +457,15 @@ def deseq2_stats(res: Deseq2Results, X, inference, contrasts, lfc_null=0.0, alt_
                 raise KeyError(a)
         pv, stat, se = wald_tests_numpy(X, res.size_factors, res.dispersions, res.lfc, cs, ridge, LN2 * nulls, alts)
     new_zero = res.replaced & ~res.refitted
-    out = []
-    for k in range(K):
-        pk, sk, ek = np.array(pv[k]), np.array(stat[k]), np.array(se[k])
-        ek[new_zero], sk[new_zero], pk[new_zero] = 0.0, 0.0, 1.0
-        if cooks_filter:
-            pk[res.cooks_outlier] = np.nan
-        padj = _adjust(res.base_mean, pk, independent_filter, alpha)
-        out.append(dataclasses.replace(res, log2_fold_change=res.lfc @ cs[k] / LN2, lfc_se=ek / LN2, stat=sk, pvalue=pk, padj=padj))
-    return out
+    pv, stat, se = np.array(pv), np.array(stat), np.array(se)
+    se[:, new_zero], stat[:, new_zero], pv[:, new_zero] = 0.0, 0.0, 1.0
+    if cooks_filter:
+        pv[:, res.cooks_outlier] = np.nan
+    padj = inference.adjust_pvalues(res.base_mean, pv, alpha, independent_filter) if hasattr(inference, "adjust_pvalues") else None
+    if padj is None:  # all K rows in one call above; row by row on the host here
+        padj = [_adjust(res.base_mean, pv[k], independent_filter, alpha) for k in range(K)]
+    return [dataclasses.replace(res, log2_fold_change=res.lfc @ cs[k] / LN2, lfc_se=se[k] / LN2, stat=stat[k], pvalue=pv[k], padj=padj[k])
+            for k in range(K)]
 
 
 # --------------------------------------------------------------------------------------- variance-stabilising transform
