@@ -35,12 +35,13 @@ typedef enum pdq_status {
     PDQ_OK = 0,
     PDQ_ERR_CUDA = -1,        /* a CUDA runtime call failed */
     PDQ_ERR_INVALID = -2,     /* bad argument (null pointer, N<=0, p<1, ld<G, ...) */
-    PDQ_ERR_UNSUPPORTED = -3, /* p > PDQ_MAX_P */
+    PDQ_ERR_UNSUPPORTED = -3, /* p > PDQ_MAX_P (PDQ_MAX_P_WIDE with pdq_set_wide_designs) */
     PDQ_ERR_NCCL = -4,        /* NCCL missing or a collective failed */
     PDQ_ERR_NO_DEVICE = -5    /* no CUDA device / not an sm_90 part */
 } pdq_status;
 
 #define PDQ_MAX_P 16 /* design columns supported (p <= 8: register-resident p x p solvers; 9..16: the same code with the small matrices in local memory) */
+#define PDQ_MAX_P_WIDE 64 /* design columns of a context with pdq_set_wide_designs(ctx, 1): 17..64 run on the wide-design kernels */
 
 /* alt_hypothesis codes of Inference.wald_test (utils.py:778-806) */
 #define PDQ_ALT_NONE 0
@@ -71,6 +72,14 @@ int pdq_set_lanes_per_gene(pdq_ctx* ctx, int lanes);
  * (`res.success == False`, utils.py:402): two-column designs then take the reference's grid_fit_beta (grid_search.py:145-221). */
 #define PDQ_DEBUG_FAIL_IRLS_OPTIMIZER 8
 int pdq_set_debug_flags(pdq_ctx* ctx, int flags);
+/* Designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns (paired designs ~subject + condition, factors with many levels): off by
+ * default, and then such designs report PDQ_ERR_UNSUPPORTED as before.  With `on` != 0 they run on kernels in which one warp
+ * owns one gene and keeps its p x p state once, in shared memory; designs of up to PDQ_MAX_P columns run the same kernels as
+ * without it.  Above PDQ_MAX_P_WIDE, and for apeGLM shrinkage (pdq_lfc_shrink*) of any wide design: PDQ_ERR_UNSUPPORTED. */
+int pdq_set_wide_designs(pdq_ctx* ctx, int on);
+/* Host only, no device needed: (X^T X)^+ (p x p row-major) and whether X (N x p, row-major, p <= PDQ_MAX_P_WIDE) has full column
+ * rank, from the one-sided Jacobi SVD every design pack is built with (numpy.linalg.matrix_rank's tolerance). */
+int pdq_design_pinv(const double* X, int N, int p, double* pinv_out, int* full_rank_out);
 /* Measured FP64 FMA throughput of the context's device in TFLOP/s (dependent-free DFMA chains on every SM, CUDA-event timed):
  * the arithmetic roofline bench.py reports next to the HBM one -- the per-gene kernels are FP64-pipe bound (DESIGN.md §5). */
 int pdq_fp64_peak_tflops(pdq_ctx* ctx, double* tflops_out);

@@ -21,6 +21,7 @@ f64p = C.POINTER(C.c_double)
 i64p = C.POINTER(C.c_int64)
 
 PDQ_MAX_P = 16
+PDQ_MAX_P_WIDE = 64  # with pdq_set_wide_designs (B200Inference(wide_designs=True))
 ALT_CODES = {None: 0, "greaterAbs": 1, "lessAbs": 2, "greater": 3, "less": 4}
 UNIQUE_ID_BYTES = 128
 PEER_HANDLE_BYTES = 64
@@ -42,6 +43,8 @@ _SIGNATURES = {
     "pdq_device_info": (C.c_int, [c_ctx, C.c_char_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_size_t)]),
     "pdq_set_lanes_per_gene": (C.c_int, [c_ctx, C.c_int]),
     "pdq_set_debug_flags": (C.c_int, [c_ctx, C.c_int]),
+    "pdq_set_wide_designs": (C.c_int, [c_ctx, C.c_int]),
+    "pdq_design_pinv": (C.c_int, [f64p, C.c_int, C.c_int, f64p, C.POINTER(C.c_int)]),
     "pdq_launch_count": (C.c_int64, [c_ctx]),
     "pdq_buffer_epoch": (C.c_int64, [c_ctx]),
     "pdq_residency_stats": (C.c_int, [c_ctx, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
@@ -184,7 +187,13 @@ class Context:
                             "this backend needs an sm_90 (H100) GPU and has no CPU fallback")
         self.h = h
         self.device = int(device)
+        self.wide_designs = False  # pdq_set_wide_designs: designs of up to PDQ_MAX_P_WIDE columns
         self._pin_pool = {}  # nbytes -> [addresses] of released page-locked blocks (cudaHostAlloc is expensive)
+
+    def set_wide_designs(self, on: bool = True):
+        """Accept designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns on this context (off by default)."""
+        self.check(self.lib.pdq_set_wide_designs(self.h, 1 if on else 0))
+        self.wide_designs = bool(on)
 
     def check(self, rc: int):
         if rc != 0:

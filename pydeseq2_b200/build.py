@@ -11,9 +11,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libpydeseq2_b200.so")
 # translation units: (source, object tag, extra defines).  pdq_kernels.cu is compiled once for p = 1..8 and once per wide design
-# width p = 9..16 (see the note at its top); the units are independent and compile in parallel.
+# width p = 9..16 (see the note at its top); pdq_wide.cu holds the kernels of designs of 17..64 columns, one build for every width
+# (p is a run-time argument there).  The units are independent and compile in parallel.
 WIDE_P = tuple(range(9, 17))
-UNITS = [("pdq_api.cu", "pdq_api", ()), ("pdq_dispatch.cu", "pdq_dispatch", ()), ("pdq_io.cpp", "pdq_io", ()), ("pdq_padj.cu", "pdq_padj", ()), ("pdq_kernels.cu", "pdq_kernels_p1to8", ())] + \
+UNITS = [("pdq_api.cu", "pdq_api", ()), ("pdq_dispatch.cu", "pdq_dispatch", ()), ("pdq_io.cpp", "pdq_io", ()), ("pdq_padj.cu", "pdq_padj", ()), ("pdq_wide.cu", "pdq_wide", ()),
+         ("pdq_kernels.cu", "pdq_kernels_p1to8", ())] + \
         [("pdq_kernels.cu", f"pdq_kernels_p{p}", (f"-DPDQ_TU_P={p}", "-Xptxas", "-O1")) for p in WIDE_P]
 # (ptxas -O1 for the wide widths: 12 s instead of 85 s per unit; their kernels keep the small matrices in local memory anyway)
 SOURCES = sorted({u[0] for u in UNITS})

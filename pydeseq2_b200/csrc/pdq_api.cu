@@ -161,6 +161,7 @@ struct pdq_ctx {
     cudaEvent_t pfork = nullptr, pjoin[2] = {nullptr, nullptr};
     int pipeline = 4;        // gene blocks per pipelined call; PDQ_PIPELINE=0 disables
     int debug = 0;           // PDQ_DEBUG_* test hooks
+    int wide = 0;            // designs of up to PDQ_MAX_P_WIDE columns (pdq_set_wide_designs)
     int64_t launches_at_capture = 0;
     int64_t buf_epoch = 0;   // bumped whenever ensure() re-allocates a context-owned buffer (captured graphs hold those pointers)
     NcclApi nccl;
@@ -361,6 +362,18 @@ extern "C" int pdq_set_debug_flags(pdq_ctx* c, int flags) {
     return PDQ_OK;
 }
 
+extern "C" int pdq_set_wide_designs(pdq_ctx* c, int on) {
+    if (!c) return PDQ_ERR_INVALID;
+    c->wide = on != 0;
+    return PDQ_OK;
+}
+
+extern "C" int pdq_design_pinv(const double* X, int N, int p, double* pinv_out, int* full_rank_out) {
+    if (!X || !pinv_out || !full_rank_out || N <= 0 || p < 1 || p > PDQ_MAX_P_WIDE) return PDQ_ERR_INVALID;
+    design_linear_algebra(X, N, p, pinv_out, full_rank_out);
+    return PDQ_OK;
+}
+
 extern "C" int64_t pdq_launch_count(const pdq_ctx* c) { return c ? c->launches : 0; }
 extern "C" int64_t pdq_buffer_epoch(const pdq_ctx* c) { return c ? c->buf_epoch : 0; }
 
@@ -475,9 +488,17 @@ extern "C" void pdq_graph_destroy(pdq_ctx* c, pdq_graph* g) {
 }
 
 // --------------------------------------------------------------------------------------------- design pack
+// the design widths the context accepts: PDQ_MAX_P, or PDQ_MAX_P_WIDE after pdq_set_wide_designs(ctx, 1)
+static int check_width(pdq_ctx* c, int p) {
+    if (p > PDQ_MAX_P && !c->wide) return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
+    if (p > PDQ_MAX_P_WIDE)
+        return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; wide designs support p <= %d", p, PDQ_MAX_P_WIDE);
+    return PDQ_OK;
+}
+
 static int design_create(pdq_ctx* c, const double* X, const double* sf, bool offsets, int N, int p, pdq_design** out) {
     if (!c || !X || !out || N <= 0 || p < 1) return fail(c, PDQ_ERR_INVALID, "pdq_design_create: bad arguments");
-    if (p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
+    if (int e = check_width(c, p)) return e;
     CU(c, cudaSetDevice(c->device));
     pdq_design* d = new pdq_design();
     DesignDev& dd = d->d;
@@ -494,7 +515,16 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
     if (const char* e = getenv("PDQ_STAGE_MAX_BYTES")) stage_max = (size_t)atoll(e);  // tuning hook
     dd.staged = pack_bytes <= stage_max && pack_bytes + 16 <= kMaxDynSmem / 2;
     dd.smem_bytes = (dd.staged ? pack_bytes : 0) + 16;
-    design_linear_algebra(X, N, p, dd.pinv, &dd.full_rank);
+    std::vector<double> pinv((size_t)p * p);
+    design_linear_algebra(X, N, p, pinv.data(), &dd.full_rank);
+    if (p <= PDQ_MAX_P) {
+        memcpy(dd.pinv, pinv.data(), pinv.size() * 8);
+    } else if (cudaMalloc((void**)&dd.pinv_dev, pinv.size() * 8) != cudaSuccess ||
+               cudaMemcpy(dd.pinv_dev, pinv.data(), pinv.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) {
+        if (dd.pinv_dev) cudaFree(dd.pinv_dev);
+        delete d;
+        return fail(c, PDQ_ERR_CUDA, "cudaMalloc/cudaMemcpy(pseudo-inverse) failed");
+    }
     dd.few_rows = design_distinct_rows(X, N, p, 16) <= 16;
     if (const char* e = getenv("PDQ_IRLS_MEMO")) dd.few_rows = dd.few_rows && atoi(e) != 0;  // tuning hook (A/B runs)
     {
@@ -506,12 +536,14 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
         if (cudaMalloc((void**)&dd.cell_plan, plan.size() * sizeof(int)) != cudaSuccess ||
             cudaMemcpy(dd.cell_plan, plan.data(), plan.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess) {
             if (dd.cell_plan) cudaFree(dd.cell_plan);
+            if (dd.pinv_dev) cudaFree(dd.pinv_dev);
             delete d;
             return fail(c, PDQ_ERR_CUDA, "cudaMalloc/cudaMemcpy(cell plan) failed");
         }
     }
     if (cudaMalloc((void**)&dd.pack, pack.size() * 8) != cudaSuccess) {
         cudaFree(dd.cell_plan);
+        if (dd.pinv_dev) cudaFree(dd.pinv_dev);
         delete d;
         return fail(c, PDQ_ERR_CUDA, "cudaMalloc(design pack) failed");
     }
@@ -519,6 +551,7 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
     if (cudaMemcpy(dd.pack, pack.data(), pack.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) {
         cudaFree(dd.pack);
         cudaFree(dd.cell_plan);
+        if (dd.pinv_dev) cudaFree(dd.pinv_dev);
         delete d;
         return fail(c, PDQ_ERR_CUDA, "cudaMemcpy(design pack) failed");
     }
@@ -535,6 +568,7 @@ extern "C" void pdq_design_destroy(pdq_ctx* c, pdq_design* d) {
     if (c) cudaSetDevice(c->device);
     if (d->d.pack) cudaFree(d->d.pack);
     if (d->d.cell_plan) cudaFree(d->d.cell_plan);
+    if (d->d.pinv_dev) cudaFree(d->d.pinv_dev);
     delete d;
 }
 
@@ -542,6 +576,7 @@ extern "C" void pdq_design_destroy(pdq_ctx* c, pdq_design* d) {
 static int cached_design(pdq_ctx* c, const double* X, const double* sf, int N, int p, pdq_design** out, bool offsets = false) {
     // a deseq2() pass alternates between three packs -- (X, sf), (X, no sf), (ones, sf) -- so a one-entry cache would
     // rebuild (SVD, cell plan, two cudaMallocs, two synchronous copies) on almost every call: keep the last few
+    if (int e = check_width(c, p)) return e;  // a cached wide pack is refused again once the opt-in is off
     const size_t nx = (size_t)N * p;
     for (size_t i = 0; i < c->dcache.size(); ++i) {
         DesignCacheEntry& e = c->dcache[i];
@@ -575,7 +610,9 @@ static int cached_design(pdq_ctx* c, const double* X, const double* sf, int N, i
 // --------------------------------------------------------------------------------------------- device-resident ops
 static int done(pdq_ctx* c, int rc, const char* what) {
     if (rc < 0) {
-        if (rc == PDQ_ERR_UNSUPPORTED) return fail(c, rc, "%s: unsupported design (p=%d..%d, shared-memory stage <= %zu bytes)", what, 1, PDQ_MAX_P, kMaxDynSmem);
+        if (rc == PDQ_ERR_UNSUPPORTED)
+            return fail(c, rc, "%s: unsupported design (p=%d..%d, shared-memory stage <= %zu bytes)", what, 1, c->wide ? PDQ_MAX_P_WIDE : PDQ_MAX_P,
+                        kMaxDynSmem);
         return fail(c, rc, "%s: kernel launch failed: %s", what, cudaGetErrorString(cudaGetLastError()));
     }
     c->launches += rc;
@@ -663,7 +700,8 @@ extern "C" int pdq_map_irls_wald_dev(pdq_ctx* c, const pdq_design* d, const int6
     // and loses 2.5 % at 20 (DESIGN.md §5).  Above 12 the three stages run as the three launches.
     const LaunchCfg lcfg = cfg(c, G, d->d.N);
     const int gpw = 32 >> lcfg.lgT;
-    if ((int64_t)(G + gpw - 1) / gpw > (int64_t)12 * 12 * lcfg.sm_count) {
+    // wide designs (p > PDQ_MAX_P) have no fused pair: always the three launches
+    if ((int64_t)(G + gpw - 1) / gpw > (int64_t)12 * 12 * lcfg.sm_count || d->d.p > PDQ_MAX_P) {
         if (int e = alpha_mle_dev(c, d, counts, ld, G, mu, ld_mu, fitted, min_disp, max_disp, prior_disp_var, prior_var_dev, 1, 1, map,
                                   map_conv, hint_in, nullptr))
             return e;
@@ -723,6 +761,7 @@ extern "C" int pdq_lfc_shrink_dev(pdq_ctx* c, const pdq_design* d, const int64_t
     if (!d || !counts || !size || !lfcs || !inv_hessians || !conv || !status || G <= 0 || ld < G || shrink_index < 0 ||
         shrink_index >= d->d.p || !(prior_no_shrink_scale > 0.0) || !(prior_scale > 0.0))
         return fail(c, PDQ_ERR_INVALID, "pdq_lfc_shrink_dev: bad arguments");
+    if (d->d.p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
     return done(c, launch_lfc_shrink(cfg(c, G, d->d.N), d->d, counts, ld, G, size, prior_no_shrink_scale, prior_scale, shrink_index, lfcs,
                                      inv_hessians, conv, status), "lfc_shrink");
 }
@@ -1421,7 +1460,10 @@ extern "C" int pdq_wald_contrasts(pdq_ctx* c, const double* X, const double* sf,
     if (!X || !sf || !disp || !lfc || !ridge || !contrasts || !lfc_null || !alt || !pv_out || !stat_out || !se_out || N <= 0 || p <= 0 ||
         G <= 0 || K <= 0 || ld_out < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: bad arguments");
-    if (p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
+    if (p > PDQ_MAX_P && !c->wide)
+        return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
+    if (p > PDQ_MAX_P_WIDE)
+        return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; wide designs support p <= %d", p, PDQ_MAX_P_WIDE);
     std::vector<double> tab((size_t)K * (p + 2));
     if (const int k = wald_contrast_table(K, p, contrasts, lfc_null, alt, tab.data()); k >= 0)
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: unknown alternative %d (contrast %d)", alt[k], k);
@@ -1551,6 +1593,7 @@ extern "C" int pdq_lfc_shrink_nbinom_glm(pdq_ctx* c, const double* X, const int6
         return fail(c, PDQ_ERR_INVALID, "pdq_lfc_shrink_nbinom_glm: bad arguments");
     pdq_design* d;  // the kernel reads the offsets from the log-size-factor row of the design pack
     if (int e = cached_design(c, X, offset, N, p, &d, true)) return e;
+    if (p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
     void *dc, *dsize, *dbeta, *dih, *dconv, *status;
     res_begin(c);
     bool up_c;

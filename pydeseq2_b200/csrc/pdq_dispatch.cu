@@ -2,7 +2,9 @@
 //
 // pdq_kernels.cu is compiled once for p = 1..8 (p x p algebra unrolled in registers) and once per wide width p = 9..16
 // (same source, the small matrices in local memory): see the note at the top of that file and pydeseq2_b200/build.py.  Every
-// unit exports its launchers under a suffixed name; the functions declared in pdq_internal.h live here.
+// unit exports its launchers under a suffixed name; the functions declared in pdq_internal.h live here.  Designs of 17..64
+// columns (only created on contexts that opted in) go to pdq_wide.cu's launchers (`_wide`); the fused MAP -> LFC pair and apeGLM
+// shrinkage have none, so those report PDQ_ERR_UNSUPPORTED for them.
 #include "pdq_internal.h"
 
 namespace pdq {
@@ -24,30 +26,36 @@ namespace pdq {
         default: return PDQ_ERR_UNSUPPORTED;                      \
     }
 
+#define PDQ_ROUTE_WIDE(name, p, ...)                                                     \
+    if ((p) > PDQ_MAX_P) return (p) <= PDQ_MAX_P_WIDE ? name##_wide(__VA_ARGS__) : PDQ_ERR_UNSUPPORTED; \
+    PDQ_ROUTE(name, p, __VA_ARGS__)
+
+#define PDQ_UNITS_ALL(X) PDQ_UNITS(X) X(_wide)
+
 #define DECL_LIN(sfx) int launch_lin_reg_mu##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, double, double*, int64_t);
-PDQ_UNITS(DECL_LIN)
+PDQ_UNITS_ALL(DECL_LIN)
 int launch_lin_reg_mu(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
                       int64_t ld_out) {
-    PDQ_ROUTE(launch_lin_reg_mu, d.p, c, d, counts, ld, G, min_mu, mu_out, ld_out)
+    PDQ_ROUTE_WIDE(launch_lin_reg_mu, d.p, c, d, counts, ld, G, min_mu, mu_out, ld_out)
 }
 
 #define DECL_IRLS(sfx)                                                                                                           \
     int launch_irls##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, const double*, const IrlsHost&, double*, \
                          double*, double*, int64_t, double*, int*, int*, const WaldHost*);
-PDQ_UNITS(DECL_IRLS)
+PDQ_UNITS_ALL(DECL_IRLS)
 int launch_irls(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& prm,
                 double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* wald) {
-    PDQ_ROUTE(launch_irls, d.p, c, d, counts, ld, G, disp, prm, beta, mu, hat, ld_out, conv, status, n_fallback, wald)
+    PDQ_ROUTE_WIDE(launch_irls, d.p, c, d, counts, ld, G, disp, prm, beta, mu, hat, ld_out, conv, status, n_fallback, wald)
 }
 
 #define DECL_ALPHA(sfx)                                                                                                          \
     int launch_alpha_mle##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, const double*, int64_t, const double*, \
                               double, double, double, const double*, int, int, double*, double*, int*, const double*, double*);
-PDQ_UNITS(DECL_ALPHA)
+PDQ_UNITS_ALL(DECL_ALPHA)
 int launch_alpha_mle(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
                      const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
                      int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
-    PDQ_ROUTE(launch_alpha_mle, d.p, c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_var, prior_var_dev, cr_reg,
+    PDQ_ROUTE_WIDE(launch_alpha_mle, d.p, c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_var, prior_var_dev, cr_reg,
               prior_reg, alpha, conv, status, hint_in, hint_out)
 }
 
@@ -62,55 +70,55 @@ int launch_map_irls(const LaunchCfg& c, const DesignDev& d, const int64_t* count
 #define DECL_WALD(sfx)                                                                                                         \
     int launch_wald##sfx(const LaunchCfg&, const DesignDev&, const double*, const double*, const double*, int64_t, int, const double*, \
                          const double*, double, int, double*, double*, double*);
-PDQ_UNITS(DECL_WALD)
+PDQ_UNITS_ALL(DECL_WALD)
 int launch_wald(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu, int64_t ld_mu, int G,
                 const double* ridge, const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
-    PDQ_ROUTE(launch_wald, d.p, c, d, disp, lfc, mu, ld_mu, G, ridge, contrast, lfc_null, alt, pv, stat, se)
+    PDQ_ROUTE_WIDE(launch_wald, d.p, c, d, disp, lfc, mu, ld_mu, G, ridge, contrast, lfc_null, alt, pv, stat, se)
 }
 
 #define DECL_WALDK(sfx)                                                                                                \
     int launch_wald_contrasts##sfx(const LaunchCfg&, const DesignDev&, const double*, const double*, int, const double*, int, \
                                    const double*, double*, double*, double*, int64_t);
-PDQ_UNITS(DECL_WALDK)
+PDQ_UNITS_ALL(DECL_WALDK)
 int launch_wald_contrasts(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
                           const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
-    PDQ_ROUTE(launch_wald_contrasts, d.p, c, d, disp, lfc, G, ridge, K, tab, pv, stat, se, ld_out)
+    PDQ_ROUTE_WIDE(launch_wald_contrasts, d.p, c, d, disp, lfc, G, ridge, K, tab, pv, stat, se, ld_out)
 }
 
 #define DECL_ROUGH(sfx) int launch_rough##sfx(const LaunchCfg&, const DesignDev&, const double*, int64_t, int, double*);
-PDQ_UNITS(DECL_ROUGH)
+PDQ_UNITS_ALL(DECL_ROUGH)
 int launch_rough(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {
-    PDQ_ROUTE(launch_rough, d.p, c, d, normed, ld, G, alpha)
+    PDQ_ROUTE_WIDE(launch_rough, d.p, c, d, normed, ld, G, alpha)
 }
 
 #define DECL_MOMENTS(sfx) int launch_moments##sfx(const LaunchCfg&, const DesignDev&, const double*, int64_t, int, double*, double*);
-PDQ_UNITS(DECL_MOMENTS)
+PDQ_UNITS_ALL(DECL_MOMENTS)
 int launch_moments(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha, double* all_zero) {
-    PDQ_ROUTE(launch_moments, d.p, c, d, normed, ld, G, alpha, all_zero)
+    PDQ_ROUTE_WIDE(launch_moments, d.p, c, d, normed, ld, G, alpha, all_zero)
 }
 
 #define DECL_MOM(sfx)                                                                                                       \
     int launch_mom_from_counts##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, double, double, double*, \
                                     double*, double, double*, int64_t);
-PDQ_UNITS(DECL_MOM)
+PDQ_UNITS_ALL(DECL_MOM)
 int launch_mom_from_counts(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp,
                            double max_disp, double* alpha, double* normed_mean, double min_mu, double* mu_hat, int64_t ld_mu) {
-    PDQ_ROUTE(launch_mom_from_counts, d.p, c, d, counts, ld, G, min_disp, max_disp, alpha, normed_mean, min_mu, mu_hat, ld_mu)
+    PDQ_ROUTE_WIDE(launch_mom_from_counts, d.p, c, d, counts, ld, G, min_disp, max_disp, alpha, normed_mean, min_mu, mu_hat, ld_mu)
 }
 
 #define DECL_MULFC(sfx) int launch_mu_from_lfc##sfx(const LaunchCfg&, const DesignDev&, const double*, int, double*, int64_t);
-PDQ_UNITS(DECL_MULFC)
+PDQ_UNITS_ALL(DECL_MULFC)
 int launch_mu_from_lfc(const LaunchCfg& c, const DesignDev& d, const double* lfc, int G, double* mu, int64_t ld_out) {
-    PDQ_ROUTE(launch_mu_from_lfc, d.p, c, d, lfc, G, mu, ld_out)
+    PDQ_ROUTE_WIDE(launch_mu_from_lfc, d.p, c, d, lfc, G, mu, ld_out)
 }
 
 #define DECL_COOKS(sfx)                                                                                                          \
     int launch_cooks##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, const double*, const double*, int64_t, \
                           double, double*, int64_t, double*, double*, double*);
-PDQ_UNITS(DECL_COOKS)
+PDQ_UNITS_ALL(DECL_COOKS)
 int launch_cooks(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
                  int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced) {
-    PDQ_ROUTE(launch_cooks, d.p, c, d, counts, ld, G, mu, hat, ld2, cutoff, cooks, ld_out, disp, outlier, replaced)
+    PDQ_ROUTE_WIDE(launch_cooks, d.p, c, d, counts, ld, G, mu, hat, ld2, cutoff, cooks, ld_out, disp, outlier, replaced)
 }
 
 #define DECL_SHRINK(sfx)                                                                                                      \

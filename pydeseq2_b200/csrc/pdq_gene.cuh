@@ -1237,10 +1237,11 @@ constexpr int kAlphaNeedsGrid = 1;  // the reference's `res.success == False` br
 // Bounded root search on dloss, shaped after what 1-D L-BFGS-B does from the same start: project x0 into
 // the box, take a unit step against the gradient, then secant (= 1-D BFGS) steps; once the root is
 // bracketed the secant point is safeguarded by the bracket (bisection when it leaves it or stalls).
-template <int P>
-PDQ_HD void alpha_gene(const Group& grp, const DesignS& d, const AlphaParams& prm, const int64_t* y, int64_t ld,
-                       const double* mu, int64_t ld_mu, double alpha_hat, double* alpha_out, double* conv_out,
-                       int* status_out, bool valid, double* psi_tab, const double* hint_in = nullptr, double* hint_out = nullptr) {
+// `dloss(x, xhat, curv)` evaluates d loss / d log(alpha) at x (alpha_dloss; curv != nullptr on the first evaluation): the search
+// is the same for every layout of the per-gene sums (the wide-design kernels pass their own, pdq_wide.cu)
+template <class DLoss>
+PDQ_HD void alpha_search(const Group& grp, const AlphaParams& prm, double alpha_hat, DLoss&& dloss, double* alpha_out, double* conv_out,
+                         int* status_out, bool valid, const double* hint_in = nullptr, double* hint_out = nullptr) {
     // hint_in = [x*, h*] of an EARLIER search on the same counts and means without the prior (the genewise fit, whose optimum x*
     // = log alpha and curvature h* of its loss there carry over): the MAP objective is that loss plus (x - xhat)^2 / (2 var), so
     // one Newton step of it from x* lands within ~1e-3 of the MAP optimum, and a second one, with the curvature h* + 1/var,
@@ -1255,7 +1256,7 @@ PDQ_HD void alpha_gene(const Group& grp, const DesignS& d, const AlphaParams& pr
     const double pgtol = 1e-5;
     double xb = fmin(fmax(xhat, prm.lo), prm.hi);
     double h0;
-    double gb = alpha_dloss<P>(grp, d, prm, y, ld, mu, ld_mu, xb, xhat, psi_tab, &h0);
+    double gb = dloss(xb, xhat, &h0);
     double xa = xb, ga = gb;
     double bl = prm.lo, br = prm.hi;  // bracket ends (valid when have_br)
     bool have_br = false, active = true, fail = false;
@@ -1298,7 +1299,7 @@ PDQ_HD void alpha_gene(const Group& grp, const DesignS& d, const AlphaParams& pr
     }
     for (int ev = 0; ev < 60; ++ev) {
         if (!grp.any(active)) break;
-        const double gt = alpha_dloss<P>(grp, d, prm, y, ld, mu, ld_mu, xt, xhat, psi_tab);
+        const double gt = dloss(xt, xhat, (double*)nullptr);
         if (!active) continue;
         if (!(gt == gt)) {
             fail = true;
@@ -1381,17 +1382,27 @@ PDQ_HD void alpha_gene(const Group& grp, const DesignS& d, const AlphaParams& pr
     }
 }
 
+template <int P>
+PDQ_HD void alpha_gene(const Group& grp, const DesignS& d, const AlphaParams& prm, const int64_t* y, int64_t ld,
+                       const double* mu, int64_t ld_mu, double alpha_hat, double* alpha_out, double* conv_out,
+                       int* status_out, bool valid, double* psi_tab, const double* hint_in = nullptr, double* hint_out = nullptr) {
+    alpha_search(
+        grp, prm, alpha_hat,
+        [&](double x, double xhat, double* curv) { return alpha_dloss<P>(grp, d, prm, y, ld, mu, ld_mu, x, xhat, psi_tab, curv); },
+        alpha_out, conv_out, status_out, valid, hint_in, hint_out);
+}
+
 // grid fallback (grid_search.py:54-142): 100-point grid on [lo, hi], then 100 points on +-1 cell around the
 // best; always cr_reg=True, prior_reg=False because the reference's call drops those flags (utils.py:558-562).
-template <int P>
-PDQ_HD void alpha_grid_gene(const Group& grp, const DesignS& d, double lo, double hi, const int64_t* y, int64_t ld,
-                            const double* mu, int64_t ld_mu, double* alpha_out, bool valid) {
+// `loss(x)` = alpha_loss with cr_reg on and no prior
+template <class Loss>
+PDQ_HD void alpha_grid_search(const Group& grp, double lo, double hi, Loss&& loss, double* alpha_out, bool valid) {
     const int K = 100;
     const double delta = (hi - lo) / (double)(K - 1);
     double best = 0.0, bestx = lo;
     for (int k = 0; k < K; ++k) {
         const double x = (k == K - 1) ? hi : fma((double)k, delta, lo);
-        const double f = alpha_loss<P>(grp, d, 1, 0, 1.0, y, ld, mu, ld_mu, x, 0.0);
+        const double f = loss(x);
         if (k == 0 || f < best) { best = f; bestx = x; }  // np.argmin: first minimum, NaN-free case
     }
     const double flo = bestx - delta, fhi = bestx + delta;
@@ -1399,10 +1410,17 @@ PDQ_HD void alpha_grid_gene(const Group& grp, const DesignS& d, double lo, doubl
     double bestf = flo;
     for (int k = 0; k < K; ++k) {
         const double x = (k == K - 1) ? fhi : fma((double)k, fd, flo);
-        const double f = alpha_loss<P>(grp, d, 1, 0, 1.0, y, ld, mu, ld_mu, x, 0.0);
+        const double f = loss(x);
         if (k == 0 || f < best) { best = f; bestf = x; }
     }
     if (valid && grp.si == 0) *alpha_out = exp(bestf);
+}
+
+template <int P>
+PDQ_HD void alpha_grid_gene(const Group& grp, const DesignS& d, double lo, double hi, const int64_t* y, int64_t ld,
+                            const double* mu, int64_t ld_mu, double* alpha_out, bool valid) {
+    alpha_grid_search(
+        grp, lo, hi, [&](double x) { return alpha_loss<P>(grp, d, 1, 0, 1.0, y, ld, mu, ld_mu, x, 0.0); }, alpha_out, valid);
 }
 
 // final dispersion of one gene (dds.py:918-932): the clipped MAP estimate, but a gene whose genewise estimate lies more than
@@ -1623,11 +1641,11 @@ PDQ_HD double trimmed_mean_cell(const Group& grp, double* v, int s, int e, int n
     return grp.sum(part) / (double)(nc - 2 * ntrim);
 }
 
-template <int P>
-PDQ_HD void cooks_gene(const Group& grp, const DesignS& d, const CellPlan& plan, const int64_t* y, int64_t ld, const double* mu,
-                       const double* hat, int64_t ld2, double cutoff, double* vals /* smem: n_in_cells */,
-                       double* sq /* smem: n_in_cells */, double* cooks_out, int64_t ld_out, double* disp_out,
-                       double* outlier_out, double* replaced_out, bool valid) {
+// `p` design columns (cooks_gene<P> for the narrow kernels, the wide-design kernels pass theirs)
+PDQ_HD void cooks_gene_cols(const Group& grp, const DesignS& d, int p, const CellPlan& plan, const int64_t* y, int64_t ld,
+                            const double* mu, const double* hat, int64_t ld2, double cutoff, double* vals /* smem: n_in_cells */,
+                            double* sq /* smem: n_in_cells */, double* cooks_out, int64_t ld_out, double* disp_out,
+                            double* outlier_out, double* replaced_out, bool valid) {
     const int nf = plan.cell_start[plan.n_cells];
     // normalised counts: mean over ALL samples, and the grouped copy of the samples that sit in cells
     double msum = 0.0;
@@ -1664,7 +1682,7 @@ PDQ_HD void cooks_gene(const Group& grp, const DesignS& d, const CellPlan& plan,
         const double yv = (double)y[n * ld], m = mu[n * ld2], h = hat[n * ld2];
         const double V = fma(m * m, alpha, m);
         const double omh = 1.0 - h;
-        const double ck = (yv - m) * (yv - m) / V / (double)P * (h / (omh * omh));
+        const double ck = (yv - m) * (yv - m) / V / (double)p * (h / (omh * omh));
         if (valid && cooks_out) cooks_out[n * ld_out] = ck;
         any_all = any_all || (ck > cutoff);
         if (ck > best) {  // lanes visit their samples in increasing n: strict > keeps the first maximum
@@ -1679,7 +1697,7 @@ PDQ_HD void cooks_gene(const Group& grp, const DesignS& d, const CellPlan& plan,
             const double yv = (double)y[n * ld], m = mu[n * ld2], h = hat[n * ld2];
             const double V = fma(m * m, alpha, m);
             const double omh = 1.0 - h;
-            const double ck = (yv - m) * (yv - m) / V / (double)P * (h / (omh * omh));
+            const double ck = (yv - m) * (yv - m) / V / (double)p * (h / (omh * omh));
             best_use = ck > best_use ? ck : best_use;
         }
     }
@@ -1711,6 +1729,13 @@ PDQ_HD void cooks_gene(const Group& grp, const DesignS& d, const CellPlan& plan,
         *outlier_out = outlier ? 1.0 : 0.0;
         *replaced_out = replaced ? 1.0 : 0.0;
     }
+}
+
+template <int P>
+PDQ_HD void cooks_gene(const Group& grp, const DesignS& d, const CellPlan& plan, const int64_t* y, int64_t ld, const double* mu,
+                       const double* hat, int64_t ld2, double cutoff, double* vals, double* sq, double* cooks_out, int64_t ld_out,
+                       double* disp_out, double* outlier_out, double* replaced_out, bool valid) {
+    cooks_gene_cols(grp, d, P, plan, y, ld, mu, hat, ld2, cutoff, vals, sq, cooks_out, ld_out, disp_out, outlier_out, replaced_out, valid);
 }
 
 }  // namespace pdq

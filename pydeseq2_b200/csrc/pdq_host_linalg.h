@@ -10,6 +10,9 @@
 #ifndef PDQ_MAX_P
 #define PDQ_MAX_P 16
 #endif
+#ifndef PDQ_MAX_P_WIDE
+#define PDQ_MAX_P_WIDE 64
+#endif
 
 namespace pdq {
 
@@ -48,7 +51,7 @@ inline int wald_contrast_table(int K, int p, const double* contrasts, const doub
     return -1;
 }
 
-// One-sided Jacobi SVD of X (N x p, p <= 8): the right singular vectors V and singular values give
+// One-sided Jacobi SVD of X (N x p, p <= PDQ_MAX_P_WIDE): the right singular vectors V and singular values give
 //   rank(X)   with numpy.linalg.matrix_rank's tolerance  s_max * max(N, p) * eps     (utils.py:349)
 //   (X^T X)^+ = V diag(1/s_i^2 for s_i > tol) V^T        (least-squares / minimum-norm projector)
 // number of distinct rows of X (capped at `cap + 1`): categorical designs have a handful, continuous covariates ~N
@@ -69,8 +72,9 @@ inline int design_distinct_rows(const double* X, int N, int p, int cap) {
 inline void design_linear_algebra(const double* X, int N, int p, double* pinv, int* full_rank) {
     std::vector<double> U((size_t)N * p);
     for (size_t i = 0; i < (size_t)N * p; ++i) U[i] = X[i];
-    double V[PDQ_MAX_P][PDQ_MAX_P] = {};
-    for (int i = 0; i < p; ++i) V[i][i] = 1.0;
+    std::vector<double> Vs((size_t)p * p, 0.0);
+    auto V = [&](int k, int a) -> double& { return Vs[(size_t)k * p + a]; };
+    for (int i = 0; i < p; ++i) V(i, i) = 1.0;
     for (int sweep = 0; sweep < 60; ++sweep) {
         double off = 0.0;
         for (int a = 0; a < p - 1; ++a)
@@ -93,14 +97,15 @@ inline void design_linear_algebra(const double* X, int N, int p, double* pinv, i
                     U[(size_t)n * p + b] = sn * ua + cs * ub;
                 }
                 for (int k = 0; k < p; ++k) {
-                    const double va = V[k][a], vb = V[k][b];
-                    V[k][a] = cs * va - sn * vb;
-                    V[k][b] = sn * va + cs * vb;
+                    const double va = V(k, a), vb = V(k, b);
+                    V(k, a) = cs * va - sn * vb;
+                    V(k, b) = sn * va + cs * vb;
                 }
             }
         if (off < 1e-15) break;
     }
-    double s[PDQ_MAX_P], smax = 0.0;
+    std::vector<double> s(p);
+    double smax = 0.0;
     for (int j = 0; j < p; ++j) {
         double q = 0;
         for (int n = 0; n < N; ++n) q += U[(size_t)n * p + j] * U[(size_t)n * p + j];
@@ -115,7 +120,7 @@ inline void design_linear_algebra(const double* X, int N, int p, double* pinv, i
         for (int k = 0; k < p; ++k) {
             double acc = 0;
             for (int j = 0; j < p; ++j)
-                if (s[j] > tol) acc += V[i][j] * V[k][j] / (s[j] * s[j]);
+                if (s[j] > tol) acc += V(i, j) * V(k, j) / (s[j] * s[j]);
             pinv[i * p + k] = acc;
         }
 }

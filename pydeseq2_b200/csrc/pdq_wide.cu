@@ -1,0 +1,1134 @@
+// pdq_wide.cu -- per-gene kernels for designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns (opt-in per context:
+// pdq_set_wide_designs).
+//
+// The kernels of pdq_kernels.cu keep one gene's p x p state per LANE: in registers for p <= 8, in local memory for 9..16.  At
+// p = 64 one packed symmetric matrix is 16.6 KB, so that layout does not scale.  Here one WARP owns one gene (one warp per block,
+// one gene per block), and the gene's matrices live once, in the block's dynamic shared memory (DESIGN.md §3):
+//   * per-sample work is split over the lanes: chunks of 32 samples, lane l takes sample n0 + l and stages its weight (and working
+//     response) in shared memory;
+//   * the rank-32 update of a packed matrix from one chunk is split over its entries (lane l owns entries l, l + 32, ...); vectors
+//     such as X^T W z are split over their components;
+//   * the Cholesky factorisation, the triangular solves and the inverse are cooperative, one warp barrier per column step.
+// The design pack is read from global memory (it stays in L1 / L2).  The per-gene semantics are those of pdq_gene.cuh -- start
+// values, ridge, stopping rules, optimiser branch, dispersion search and grid, Wald alternatives, Cook's distances -- written
+// against libdevice's exp / log and the series of pdq_math.cuh instead of the table-driven cores; parity is to the reference's
+// tolerances, not bit for bit with the narrow kernels (which never run the same designs).
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "pdq_gene.cuh"
+#include "pdq_internal.h"
+
+namespace pdq {
+namespace {
+
+constexpr int kMaxTri = PDQ_MAX_P_WIDE * (PDQ_MAX_P_WIDE + 1) / 2;
+constexpr int kVecs = 8;  // vectors of p doubles in the workspace
+
+__host__ __device__ constexpr int tri_count(int p) { return (p * (p + 1) / 2 + 1) & ~1; }
+// workspace of one gene: three packed p x p matrices, kVecs vectors of p, two chunk buffers of 32
+__host__ __device__ constexpr size_t wide_ws_doubles(int p) { return 3 * (size_t)tri_count(p) + (size_t)kVecs * p + 64; }
+
+struct Ws {
+    double *A, *L, *Li;  // packed lower triangles
+    double* v[kVecs];
+    double *cw, *cz;     // per-chunk staging, one slot per lane
+    int p, np;
+};
+
+__device__ __forceinline__ Ws carve(double* s, int p) {
+    Ws w;
+    w.p = p;
+    w.np = p * (p + 1) / 2;
+    const int t = tri_count(p);
+    w.A = s;
+    w.L = s + t;
+    w.Li = s + 2 * t;
+    for (int k = 0; k < kVecs; ++k) w.v[k] = s + 3 * t + k * p;
+    w.cw = s + 3 * t + kVecs * p;
+    w.cz = w.cw + 32;
+    return w;
+}
+
+__device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
+__device__ __forceinline__ double wsum(double v) {
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+__device__ __forceinline__ bool wany(bool b) { return __any_sync(0xffffffffu, b) != 0; }
+
+__device__ __forceinline__ DesignS design_of(const double* pack, int N, int p) {
+    DesignS d;
+    d.X = pack;
+    d.sf = pack + p;
+    d.lsf = pack + p + 1;
+    d.N = N;
+    d.RS = design_row_stride(p);
+    return d;
+}
+__device__ __forceinline__ const double* row_of(const DesignS& d, int n) { return d.X + (size_t)n * d.RS; }
+
+__device__ __forceinline__ void wfill(double* a, int n, double v) {
+    for (int k = lane_id(); k < n; k += 32) a[k] = v;
+}
+__device__ __forceinline__ void wcopy(double* dst, const double* src, int n) {
+    for (int k = lane_id(); k < n; k += 32) dst[k] = src[k];
+}
+
+// S += sum_{s < cnt} w[s] x_{n0+s} x_{n0+s}^T over the packed lower triangle, entries k = lane, lane + 32, ...
+__device__ void rank_chunk(const DesignS& d, int p, int n0, int cnt, const double* w, double* S) {
+    const int np = p * (p + 1) / 2;
+    int i = 0, j = lane_id();
+    while (j > i) {
+        j -= i + 1;
+        ++i;
+    }
+    for (int k = lane_id(); k < np; k += 32) {
+        double acc = S[k];
+        for (int s = 0; s < cnt; ++s) {
+            const double* x = row_of(d, n0 + s);
+            acc = fma(w[s] * x[i], x[j], acc);
+        }
+        S[k] = acc;
+        j += 32;
+        while (j > i) {
+            j -= i + 1;
+            ++i;
+        }
+    }
+}
+
+// v += sum_{s < cnt} z[s] x_{n0+s}, components split over the lanes
+__device__ void vec_chunk(const DesignS& d, int p, int n0, int cnt, const double* z, double* v) {
+    for (int j = lane_id(); j < p; j += 32) {
+        double acc = v[j];
+        for (int s = 0; s < cnt; ++s) acc = fma(z[s], row_of(d, n0 + s)[j], acc);
+        v[j] = acc;
+    }
+}
+
+__device__ __forceinline__ double xdot(const double* x, const double* b, int p) {
+    double e = 0.0;
+    for (int j = 0; j < p; ++j) e = fma(x[j], b[j], e);
+    return e;
+}
+
+// in-place L L^T = L (packed); a non-positive pivot gives NaN through sqrt, as chol<P>
+__device__ void chol_w(double* L, int p) {
+    const int lane = lane_id();
+    for (int j = 0; j < p; ++j) {
+        __syncwarp();
+        const double dj = sqrt(L[tri(j, j)]);
+        const double inv = 1.0 / dj;
+        __syncwarp();
+        for (int i = j + 1 + lane; i < p; i += 32) L[tri(i, j)] *= inv;
+        if (lane == 0) L[tri(j, j)] = dj;
+        __syncwarp();
+        for (int i = j + 1 + lane; i < p; i += 32) {
+            const double lij = L[tri(i, j)];
+            for (int k = j + 1; k <= i; ++k) L[tri(i, k)] = fma(-lij, L[tri(k, j)], L[tri(i, k)]);
+        }
+    }
+    __syncwarp();
+}
+
+// solve (L L^T) x = v in place
+__device__ void chol_solve_w(const double* L, double* v, int p) {
+    const int lane = lane_id();
+    for (int i = 0; i < p; ++i) {
+        __syncwarp();
+        const double xi = v[i] / L[tri(i, i)];
+        __syncwarp();
+        if (lane == 0) v[i] = xi;
+        for (int r = i + 1 + lane; r < p; r += 32) v[r] = fma(-L[tri(r, i)], xi, v[r]);
+    }
+    for (int i = p - 1; i >= 0; --i) {
+        __syncwarp();
+        const double xi = v[i] / L[tri(i, i)];
+        __syncwarp();
+        if (lane == 0) v[i] = xi;
+        for (int r = lane; r < i; r += 32) v[r] = fma(-L[tri(i, r)], xi, v[r]);
+    }
+    __syncwarp();
+}
+
+// H = (L L^T)^-1; Li = L^-1 (scratch).  H may be L itself: the second phase reads Li only
+__device__ void chol_inverse_w(const double* L, double* Li, double* H, int p) {
+    __syncwarp();
+    for (int j = lane_id(); j < p; j += 32) {
+        Li[tri(j, j)] = 1.0 / L[tri(j, j)];
+        for (int i = j + 1; i < p; ++i) {
+            double s = 0.0;
+            for (int k = j; k < i; ++k) s = fma(-L[tri(i, k)], Li[tri(k, j)], s);
+            Li[tri(i, j)] = s / L[tri(i, i)];
+        }
+    }
+    __syncwarp();
+    for (int i = lane_id(); i < p; i += 32)
+        for (int j = 0; j <= i; ++j) {
+            double s = 0.0;
+            for (int k = i; k < p; ++k) s = fma(Li[tri(k, i)], Li[tri(k, j)], s);
+            H[tri(i, j)] = s;
+        }
+    __syncwarp();
+}
+
+// x^T S x (one lane, x a design row)
+__device__ __forceinline__ double quad_w(const double* S, const double* x, int p) {
+    double q = 0.0;
+    for (int i = 0; i < p; ++i) {
+        double r = 0.0;
+        for (int j = 0; j < i; ++j) r = fma(S[tri(i, j)], x[j], r);
+        q = fma(x[i], fma(2.0, r, S[tri(i, i)] * x[i]), q);
+    }
+    return q;
+}
+
+// y = S x, rows split over the lanes
+__device__ void matvec_w(const double* S, const double* x, double* y, int p) {
+    __syncwarp();
+    for (int i = lane_id(); i < p; i += 32) {
+        double r = 0.0;
+        for (int j = 0; j < p; ++j) r = fma(S[j <= i ? tri(i, j) : tri(j, i)], x[j], r);
+        y[i] = r;
+    }
+    __syncwarp();
+}
+
+// sum_ij S_ij T_ij
+__device__ double symdot_w(const double* S, const double* T, int p) {
+    double dg = 0.0, o = 0.0;
+    int i = 0, j = lane_id();
+    while (j > i) {
+        j -= i + 1;
+        ++i;
+    }
+    for (int k = lane_id(); k < p * (p + 1) / 2; k += 32) {
+        if (i == j) dg = fma(S[k], T[k], dg);
+        else o = fma(S[k], T[k], o);
+        j += 32;
+        while (j > i) {
+            j -= i + 1;
+            ++i;
+        }
+    }
+    return fma(2.0, wsum(o), wsum(dg));
+}
+
+// L = S + diag(ridge) / + the packed lower triangle `ridge_tri`, then factor
+__device__ void factor_ridged(const double* S, double* L, int p, double ridge, const double* ridge_tri) {
+    __syncwarp();
+    for (int k = lane_id(); k < p * (p + 1) / 2; k += 32) L[k] = S[k] + (ridge_tri ? ridge_tri[k] : 0.0);
+    __syncwarp();
+    if (!ridge_tri)
+        for (int i = lane_id(); i < p; i += 32) L[tri(i, i)] += ridge;
+    chol_w(L, p);
+}
+
+// beta = (X^T X)^+ v (rows of pinv split over the lanes)
+__device__ void apply_pinv(const double* pinv, const double* v, double* beta, int p) {
+    __syncwarp();
+    for (int i = lane_id(); i < p; i += 32) {
+        double s = 0.0;
+        for (int j = 0; j < p; ++j) s = fma(pinv[(size_t)i * p + j], v[j], s);
+        beta[i] = s;
+    }
+    __syncwarp();
+}
+
+// ---------------------------------------------------------------------------------------------
+// Wald test from M = X^T W X (wald_inverse + wald_contrast of pdq_gene.cuh)
+// ---------------------------------------------------------------------------------------------
+struct WideWald {
+    double ridge[kMaxTri];             // lower triangle of the caller's p x p ridge matrix, packed (the only part wald_inverse reads)
+    double contrast[PDQ_MAX_P_WIDE];
+    double lfc_null;
+    int alt;
+};
+
+// statistic and p-value of alternative `alt` given SE (every lane, replicated; the same expressions as wald_contrast)
+__device__ void wald_alt(const double* c, const double* b, int p, double se, double t0, int alt, double& pv, double& stat) {
+    auto greater = [&](double t, double& s, double& q) {
+        s = 0.0;
+        for (int j = 0; j < p; ++j) s = fma(c[j], fmax((b[j] - t) / se, 0.0), s);
+        q = norm_sf(s);
+    };
+    auto less = [&](double t, double& s, double& q) {
+        s = 0.0;
+        for (int j = 0; j < p; ++j) s = fma(c[j], fmin((b[j] - t) / se, 0.0), s);
+        q = norm_sf(fabs(s));
+    };
+    if (alt == 0) {
+        double s = 0.0;
+        for (int j = 0; j < p; ++j) s = fma(c[j], b[j] - t0, s);
+        stat = s / se;
+        pv = 2.0 * norm_sf(fabs(stat));
+    } else if (alt == 1) {
+        double s = 0.0;
+        for (int j = 0; j < p; ++j) s = fma(c[j], sgn(b[j]) * fmax((fabs(b[j]) - t0) / se, 0.0), s);
+        stat = s;
+        pv = 2.0 * norm_sf(fabs(s));
+    } else if (alt == 2) {
+        double sa, pa, sb, pb;
+        greater(-fabs(t0), sa, pa);
+        less(fabs(t0), sb, pb);
+        stat = (fabs(sb) < fabs(sa)) ? sb : sa;
+        pv = (pb > pa) ? pb : pa;
+    } else if (alt == 3) {
+        greater(t0, stat, pv);
+    } else {
+        less(t0, stat, pv);
+    }
+}
+
+// H = (M + ridge)^-1 into ws.L (ws.Li scratch); M in `M`
+__device__ void wald_inverse_w(const double* M, const double* ridge_tri, Ws& ws) {
+    factor_ridged(M, ws.L, ws.p, 0.0, ridge_tri);
+    chol_inverse_w(ws.L, ws.Li, ws.L, ws.p);
+}
+
+// SE of contrast c (shared memory or parameter space) against M and H = ws.L; ws.v[6], ws.v[7] scratch
+__device__ double wald_se_w(const double* M, const double* c, Ws& ws) {
+    matvec_w(ws.L, c, ws.v[6], ws.p);
+    matvec_w(M, ws.v[6], ws.v[7], ws.p);
+    double q = 0.0;
+    for (int j = lane_id(); j < ws.p; j += 32) q = fma(ws.v[6][j], ws.v[7][j], q);
+    return sqrt(wsum(q));
+}
+
+__device__ void wald_finish_w(const double* M, const WideWald& w, const double* beta, Ws& ws, double* p_out, double* stat_out,
+                              double* se_out) {
+    wald_inverse_w(M, w.ridge, ws);
+    const double se = wald_se_w(M, w.contrast, ws);
+    double pv, stat;
+    wald_alt(w.contrast, beta, ws.p, se, w.lfc_null, w.alt, pv, stat);
+    if (lane_id() == 0) {
+        *p_out = pv;
+        *stat_out = stat;
+        *se_out = se;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// kernels: one warp per block, one gene per block
+// ---------------------------------------------------------------------------------------------
+struct WideBase {
+    const double* pack;  // design pack (global)
+    const double* pinv;  // (X^T X)^+ p x p row-major (global)
+    int N, p, G;
+};
+
+struct LinArgs {
+    WideBase b;
+    const int64_t* counts;
+    int64_t ld;
+    double min_mu;
+    double* mu;
+    int64_t ld_out;
+};
+
+// v = X^T t with t = y / sf per sample (the projection lin_reg_mu / fit_rough_dispersions start from); returns sum t
+template <class Y>
+__device__ double project(const DesignS& d, int p, const Y& yy, Ws& ws, double* v) {
+    wfill(v, p, 0.0);
+    double s = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        const double t = n < d.N ? yy.at(d, n) : 0.0;
+        s += t;
+        __syncwarp();
+        ws.cz[lane_id()] = t;
+        __syncwarp();
+        vec_chunk(d, p, n0, min(32, d.N - n0), ws.cz, v);
+    }
+    __syncwarp();
+    return wsum(s);
+}
+
+__global__ void __launch_bounds__(32) k_wide_lin_reg_mu(const __grid_constant__ LinArgs a) {
+    extern __shared__ __align__(16) double wsm[];
+    Ws ws = carve(wsm, a.b.p);
+    const int g = blockIdx.x, p = a.b.p;
+    const DesignS d = design_of(a.b.pack, a.b.N, p);
+    project(d, p, NormedFromCounts{a.counts + g, a.ld}, ws, ws.v[0]);
+    apply_pinv(a.b.pinv, ws.v[0], ws.v[1], p);
+    for (int n = lane_id(); n < d.N; n += 32) {
+        const double m = d.sf[n * d.RS] * xdot(row_of(d, n), ws.v[1], p);
+        a.mu[(int64_t)n * a.ld_out + g] = (m < a.min_mu) ? a.min_mu : m;  // np.maximum (NaN propagates)
+    }
+}
+
+struct MomArgsW {
+    WideBase b;
+    const double* normed;   // rough / moments: (N, G) normalised counts
+    const int64_t* counts;  // mom_from_counts: raw counts
+    int64_t ld;
+    double s_mean_inv, min_disp, max_disp, min_mu;
+    double *alpha, *aux;    // aux: all-zero flags (moments) or normalised means (mom_from_counts)
+    double* mu;             // mom_from_counts: initial mu_hat, or nullptr
+    int64_t ld_mu;
+};
+
+// fit_rough_dispersions (rough_disp_gene); `fit` receives nothing, beta stays in ws.v[1]
+template <class Y>
+__device__ double rough_w(const DesignS& d, const double* pinv, int p, const Y& yy, Ws& ws, double* mean, double* mu_out,
+                          int64_t ld_mu, double min_mu) {
+    const double s = project(d, p, yy, ws, ws.v[0]);
+    apply_pinv(pinv, ws.v[0], ws.v[1], p);
+    const double m = s / (double)d.N;
+    double acc = 0.0, ss = 0.0;
+    for (int n = lane_id(); n < d.N; n += 32) {
+        const double fit = xdot(row_of(d, n), ws.v[1], p);
+        const double t = yy.at(d, n);
+        const double yh = (fit < 1.0) ? 1.0 : fit;  // np.maximum(y_hat, 1)
+        const double e = t - yh;
+        acc += (e * e - yh) / (yh * yh);
+        const double dm = t - m;
+        ss = fma(dm, dm, ss);
+        if (mu_out) {
+            const double mu = d.sf[n * d.RS] * fit;
+            mu_out[(int64_t)n * ld_mu] = (mu < min_mu) ? min_mu : mu;
+        }
+    }
+    acc = wsum(acc) / (double)(d.N - p);
+    if (mean) *mean = wsum(ss);  // sum of squared deviations from the mean (mom_from_counts)
+    return (acc < 0.0) ? 0.0 : acc;  // np.maximum(alpha_rde, 0)
+}
+
+__global__ void __launch_bounds__(32) k_wide_rough(const __grid_constant__ MomArgsW a) {
+    extern __shared__ __align__(16) double wsm[];
+    Ws ws = carve(wsm, a.b.p);
+    const int g = blockIdx.x;
+    const DesignS d = design_of(a.b.pack, a.b.N, a.b.p);
+    const double r = rough_w(d, a.b.pinv, a.b.p, NormedF64{a.normed + g, a.ld}, ws, nullptr, nullptr, 0, 0.0);
+    if (lane_id() == 0) a.alpha[g] = r;
+}
+
+__global__ void __launch_bounds__(32) k_wide_moments(const __grid_constant__ MomArgsW a) {
+    const int g = blockIdx.x;
+    const DesignS d = design_of(a.b.pack, a.b.N, a.b.p);
+    const Group grp{lane_id(), 32, 1};
+    double mean;
+    bool all_zero;
+    const double m = moments_disp_gene(grp, d, NormedF64{a.normed + g, a.ld}, a.s_mean_inv, mean, all_zero);
+    if (lane_id() == 0) {
+        a.alpha[g] = m;
+        if (a.aux) a.aux[g] = all_zero ? 1.0 : 0.0;
+    }
+}
+
+// rough + moments, their min / clip, the normalised mean and (lin_reg_mu branch) mu_hat: mom_fused_gene
+__global__ void __launch_bounds__(32) k_wide_mom_from_counts(const __grid_constant__ MomArgsW a) {
+    extern __shared__ __align__(16) double wsm[];
+    Ws ws = carve(wsm, a.b.p);
+    const int g = blockIdx.x;
+    const DesignS d = design_of(a.b.pack, a.b.N, a.b.p);
+    double ss;
+    const NormedFromCounts yy{a.counts + g, a.ld};
+    // the mean is needed inside the sweep: one projection pass for it first (rough_w recomputes the same sums)
+    const double m = project(d, a.b.p, yy, ws, ws.v[0]) / (double)d.N;
+    const double rough = rough_w(d, a.b.pinv, a.b.p, yy, ws, &ss, a.mu ? a.mu + g : nullptr, a.ld_mu, a.min_mu);
+    const double var = ss / (double)(d.N - 1);
+    double mde = (var - a.s_mean_inv * m) / (m * m);
+    if (!(mde == mde)) mde = 0.0;  // np.nan_to_num
+    else if (mde > 1.7976931348623157e308) mde = 1.7976931348623157e308;
+    else if (mde < -1.7976931348623157e308) mde = -1.7976931348623157e308;
+    if (lane_id() == 0) {
+        double al = (mde < rough) ? mde : rough;                                    // np.minimum (dds.py:1158)
+        al = (al < a.min_disp) ? a.min_disp : ((al > a.max_disp) ? a.max_disp : al);  // np.clip (dds.py:1161)
+        a.alpha[g] = al;
+        a.aux[g] = m;
+    }
+}
+
+struct MuLfcArgsW {
+    WideBase b;
+    const double* lfc;
+    double* mu;
+    int64_t ld_out;
+};
+
+__global__ void __launch_bounds__(32) k_wide_mu_from_lfc(const __grid_constant__ MuLfcArgsW a) {
+    const int g = blockIdx.x, p = a.b.p;
+    const DesignS d = design_of(a.b.pack, a.b.N, p);
+    const double* b = a.lfc + (int64_t)g * p;
+    for (int n = lane_id(); n < d.N; n += 32) a.mu[(int64_t)n * a.ld_out + g] = exp(xdot(row_of(d, n), b, p)) * d.sf[n * d.RS];
+}
+
+// ---------------------------------------------------------------------------------------------
+// irls (irls_gene + irls_optimizer_gene)
+// ---------------------------------------------------------------------------------------------
+struct IrlsArgsW {
+    WideBase b;
+    IrlsParams prm;
+    const int64_t* counts;
+    int64_t ld;
+    const double* disp;
+    double *beta, *mu, *hat, *conv;
+    int64_t ld_out;
+    int* status;
+    int* n_fallback;
+    int force;
+    int with_wald;
+    WideWald wald;
+    double *wald_p, *wald_stat, *wald_se;
+};
+
+// start value (utils.py:349-357) into `beta`; also returns sum lgamma(y + 1) - lgamma(y + r) through lgsum when asked
+__device__ void irls_start(const DesignS& d, const double* pinv, int p, int full_rank, const int64_t* y, int64_t ld, double r,
+                           Ws& ws, double* beta, double* lgsum) {
+    double* v = ws.v[0];
+    wfill(v, p, 0.0);
+    double logmean = 0.0, lg = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double t = 0.0;
+        if (n < d.N) {
+            const double yv = (double)y[(int64_t)n * ld];
+            const double q = yv / d.sf[n * d.RS];
+            if (full_rank) t = log(q + 0.1);
+            else logmean += log(q);
+            if (lgsum) lg += lgamma_pos(yv + 1.0) - lgamma_pos(yv + r);
+        }
+        __syncwarp();
+        ws.cz[lane_id()] = t;
+        __syncwarp();
+        if (full_rank) vec_chunk(d, p, n0, min(32, d.N - n0), ws.cz, v);
+    }
+    __syncwarp();
+    if (lgsum) *lgsum = wsum(lg);
+    if (full_rank) {
+        apply_pinv(pinv, v, beta, p);
+    } else {
+        logmean = wsum(logmean);
+        wfill(beta, p, 0.0);
+        __syncwarp();
+        if (lane_id() == 0) beta[0] = logmean / (double)d.N;
+        __syncwarp();
+    }
+}
+
+// one IRLS sweep at `beta`: A = X^T W X, b = X^T W z (W, z from the clamped mu); returns S = sum (y + r) log(r + mu) - y log(mu)
+__device__ double irls_sweep_w(const DesignS& d, int p, const int64_t* y, int64_t ld, const double* beta, double alpha, double r,
+                               double min_mu, double log_min_mu, Ws& ws, double* A, double* b) {
+    wfill(A, p * (p + 1) / 2, 0.0);
+    wfill(b, p, 0.0);
+    double S = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double W = 0.0, Wz = 0.0;
+        if (n < d.N) {
+            const double* x = row_of(d, n);
+            const double yv = (double)y[(int64_t)n * ld];
+            const double eta = xdot(x, beta, p);
+            const double sfn = x[p], lsfn = x[p + 1];
+            const double mu_raw = sfn * exp(eta);
+            const bool cl = mu_raw < min_mu;
+            const double mu = cl ? min_mu : mu_raw;
+            const double lmu = cl ? log_min_mu : (eta + lsfn);
+            const double iden = 1.0 / fma(mu, alpha, 1.0);
+            W = mu * iden;
+            Wz = fma(yv - mu, iden, W * (lmu - lsfn));
+            S += fma(yv + r, log(r + mu), -yv * lmu);
+        }
+        __syncwarp();
+        ws.cw[lane_id()] = W;
+        ws.cz[lane_id()] = Wz;
+        __syncwarp();
+        const int cnt = min(32, d.N - n0);
+        rank_chunk(d, p, n0, cnt, ws.cw, A);
+        vec_chunk(d, p, n0, cnt, ws.cz, b);
+    }
+    __syncwarp();
+    return wsum(S);
+}
+
+// mu (unclamped) and hat = W x^T H x with H = (A + ridge)^-1 (A: W from the clamped mu of `beta`); H ends in ws.L
+__device__ void irls_outputs(const DesignS& d, int p, const double* beta, double alpha, double min_mu, Ws& ws, const double* A,
+                             double* mu_out, double* hat_out, int64_t ld_out) {
+    factor_ridged(A, ws.L, p, kRidge, nullptr);
+    chol_inverse_w(ws.L, ws.Li, ws.L, p);
+    for (int n = lane_id(); n < d.N; n += 32) {
+        const double* x = row_of(d, n);
+        const double mu_raw = x[p] * exp(xdot(x, beta, p));
+        const double mu = (mu_raw < min_mu) ? min_mu : mu_raw;
+        mu_out[(int64_t)n * ld_out] = mu_raw;
+        hat_out[(int64_t)n * ld_out] = mu / fma(mu, alpha, 1.0) * quad_w(ws.L, x, p);
+    }
+}
+
+// M = sum w x x^T with w = mu / (1 + mu alpha) of the UNCLAMPED (clamped = false) or clamped mu of `beta`
+__device__ void weight_matrix(const DesignS& d, int p, const double* beta, double alpha, double min_mu, bool clamp, Ws& ws,
+                              double* M) {
+    wfill(M, p * (p + 1) / 2, 0.0);
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double W = 0.0;
+        if (n < d.N) {
+            const double* x = row_of(d, n);
+            const double mu_raw = x[p] * exp(xdot(x, beta, p));
+            const double mu = (clamp && mu_raw < min_mu) ? min_mu : mu_raw;
+            W = mu / fma(mu, alpha, 1.0);
+        }
+        __syncwarp();
+        ws.cw[lane_id()] = W;
+        __syncwarp();
+        rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, M);
+    }
+    __syncwarp();
+}
+
+// f(beta) = nb_nll (mu-dependent part) + 0.5 ridge |beta|^2, its gradient g and Hessian H (irls_obj_sweep)
+__device__ double obj_sweep_w(const DesignS& d, int p, const int64_t* y, int64_t ld, const double* beta, double alpha, double r,
+                              double min_mu, double log_min_mu, Ws& ws, double* g, double* H) {
+    wfill(H, p * (p + 1) / 2, 0.0);
+    wfill(g, p, 0.0);
+    double f = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double gi = 0.0, hi = 0.0;
+        if (n < d.N) {
+            const double* x = row_of(d, n);
+            const double yv = (double)y[(int64_t)n * ld];
+            const double eta = xdot(x, beta, p);
+            const double mu_raw = x[p] * exp(eta);
+            const bool cl = mu_raw < min_mu;
+            const double mu = cl ? min_mu : mu_raw;
+            const double lmu = cl ? log_min_mu : (eta + x[p + 1]);
+            f += fma(yv + r, log(r + mu), -yv * lmu);
+            const double t = (r + yv) * mu / (r + mu);
+            gi = t - yv;
+            hi = t * r / (r + mu);
+        }
+        __syncwarp();
+        ws.cw[lane_id()] = hi;
+        ws.cz[lane_id()] = gi;
+        __syncwarp();
+        const int cnt = min(32, d.N - n0);
+        rank_chunk(d, p, n0, cnt, ws.cw, H);
+        vec_chunk(d, p, n0, cnt, ws.cz, g);
+    }
+    __syncwarp();
+    f = wsum(f);
+    for (int j = 0; j < p; ++j) f = fma(0.5 * kRidge * beta[j], beta[j], f);
+    for (int j = lane_id(); j < p; j += 32) {
+        g[j] = fma(kRidge, beta[j], g[j]);
+        H[tri(j, j)] += kRidge;
+    }
+    __syncwarp();
+    return f;
+}
+
+__device__ __forceinline__ bool is_fixed(double b, double g, double lo, double hi) { return (b <= lo && g > 0.0) || (b >= hi && g < 0.0); }
+
+// the reference's L-BFGS-B branch (utils.py:374-413) as projected Newton: irls_optimizer_gene, every output written here
+__device__ void irls_optimizer_w(const IrlsArgsW& a, const DesignS& d, Ws& ws, int g) {
+    const int p = a.b.p, lane = lane_id();
+    const IrlsParams& prm = a.prm;
+    const int64_t* y = a.counts + g;
+    const double alpha = a.disp[g], r = 1.0 / alpha, log_min_mu = log(prm.min_mu);
+    double *beta = ws.v[1], *dir = ws.v[2], *gr = ws.v[3], *bt = ws.v[4], *gt = ws.v[5];
+    irls_start(d, a.b.pinv, p, prm.full_rank, y, a.ld, r, ws, beta, nullptr);
+    for (int j = lane; j < p; j += 32) beta[j] = fmin(fmax(beta[j], prm.min_beta), prm.max_beta);
+    __syncwarp();
+    double f = obj_sweep_w(d, p, y, a.ld, beta, alpha, r, prm.min_mu, log_min_mu, ws, gr, ws.A);
+    bool ok = false;
+    for (int it = 0; it < 100; ++it) {
+        double pg = 0.0;
+        for (int j = 0; j < p; ++j)
+            if (!is_fixed(beta[j], gr[j], prm.min_beta, prm.max_beta)) pg = fmax(pg, fabs(gr[j]));
+        if (pg <= 1e-9 * (1.0 + fabs(f)) || !(pg == pg)) {
+            ok = (pg == pg);
+            break;
+        }
+        // Newton direction on the free set: fixed rows / columns of H replaced by the identity
+        __syncwarp();
+        for (int i = lane; i < p; i += 32) {
+            const bool fi = is_fixed(beta[i], gr[i], prm.min_beta, prm.max_beta);
+            dir[i] = fi ? 0.0 : -gr[i];
+            for (int j = 0; j <= i; ++j) {
+                const bool fj = is_fixed(beta[j], gr[j], prm.min_beta, prm.max_beta);
+                ws.L[tri(i, j)] = (i == j) ? (fi ? 1.0 : ws.A[tri(i, i)]) : ((fi || fj) ? 0.0 : ws.A[tri(i, j)]);
+            }
+        }
+        chol_w(ws.L, p);
+        chol_solve_w(ws.L, dir, p);
+        double slope = 0.0;
+        for (int j = 0; j < p; ++j) slope = fma(gr[j], dir[j], slope);
+        if (!(slope < 0.0)) {  // not a descent direction (indefinite / NaN): steepest descent on the free set
+            __syncwarp();
+            for (int j = lane; j < p; j += 32) dir[j] = is_fixed(beta[j], gr[j], prm.min_beta, prm.max_beta) ? 0.0 : -gr[j];
+            __syncwarp();
+        }
+        // backtracking line search with projection onto the box; the trial Hessian goes to ws.Li
+        double step = 1.0, fn = f;
+        bool accepted = false;
+        for (int ls = 0; ls < 30; ++ls) {
+            __syncwarp();
+            for (int j = lane; j < p; j += 32) bt[j] = fmin(fmax(fma(step, dir[j], beta[j]), prm.min_beta), prm.max_beta);
+            __syncwarp();
+            double dec = 0.0;
+            for (int j = 0; j < p; ++j) dec = fma(gr[j], bt[j] - beta[j], dec);
+            const double ft = obj_sweep_w(d, p, y, a.ld, bt, alpha, r, prm.min_mu, log_min_mu, ws, gt, ws.Li);
+            if (ft <= f + 1e-4 * dec) {
+                accepted = true;
+                fn = ft;
+                break;
+            }
+            step *= 0.5;
+        }
+        if (!accepted) {  // line search failed: res.success == False
+            ok = false;
+            break;
+        }
+        const double df = f - fn;
+        f = fn;
+        wcopy(ws.A, ws.Li, p * (p + 1) / 2);
+        wcopy(gr, gt, p);
+        wcopy(beta, bt, p);
+        __syncwarp();
+        if (df <= 1e-15 * (1.0 + fabs(f))) {  // no further decrease possible in FP64
+            ok = true;
+            break;
+        }
+    }
+    if (prm.fail_optimizer) ok = false;
+    // (the two-column grid_fit_beta of utils.py:402-409 is never reached: p > 16 here)
+    if (a.with_wald) {
+        weight_matrix(d, p, beta, alpha, prm.min_mu, false, ws, ws.A);
+        wald_finish_w(ws.A, a.wald, beta, ws, a.wald_p + g, a.wald_stat + g, a.wald_se + g);
+    }
+    weight_matrix(d, p, beta, alpha, prm.min_mu, true, ws, ws.A);
+    irls_outputs(d, p, beta, alpha, prm.min_mu, ws, ws.A, a.mu + g, a.hat + g, a.ld_out);
+    for (int j = lane; j < p; j += 32) a.beta[(int64_t)g * p + j] = beta[j];
+    if (lane == 0) a.conv[g] = ok ? 1.0 : 0.0;
+}
+
+__global__ void __maxnreg__(224) k_wide_irls(const __grid_constant__ IrlsArgsW a) {
+    extern __shared__ __align__(16) double wsm[];
+    Ws ws = carve(wsm, a.b.p);
+    const int g = blockIdx.x, p = a.b.p, lane = lane_id();
+    const DesignS d = design_of(a.b.pack, a.b.N, p);
+    const IrlsParams& prm = a.prm;
+    const int64_t* y = a.counts + g;
+    const double alpha = a.disp[g], r = 1.0 / alpha, Nd = (double)d.N, log_min_mu = log(prm.min_mu);
+    double *b = ws.v[0], *beta = ws.v[1], *bh = ws.v[2];
+    double lgsum;
+    irls_start(d, a.b.pinv, p, prm.full_rank, y, a.ld, r, ws, beta, &lgsum);
+    const double C = Nd * r * log(alpha) + Nd * lgamma_pos(r) + lgsum;  // nb_nll = C + S(mu)
+    double dev = 1000.0, ratio = 1.0;
+    int it = 0, status = kIrlsOk;
+    bool first = true;
+    for (;;) {
+        const double S = irls_sweep_w(d, p, y, a.ld, beta, alpha, r, prm.min_mu, log_min_mu, ws, ws.A, b);
+        if (!first) {
+            const double old = dev;
+            dev = -2.0 * (C + S);
+            ratio = fabs(dev - old) / (fabs(dev) + 0.1);
+        }
+        first = false;
+        if (!(ratio > prm.beta_tol)) break;  // `while dev_ratio > beta_tol` (NaN exits)
+        factor_ridged(ws.A, ws.L, p, kRidge, nullptr);
+        wcopy(bh, b, p);
+        chol_solve_w(ws.L, bh, p);
+        ++it;
+        bool div = false;
+        for (int j = lane; j < p; j += 32) div = div || (fabs(bh[j]) > prm.max_beta);
+        if (wany(div) || it >= prm.maxiter) {
+            status = kIrlsNeedsOptimizer;
+            break;
+        }
+        wcopy(beta, bh, p);
+        __syncwarp();
+    }
+    if (a.force) status = kIrlsNeedsOptimizer;
+    if (status != kIrlsOk) {
+        if (lane == 0) {
+            a.status[g] = status;
+            if (a.n_fallback) atomicAdd(a.n_fallback, 1);
+        }
+        irls_optimizer_w(a, d, ws, g);
+        return;
+    }
+    irls_outputs(d, p, beta, alpha, prm.min_mu, ws, ws.A, a.mu + g, a.hat + g, a.ld_out);
+    if (a.with_wald) {
+        // run_wald_test uses the UNCLAMPED mu (ds.py:320-324): A + the correction of the samples on the min_mu clamp
+        for (int n0 = 0; n0 < d.N; n0 += 32) {
+            const int n = n0 + lane;
+            double wd = 0.0;
+            if (n < d.N) {
+                const double* x = row_of(d, n);
+                const double mu_raw = x[p] * exp(xdot(x, beta, p));
+                if (mu_raw < prm.min_mu) wd = mu_raw / fma(mu_raw, alpha, 1.0) - prm.min_mu / fma(prm.min_mu, alpha, 1.0);
+            }
+            if (!wany(wd != 0.0)) continue;
+            __syncwarp();
+            ws.cw[lane] = wd;
+            __syncwarp();
+            rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, ws.A);
+        }
+        __syncwarp();
+        wald_finish_w(ws.A, a.wald, beta, ws, a.wald_p + g, a.wald_stat + g, a.wald_se + g);
+    }
+    for (int j = lane; j < p; j += 32) a.beta[(int64_t)g * p + j] = beta[j];
+    if (lane == 0) {
+        a.conv[g] = 1.0;  // IRLS exits are "converged" (utils.py:365)
+        a.status[g] = kIrlsOk;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// alpha_mle (alpha_dloss / alpha_loss with the search and grid of pdq_gene.cuh)
+// ---------------------------------------------------------------------------------------------
+struct AlphaArgsW {
+    WideBase b;
+    AlphaParams prm;
+    const int64_t* counts;
+    int64_t ld;
+    const double* mu;
+    int64_t ld_mu;
+    const double* alpha_hat;
+    double *alpha, *conv;
+    int* status;
+    const double* prior_var_dev;
+    int force;
+    const double* hint_in;
+    double* hint_out;
+};
+
+// d loss / d log(alpha) at x (curv: also the NB part's curvature, see alpha_dloss)
+__device__ double dloss_w(const DesignS& d, int p, const AlphaParams& prm, const int64_t* y, int64_t ld, const double* mu,
+                          int64_t ld_mu, double x, double xhat, double* curv, Ws& ws) {
+    const double a = exp(x), r = 1.0 / a, Nd = (double)d.N;
+    const bool cr = prm.cr_reg != 0;
+    if (cr) {
+        wfill(ws.A, p * (p + 1) / 2, 0.0);
+        wfill(ws.Li, p * (p + 1) / 2, 0.0);
+    }
+    double Sg = 0.0, S2 = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double W = 0.0;
+        if (n < d.N) {
+            const double yv = (double)y[(int64_t)n * ld], m = mu[(int64_t)n * ld_mu];
+            const double inv = 1.0 / (r + m);
+            Sg += log(r + m) - digamma_pos(yv + r) + (yv - m) * inv;
+            if (curv) S2 += fma(-(yv - m) * inv, inv, inv - trigamma_pos(yv + r));
+            W = m * r * inv;
+        }
+        if (!cr) continue;
+        __syncwarp();
+        ws.cw[lane_id()] = W;
+        ws.cz[lane_id()] = W * W;
+        __syncwarp();
+        const int cnt = min(32, d.N - n0);
+        rank_chunk(d, p, n0, cnt, ws.cw, ws.A);
+        rank_chunk(d, p, n0, cnt, ws.cz, ws.Li);
+    }
+    __syncwarp();
+    Sg = wsum(Sg);
+    const double F = Nd * (digamma_pos(r) + x) + Sg;
+    double g = -r * F;
+    if (curv) {
+        S2 = wsum(S2);
+        const double Fp = Nd * (trigamma_pos(r) - a) + S2;
+        *curv = r * (F + r * Fp) + (prm.prior_reg ? 1.0 / prm.prior_var : 0.0);
+    }
+    if (cr) {
+        // tr((X^T W X)^-1 X^T W^2 X): A is factored in ws.L and inverted back into ws.L; ws.Li holds X^T W^2 X, so A's own buffer
+        // is the inverse's scratch
+        wcopy(ws.L, ws.A, p * (p + 1) / 2);
+        chol_w(ws.L, p);
+        chol_inverse_w(ws.L, ws.A, ws.L, p);
+        g -= 0.5 * a * symdot_w(ws.L, ws.Li, p);
+    }
+    if (prm.prior_reg) g += (x - xhat) / prm.prior_var;
+    return g;
+}
+
+// loss up to an alpha-independent constant, cr_reg on, no prior (the grid's objective, alpha_loss)
+__device__ double loss_w(const DesignS& d, int p, const int64_t* y, int64_t ld, const double* mu, int64_t ld_mu, double x, Ws& ws) {
+    const double a = exp(x), r = 1.0 / a, Nd = (double)d.N;
+    wfill(ws.A, p * (p + 1) / 2, 0.0);
+    double Sf = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double W = 0.0;
+        if (n < d.N) {
+            const double yv = (double)y[(int64_t)n * ld], m = mu[(int64_t)n * ld_mu];
+            const double rm = r + m;
+            Sf += fma(yv + r, log(rm), -lgamma_pos(yv + r));
+            W = m * r / rm;
+        }
+        __syncwarp();
+        ws.cw[lane_id()] = W;
+        __syncwarp();
+        rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, ws.A);
+    }
+    __syncwarp();
+    double f = Nd * (r * x + lgamma_pos(r)) + wsum(Sf);
+    chol_w(ws.A, p);
+    double ld2 = 0.0;
+    for (int i = 0; i < p; ++i) ld2 += log(ws.A[tri(i, i)]);
+    return f + 0.5 * (2.0 * ld2);
+}
+
+__global__ void __launch_bounds__(32) k_wide_alpha_mle(const __grid_constant__ AlphaArgsW a) {
+    extern __shared__ __align__(16) double wsm[];
+    Ws ws = carve(wsm, a.b.p);
+    const int g = blockIdx.x, p = a.b.p;
+    const DesignS d = design_of(a.b.pack, a.b.N, p);
+    AlphaParams prm = a.prm;
+    if (a.prior_var_dev) prm.prior_var = *a.prior_var_dev;
+    const int64_t* y = a.counts + g;
+    const double* mu = a.mu + g;
+    const Group grp{lane_id(), 32, 1};
+    alpha_search(grp, prm, a.alpha_hat[g],
+                 [&](double x, double xhat, double* curv) { return dloss_w(d, p, prm, y, a.ld, mu, a.ld_mu, x, xhat, curv, ws); },
+                 a.alpha + g, a.conv + g, a.status + g, true, a.hint_in ? a.hint_in + 2 * (int64_t)g : nullptr,
+                 a.hint_out ? a.hint_out + 2 * (int64_t)g : nullptr);
+    __syncwarp();
+    if (a.force && lane_id() == 0) {
+        a.status[g] = kAlphaNeedsGrid;
+        a.conv[g] = 0.0;
+    }
+    __syncwarp();
+    if (a.status[g] == kAlphaNeedsGrid)
+        alpha_grid_search(grp, prm.lo, prm.hi, [&](double x) { return loss_w(d, p, y, a.ld, mu, a.ld_mu, x, ws); }, a.alpha + g, true);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Wald tests
+// ---------------------------------------------------------------------------------------------
+struct WaldArgsW {
+    WideBase b;
+    WideWald w;
+    const double *disp, *lfc, *mu;
+    int64_t ld_mu;
+    double *pv, *stat, *se;
+};
+
+__global__ void __launch_bounds__(32) k_wide_wald(const __grid_constant__ WaldArgsW a) {
+    extern __shared__ __align__(16) double wsm[];
+    Ws ws = carve(wsm, a.b.p);
+    const int g = blockIdx.x, p = a.b.p;
+    const DesignS d = design_of(a.b.pack, a.b.N, p);
+    const double disp = a.disp[g];
+    wfill(ws.A, p * (p + 1) / 2, 0.0);
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double W = 0.0;
+        if (n < d.N) {
+            const double m = a.mu[(int64_t)n * a.ld_mu + g];
+            W = m / fma(m, disp, 1.0);
+        }
+        __syncwarp();
+        ws.cw[lane_id()] = W;
+        __syncwarp();
+        rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, ws.A);
+    }
+    __syncwarp();
+    wcopy(ws.v[1], a.lfc + (int64_t)g * p, p);
+    __syncwarp();
+    wald_finish_w(ws.A, a.w, ws.v[1], ws, a.pv + g, a.stat + g, a.se + g);
+}
+
+struct WaldKArgsW {
+    WideBase b;
+    double ridge[kMaxTri];
+    const double *disp, *lfc, *tab;  // tab (K, p + 2): contrast | lfc_null | alt
+    int K;
+    double *pv, *stat, *se;
+    int64_t ld_out;
+};
+
+__global__ void __launch_bounds__(32) k_wide_wald_contrasts(const __grid_constant__ WaldKArgsW a) {
+    extern __shared__ __align__(16) double wsm[];
+    Ws ws = carve(wsm, a.b.p);
+    const int g = blockIdx.x, p = a.b.p;
+    const DesignS d = design_of(a.b.pack, a.b.N, p);
+    double* beta = ws.v[1];
+    wcopy(beta, a.lfc + (int64_t)g * p, p);
+    __syncwarp();
+    weight_matrix(d, p, beta, a.disp[g], 0.0, false, ws, ws.A);  // mu = sf exp(x'beta), as k_mu_from_lfc writes it
+    wald_inverse_w(ws.A, a.ridge, ws);
+    for (int k = 0; k < a.K; ++k) {
+        const double* row = a.tab + (int64_t)k * (p + 2);
+        const double se = wald_se_w(ws.A, row, ws);
+        double pv, stat;
+        wald_alt(row, beta, p, se, row[p], (int)row[p + 1], pv, stat);
+        if (lane_id() == 0) {
+            a.pv[(int64_t)k * a.ld_out + g] = pv;
+            a.stat[(int64_t)k * a.ld_out + g] = stat;
+            a.se[(int64_t)k * a.ld_out + g] = se;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Cook's distances (cooks_gene with the warp as the gene's lane group)
+// ---------------------------------------------------------------------------------------------
+struct CooksArgsW {
+    WideBase b;
+    const int* plan;  // [n_cells, global_mode, starts (n_cells + 1), order (n_in_cells)]
+    int n_cells, n_in_cells;
+    const int64_t* counts;
+    int64_t ld;
+    const double *mu, *hat;
+    int64_t ld2;
+    double cutoff;
+    double* cooks;
+    int64_t ld_out;
+    double *disp, *outlier, *replaced;
+};
+
+__global__ void __launch_bounds__(32) k_wide_cooks(const __grid_constant__ CooksArgsW a) {
+    extern __shared__ __align__(16) double wsm[];
+    const int g = blockIdx.x;
+    const DesignS d = design_of(a.b.pack, a.b.N, a.b.p);
+    const CellPlan plan{a.plan + 2 + a.n_cells + 1, a.plan + 2, a.n_cells, a.plan[1]};
+    const Group grp{lane_id(), 32, 1};
+    cooks_gene_cols(grp, d, a.b.p, plan, a.counts + g, a.ld, a.mu + g, a.hat + g, a.ld2, a.cutoff, wsm, wsm + a.n_in_cells,
+                    a.cooks ? a.cooks + g : nullptr, a.ld_out, a.disp + g, a.outlier + g, a.replaced + g, true);
+}
+
+// ---------------------------------------------------------------------------------------------
+// launch helpers
+// ---------------------------------------------------------------------------------------------
+template <class K>
+int prep(K kernel, size_t smem) {
+    if (smem > kMaxDynSmem) return PDQ_ERR_UNSUPPORTED;
+    if (smem > 48 * 1024 && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+        return PDQ_ERR_CUDA;
+    return 0;
+}
+
+inline int check_launch() { return cudaGetLastError() == cudaSuccess ? 0 : PDQ_ERR_CUDA; }
+inline size_t ws_bytes(int p) { return wide_ws_doubles(p) * sizeof(double); }
+inline WideBase base_of(const DesignDev& d, int G) { return WideBase{d.pack, d.pinv_dev, d.N, d.p, G}; }
+
+void pack_lower(const double* full, int p, double* tri_out) {
+    for (int i = 0; i < p; ++i)
+        for (int j = 0; j <= i; ++j) tri_out[tri(i, j)] = full[i * p + j];
+}
+
+void wide_wald(const WaldHost& h, int p, WideWald& w) {
+    pack_lower(h.ridge, p, w.ridge);
+    for (int j = 0; j < p; ++j) w.contrast[j] = h.contrast[j];
+    w.lfc_null = h.lfc_null;
+    w.alt = h.alt;
+}
+
+}  // namespace
+
+int launch_lin_reg_mu_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
+                           int64_t ld_out) {
+    const LinArgs a{base_of(d, G), counts, ld, min_mu, mu_out, ld_out};
+    if (int e = prep(k_wide_lin_reg_mu, ws_bytes(d.p))) return e;
+    k_wide_lin_reg_mu<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_irls_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
+                     double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
+    if (n_fallback && cudaMemsetAsync(n_fallback, 0, sizeof(int), c.stream) != cudaSuccess) return PDQ_ERR_CUDA;
+    IrlsArgsW a{};
+    a.b = base_of(d, G);
+    a.prm = IrlsParams{h.min_mu, h.beta_tol, h.min_beta, h.max_beta, h.maxiter, d.full_rank, d.few_rows,
+                       (c.debug & PDQ_DEBUG_FAIL_IRLS_OPTIMIZER) ? 1 : 0};
+    a.counts = counts; a.ld = ld; a.disp = disp;
+    a.beta = beta; a.mu = mu; a.hat = hat; a.conv = conv; a.ld_out = ld_out;
+    a.status = status; a.n_fallback = n_fallback;
+    a.force = (c.debug & PDQ_DEBUG_FORCE_IRLS_OPTIMIZER) ? 1 : 0;
+    a.with_wald = w ? 1 : 0;
+    if (w) {
+        wide_wald(*w, d.p, a.wald);
+        a.wald_p = w->pv; a.wald_stat = w->stat; a.wald_se = w->se;
+    }
+    if (int e = prep(k_wide_irls, ws_bytes(d.p))) return e;
+    k_wide_irls<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_alpha_mle_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
+                          const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
+                          int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
+    const AlphaArgsW a{base_of(d, G), AlphaParams{log(min_disp), log(max_disp), prior_var, cr_reg, prior_reg}, counts, ld, mu, ld_mu,
+                       alpha_hat, alpha, conv, status, prior_var_dev, (c.debug & PDQ_DEBUG_FORCE_ALPHA_GRID) ? 1 : 0, hint_in, hint_out};
+    if (int e = prep(k_wide_alpha_mle, ws_bytes(d.p))) return e;
+    k_wide_alpha_mle<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_wald_wide(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu, int64_t ld_mu, int G,
+                     const double* ridge, const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
+    WaldArgsW a{};
+    a.b = base_of(d, G);
+    wide_wald(WaldHost{ridge, contrast, lfc_null, alt, pv, stat, se}, d.p, a.w);
+    a.disp = disp; a.lfc = lfc; a.mu = mu; a.ld_mu = ld_mu;
+    a.pv = pv; a.stat = stat; a.se = se;
+    if (int e = prep(k_wide_wald, ws_bytes(d.p))) return e;
+    k_wide_wald<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_wald_contrasts_wide(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
+                               const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
+    WaldKArgsW a{};
+    a.b = base_of(d, G);
+    pack_lower(ridge, d.p, a.ridge);
+    a.disp = disp; a.lfc = lfc; a.tab = tab; a.K = K;
+    a.pv = pv; a.stat = stat; a.se = se; a.ld_out = ld_out;
+    if (int e = prep(k_wide_wald_contrasts, ws_bytes(d.p))) return e;
+    k_wide_wald_contrasts<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_rough_wide(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {
+    const MomArgsW a{base_of(d, G), normed, nullptr, ld, d.s_mean_inv, 0.0, 0.0, 0.0, alpha, nullptr, nullptr, 0};
+    if (int e = prep(k_wide_rough, ws_bytes(d.p))) return e;
+    k_wide_rough<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_moments_wide(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha, double* all_zero) {
+    const MomArgsW a{base_of(d, G), normed, nullptr, ld, d.s_mean_inv, 0.0, 0.0, 0.0, alpha, all_zero, nullptr, 0};
+    k_wide_moments<<<G, 32, 0, c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_mom_from_counts_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp,
+                                double max_disp, double* alpha, double* normed_mean, double min_mu, double* mu_hat, int64_t ld_mu) {
+    const MomArgsW a{base_of(d, G), nullptr, counts, ld, d.s_mean_inv, min_disp, max_disp, min_mu, alpha, normed_mean, mu_hat, ld_mu};
+    if (int e = prep(k_wide_mom_from_counts, ws_bytes(d.p))) return e;
+    k_wide_mom_from_counts<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_mu_from_lfc_wide(const LaunchCfg& c, const DesignDev& d, const double* lfc, int G, double* mu, int64_t ld_out) {
+    const MuLfcArgsW a{base_of(d, G), lfc, mu, ld_out};
+    k_wide_mu_from_lfc<<<G, 32, 0, c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_cooks_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
+                      int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced) {
+    const size_t smem = 2 * (size_t)d.n_in_cells * sizeof(double);
+    const CooksArgsW a{base_of(d, G), d.cell_plan, d.n_cells, d.n_in_cells, counts, ld, mu, hat, ld2, cutoff, cooks, ld_out, disp,
+                       outlier, replaced};
+    if (int e = prep(k_wide_cooks, smem)) return e;
+    k_wide_cooks<<<G, 32, smem, c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+}  // namespace pdq

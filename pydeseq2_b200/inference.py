@@ -112,7 +112,7 @@ def _rows(a, dtype, name):
 class _CudaOps:
     """Raw ops on numpy buffers through the C ABI (host-buffer entry points)."""
 
-    def __init__(self, device=0, lanes_per_gene=0, pinned_outputs=True, ctx=None):
+    def __init__(self, device=0, lanes_per_gene=0, pinned_outputs=True, ctx=None, wide_designs=False):
         self.ctx = ctx if ctx is not None else _lib.Context(device)  # ctx: share an existing context (its device and stream)
         self.lib = self.ctx.lib
         self.pinned_outputs = pinned_outputs
@@ -120,6 +120,13 @@ class _CudaOps:
         self.d2h_bytes = 0
         if lanes_per_gene:
             self.ctx.check(self.lib.pdq_set_lanes_per_gene(self.ctx.h, int(lanes_per_gene)))
+        if wide_designs:
+            self.ctx.set_wide_designs(True)
+
+    @property
+    def max_p(self):
+        """Widest design the context accepts (the opt-in belongs to the context, so ops sharing it agree)."""
+        return _lib.PDQ_MAX_P_WIDE if getattr(self.ctx, "wide_designs", False) else _lib.PDQ_MAX_P
 
     def empty(self, shape):
         # large outputs land in recycled page-locked blocks: the D2H copy then runs at full PCIe rate
@@ -254,16 +261,20 @@ class B200Inference(_InferenceBase):
         0 (default) picks the lanes cooperating on one gene from the number of genes.
     trace : bool
         Record every plugin call in ``self.trace`` (method, milliseconds, bytes requested host→device / device→host).
+    wide_designs : bool
+        Also fit designs of 17 to 64 columns (paired designs such as ``~subject + condition``, factors with many levels) on the
+        wide-design kernels.  Off by default: such designs then raise ``B200Error`` as before.  Designs of up to 16 columns run
+        the same kernels either way.  apeGLM shrinkage (``lfc_shrink_nbinom_glm``) of a wide design is not implemented.
     """
 
     _TRACED = ("lin_reg_mu", "irls", "alpha_mle", "wald_test", "wald_tests", "fit_rough_dispersions", "fit_moments_dispersions",
                "dispersion_trend_gamma_glm", "lfc_shrink_nbinom_glm", "size_factors", "calculate_cooks", "adjust_pvalues")
 
     def __init__(self, device: int = 0, n_cpus: int | None = None, lanes_per_gene: int = 0, _ops=None, trace: bool = False,
-                 pinned_outputs: bool = True):
+                 pinned_outputs: bool = True, wide_designs: bool = False):
         # pinned_outputs: large results are returned in page-locked numpy blocks (full-rate device-to-host copies, and full-rate
         # uploads when the caller hands them back); False returns ordinary pageable arrays
-        self._ops = _ops if _ops is not None else _CudaOps(device, lanes_per_gene, pinned_outputs)
+        self._ops = _ops if _ops is not None else _CudaOps(device, lanes_per_gene, pinned_outputs, wide_designs=wide_designs)
         self._n_cpus = n_cpus or 1
         self.last_irls_fallbacks = 0
         # per-call tracing (the reference prints wall-clock per phase to stderr, dds.py:626-711 ...; a backend is better served by
@@ -665,11 +676,13 @@ class B200Inference(_InferenceBase):
         return lfcs, ih, conv
 
     # ------------------------------------------------------------------ helpers
-    @staticmethod
-    def _check_design(X, N, sf=None):
+    def _check_design(self, X, N, sf=None):
         if X.shape[0] != N:
             raise ValueError(f"design_matrix has {X.shape[0]} rows for {N} samples")
-        if X.shape[1] > _lib.PDQ_MAX_P:
+        max_p = getattr(self._ops, "max_p", _lib.PDQ_MAX_P)
+        if X.shape[1] > max_p:
+            if max_p > _lib.PDQ_MAX_P:
+                raise B200Error(f"design has {X.shape[1]} columns; wide designs support p <= {max_p}")
             raise B200Error(f"design has {X.shape[1]} columns; this build supports p <= {_lib.PDQ_MAX_P}")
         if sf is not None and sf.shape[0] != N:
             raise ValueError(f"size_factors has {sf.shape[0]} entries for {N} samples")
