@@ -75,8 +75,13 @@ int pdq_set_debug_flags(pdq_ctx* ctx, int flags);
 /* Designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns (paired designs ~subject + condition, factors with many levels): off by
  * default, and then such designs report PDQ_ERR_UNSUPPORTED as before.  With `on` != 0 they run on kernels in which one warp
  * owns one gene and keeps its p x p state once, in shared memory; designs of up to PDQ_MAX_P columns run the same kernels as
- * without it.  Above PDQ_MAX_P_WIDE, and for apeGLM shrinkage (pdq_lfc_shrink*) of any wide design: PDQ_ERR_UNSUPPORTED. */
+ * without it.  Above PDQ_MAX_P_WIDE: PDQ_ERR_UNSUPPORTED.  apeGLM shrinkage (pdq_lfc_shrink*) of a wide design is a second opt-in,
+ * pdq_set_wide_shrink; without it such calls report PDQ_ERR_UNSUPPORTED ("not implemented") as before. */
 int pdq_set_wide_designs(pdq_ctx* ctx, int on);
+/* apeGLM shrinkage of designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns (off by default).  It runs only on a context that also
+ * has pdq_set_wide_designs on: otherwise the design is refused with the message of pdq_set_wide_designs (p <= PDQ_MAX_P), also
+ * for a pack made while wide designs were on.  Outputs are those of the narrow path; no gene is refitted on a grid. */
+int pdq_set_wide_shrink(pdq_ctx* ctx, int on);
 /* Host only, no device needed: (X^T X)^+ (p x p row-major) and whether X (N x p, row-major, p <= PDQ_MAX_P_WIDE) has full column
  * rank, from the one-sided Jacobi SVD every design pack is built with (numpy.linalg.matrix_rank's tolerance). */
 int pdq_design_pinv(const double* X, int N, int p, double* pinv_out, int* full_rank_out);
@@ -118,6 +123,8 @@ int pdq_host_free(pdq_ctx* ctx, void* hptr);
 int pdq_memcpy_h2d(pdq_ctx* ctx, void* dst, const void* src, size_t bytes); /* async on ctx stream */
 int pdq_memcpy_d2h(pdq_ctx* ctx, void* dst, const void* src, size_t bytes); /* async on ctx stream */
 int pdq_memcpy_d2d(pdq_ctx* ctx, void* dst, const void* src, size_t bytes); /* async on ctx stream */
+/* async on ctx stream: `count` elements of `elem_bytes`, `src_stride` bytes apart on the device, packed into `dst` */
+int pdq_memcpy_d2h_strided(pdq_ctx* ctx, void* dst, const void* src, size_t elem_bytes, size_t src_stride, size_t count);
 int pdq_memset(pdq_ctx* ctx, void* dst, int value, size_t bytes);
 int pdq_sync(pdq_ctx* ctx);
 /* CUDA-event timing on the context's stream (bench.py): record slot 0/1, elapsed ms between them */

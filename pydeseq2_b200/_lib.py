@@ -44,6 +44,7 @@ _SIGNATURES = {
     "pdq_set_lanes_per_gene": (C.c_int, [c_ctx, C.c_int]),
     "pdq_set_debug_flags": (C.c_int, [c_ctx, C.c_int]),
     "pdq_set_wide_designs": (C.c_int, [c_ctx, C.c_int]),
+    "pdq_set_wide_shrink": (C.c_int, [c_ctx, C.c_int]),
     "pdq_design_pinv": (C.c_int, [f64p, C.c_int, C.c_int, f64p, C.POINTER(C.c_int)]),
     "pdq_launch_count": (C.c_int64, [c_ctx]),
     "pdq_buffer_epoch": (C.c_int64, [c_ctx]),
@@ -58,6 +59,7 @@ _SIGNATURES = {
     "pdq_host_free": (C.c_int, [c_ctx, C.c_void_p]),
     "pdq_memcpy_h2d": (C.c_int, [c_ctx, c_dptr, C.c_void_p, C.c_size_t]),
     "pdq_memcpy_d2h": (C.c_int, [c_ctx, C.c_void_p, c_dptr, C.c_size_t]),
+    "pdq_memcpy_d2h_strided": (C.c_int, [c_ctx, C.c_void_p, c_dptr, C.c_size_t, C.c_size_t, C.c_size_t]),
     "pdq_memcpy_d2d": (C.c_int, [c_ctx, c_dptr, c_dptr, C.c_size_t]),
     "pdq_memset": (C.c_int, [c_ctx, c_dptr, C.c_int, C.c_size_t]),
     "pdq_sync": (C.c_int, [c_ctx]),
@@ -188,12 +190,19 @@ class Context:
         self.h = h
         self.device = int(device)
         self.wide_designs = False  # pdq_set_wide_designs: designs of up to PDQ_MAX_P_WIDE columns
+        self.wide_shrink = False   # pdq_set_wide_shrink: apeGLM shrinkage of those designs
         self._pin_pool = {}  # nbytes -> [addresses] of released page-locked blocks (cudaHostAlloc is expensive)
 
     def set_wide_designs(self, on: bool = True):
         """Accept designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns on this context (off by default)."""
         self.check(self.lib.pdq_set_wide_designs(self.h, 1 if on else 0))
         self.wide_designs = bool(on)
+
+    def set_wide_shrink(self, on: bool = True):
+        """Run apeGLM shrinkage of designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns on this context (off by default; needs
+        :meth:`set_wide_designs` as well, or such designs are refused as without it)."""
+        self.check(self.lib.pdq_set_wide_shrink(self.h, 1 if on else 0))
+        self.wide_shrink = bool(on)
 
     def check(self, rc: int):
         if rc != 0:
@@ -239,6 +248,12 @@ class Context:
     def d2h(self, arr: np.ndarray, dptr):
         assert arr.flags.c_contiguous
         self.check(self.lib.pdq_memcpy_d2h(self.h, arr.ctypes.data_as(C.c_void_p), c_dptr(dptr), arr.nbytes))
+
+    def d2h_strided(self, arr: np.ndarray, dptr, stride: int):
+        """arr[i] = the element at dptr + i * stride bytes (one element per `stride` bytes of device memory)."""
+        assert arr.flags.c_contiguous and arr.ndim == 1
+        self.check(self.lib.pdq_memcpy_d2h_strided(self.h, arr.ctypes.data_as(C.c_void_p), c_dptr(dptr), arr.itemsize, int(stride),
+                                                   arr.size))
 
     def sync(self):
         self.check(self.lib.pdq_sync(self.h))

@@ -162,6 +162,7 @@ struct pdq_ctx {
     int pipeline = 4;        // gene blocks per pipelined call; PDQ_PIPELINE=0 disables
     int debug = 0;           // PDQ_DEBUG_* test hooks
     int wide = 0;            // designs of up to PDQ_MAX_P_WIDE columns (pdq_set_wide_designs)
+    int wide_shrink = 0;     // apeGLM shrinkage of those designs (pdq_set_wide_shrink)
     int64_t launches_at_capture = 0;
     int64_t buf_epoch = 0;   // bumped whenever ensure() re-allocates a context-owned buffer (captured graphs hold those pointers)
     NcclApi nccl;
@@ -368,6 +369,12 @@ extern "C" int pdq_set_wide_designs(pdq_ctx* c, int on) {
     return PDQ_OK;
 }
 
+extern "C" int pdq_set_wide_shrink(pdq_ctx* c, int on) {
+    if (!c) return PDQ_ERR_INVALID;
+    c->wide_shrink = on != 0;
+    return PDQ_OK;
+}
+
 extern "C" int pdq_design_pinv(const double* X, int N, int p, double* pinv_out, int* full_rank_out) {
     if (!X || !pinv_out || !full_rank_out || N <= 0 || p < 1 || p > PDQ_MAX_P_WIDE) return PDQ_ERR_INVALID;
     design_linear_algebra(X, N, p, pinv_out, full_rank_out);
@@ -407,6 +414,11 @@ extern "C" int pdq_memcpy_h2d(pdq_ctx* c, void* dst, const void* src, size_t byt
 extern "C" int pdq_memcpy_d2h(pdq_ctx* c, void* dst, const void* src, size_t bytes) {
     if (!c) return PDQ_ERR_INVALID;
     CU(c, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
+    return PDQ_OK;
+}
+extern "C" int pdq_memcpy_d2h_strided(pdq_ctx* c, void* dst, const void* src, size_t elem_bytes, size_t src_stride, size_t count) {
+    if (!c || elem_bytes == 0 || src_stride < elem_bytes) return PDQ_ERR_INVALID;
+    if (count) CU(c, cudaMemcpy2DAsync(dst, elem_bytes, src, src_stride, elem_bytes, count, cudaMemcpyDeviceToHost, c->stream));
     return PDQ_OK;
 }
 extern "C" int pdq_memcpy_d2d(pdq_ctx* c, void* dst, const void* src, size_t bytes) {
@@ -761,7 +773,11 @@ extern "C" int pdq_lfc_shrink_dev(pdq_ctx* c, const pdq_design* d, const int64_t
     if (!d || !counts || !size || !lfcs || !inv_hessians || !conv || !status || G <= 0 || ld < G || shrink_index < 0 ||
         shrink_index >= d->d.p || !(prior_no_shrink_scale > 0.0) || !(prior_scale > 0.0))
         return fail(c, PDQ_ERR_INVALID, "pdq_lfc_shrink_dev: bad arguments");
-    if (d->d.p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
+    if (d->d.p > PDQ_MAX_P) {
+        if (!c->wide_shrink)
+            return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
+        if (int e = check_width(c, d->d.p)) return e;  // a pack made before the wide-design opt-in was turned off
+    }
     return done(c, launch_lfc_shrink(cfg(c, G, d->d.N), d->d, counts, ld, G, size, prior_no_shrink_scale, prior_scale, shrink_index, lfcs,
                                      inv_hessians, conv, status), "lfc_shrink");
 }
@@ -1593,7 +1609,8 @@ extern "C" int pdq_lfc_shrink_nbinom_glm(pdq_ctx* c, const double* X, const int6
         return fail(c, PDQ_ERR_INVALID, "pdq_lfc_shrink_nbinom_glm: bad arguments");
     pdq_design* d;  // the kernel reads the offsets from the log-size-factor row of the design pack
     if (int e = cached_design(c, X, offset, N, p, &d, true)) return e;
-    if (p > PDQ_MAX_P) return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
+    if (p > PDQ_MAX_P && !c->wide_shrink)
+        return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
     void *dc, *dsize, *dbeta, *dih, *dconv, *status;
     res_begin(c);
     bool up_c;

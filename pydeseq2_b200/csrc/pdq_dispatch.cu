@@ -3,8 +3,9 @@
 // pdq_kernels.cu is compiled once for p = 1..8 (p x p algebra unrolled in registers) and once per wide width p = 9..16
 // (same source, the small matrices in local memory): see the note at the top of that file and pydeseq2_b200/build.py.  Every
 // unit exports its launchers under a suffixed name; the functions declared in pdq_internal.h live here.  Designs of 17..64
-// columns (only created on contexts that opted in) go to pdq_wide.cu's launchers (`_wide`); the fused MAP -> LFC pair and apeGLM
-// shrinkage have none, so those report PDQ_ERR_UNSUPPORTED for them.
+// columns (only created on contexts that opted in) go to pdq_wide.cu's launchers (`_wide`).  The fused MAP -> LFC pair has none and
+// reports PDQ_ERR_UNSUPPORTED for them; apeGLM shrinkage reaches its wide launcher only on a context that also opted in to wide
+// shrinkage (pdq_set_wide_shrink, checked in pdq_api.cu).
 #include "pdq_internal.h"
 
 namespace pdq {
@@ -124,12 +125,12 @@ int launch_cooks(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, 
 #define DECL_SHRINK(sfx)                                                                                                      \
     int launch_lfc_shrink##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, const double*, double, double, \
                                int, double*, double*, double*, int*);
-PDQ_UNITS(DECL_SHRINK)
+PDQ_UNITS_ALL(DECL_SHRINK)
 int launch_lfc_shrink(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* size,
                       double prior_no_shrink_scale, double prior_scale, int shrink_index, double* beta, double* inv_hessian, double* conv,
                       int* status) {
-    PDQ_ROUTE(launch_lfc_shrink, d.p, c, d, counts, ld, G, size, prior_no_shrink_scale, prior_scale, shrink_index, beta, inv_hessian, conv,
-              status)
+    PDQ_ROUTE_WIDE(launch_lfc_shrink, d.p, c, d, counts, ld, G, size, prior_no_shrink_scale, prior_scale, shrink_index, beta, inv_hessian,
+                   conv, status)
 }
 
 }  // namespace pdq

@@ -18,6 +18,7 @@
 
 #include "pdq_gene.cuh"
 #include "pdq_internal.h"
+#include "pdq_shrink.cuh"
 
 namespace pdq {
 namespace {
@@ -993,6 +994,323 @@ __global__ void __launch_bounds__(32) k_wide_cooks(const __grid_constant__ Cooks
 }
 
 // ---------------------------------------------------------------------------------------------
+// apeGLM shrinkage (shrink_gene / shrink_eval / shrink_inv_hessian of pdq_shrink.cuh)
+// ---------------------------------------------------------------------------------------------
+// The narrow driver keeps its vectors in per-lane register arrays indexed by unrolled loops; here they are shared-memory vectors
+// split over the lanes, so the driver below restates shrink_gene step for step (the line search, dcsrch_start / dcsrch_step /
+// dcstep, is shared as is).  Every scalar of the optimiser is computed redundantly on all lanes from butterfly sums or shared
+// vectors, so all branches are warp-uniform.
+//
+// Workspace of one gene: two packed p x p matrices (X'FX and its inverse's scratch), kShrinkVecs vectors of p, the L-BFGS memory
+// S, Y (2 kShrinkMem p) with s'y and the two-loop's alphas (kShrinkMem each), two chunk buffers of 32.
+constexpr int kShrinkVecs = 9;
+__host__ __device__ constexpr size_t shrink_ws_doubles(int p) {
+    return 2 * (size_t)tri_count(p) + (size_t)(kShrinkVecs + 2 * kShrinkMem) * p + 2 * kShrinkMem + 64;
+}
+
+struct ShrinkWs {
+    double *A, *Li;
+    double *x, *g, *t, *r, *dir, *z, *xt, *gt, *q;
+    double *S, *Y, *sy, *al;
+    double *cw, *cz;
+};
+
+__device__ __forceinline__ ShrinkWs carve_shrink(double* s, int p) {
+    ShrinkWs w;
+    const int t = tri_count(p);
+    w.A = s;
+    w.Li = s + t;
+    double* v = s + 2 * t;
+    double** vecs[kShrinkVecs] = {&w.x, &w.g, &w.t, &w.r, &w.dir, &w.z, &w.xt, &w.gt, &w.q};
+    for (int k = 0; k < kShrinkVecs; ++k) *vecs[k] = v + k * p;
+    w.S = v + kShrinkVecs * p;
+    w.Y = w.S + kShrinkMem * p;
+    w.sy = w.Y + kShrinkMem * p;
+    w.al = w.sy + kShrinkMem;
+    w.cw = w.al + kShrinkMem;
+    w.cz = w.cw + 32;
+    return w;
+}
+
+// sum_j a[j] b[j], lanes over the components, butterfly total (bit-identical on every lane)
+__device__ __forceinline__ double wdot(const double* a, const double* b, int p) {
+    double s = 0.0;
+    for (int j = lane_id(); j < p; j += 32) s = fma(a[j], b[j], s);
+    return wsum(s);
+}
+__device__ __forceinline__ double wmaxabs(const double* a, int p) {
+    double m = 0.0;
+    for (int j = lane_id(); j < p; j += 32) m = fmax(m, fabs(a[j]));
+    for (int o = 16; o; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    return m;
+}
+
+// unscaled f (returned) and, when `grad`, its gradient: shrink_eval
+__device__ double shrink_eval_w(const DesignS& d, int p, const ShrinkParams& prm, const int64_t* y, int64_t ld, double size,
+                                double lsize, const double* beta, double* grad, ShrinkWs& ws) {
+    if (grad) wfill(grad, p, 0.0);
+    double nll = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double gi = 0.0;
+        if (n < d.N) {
+            const double* x = row_of(d, n);
+            const double yv = (double)y[(int64_t)n * ld];
+            const double xb = xdot(x, beta, p);
+            const double e = xb + x[p + 1];
+            const double dd = e - lsize;
+            const double t = exp(-fabs(dd));               // in (0, 1]
+            const double lae = fmax(e, lsize) + log1p(t);  // logaddexp(e, log s)
+            const double ys = yv + size;
+            nll += yv * xb - ys * lae;
+            const double q = ((dd >= 0.0) ? 1.0 : t) / (1.0 + t);  // 1 / (1 + s exp(-e)) without overflow
+            gi = ys * q - yv;
+        }
+        if (!grad) continue;
+        __syncwarp();
+        ws.cz[lane_id()] = gi;
+        __syncwarp();
+        vec_chunk(d, p, n0, min(32, d.N - n0), ws.cz, grad);
+    }
+    nll = wsum(nll);
+    double prior = 0.0;
+    for (int j = 0; j < p; ++j)
+        prior += (j == prm.k) ? log1p(beta[j] * beta[j] / prm.scale2) : 0.5 * beta[j] * beta[j] * prm.inv_var0;
+    if (grad) {
+        __syncwarp();
+        for (int j = lane_id(); j < p; j += 32)
+            grad[j] += (j == prm.k) ? 2.0 * beta[j] / (prm.scale2 + beta[j] * beta[j]) : beta[j] * prm.inv_var0;
+    }
+    __syncwarp();
+    return prior - nll;
+}
+
+// shrink_inv_hessian: (X'FX + 1 h')^-1 through Sherman-Morrison on the Cholesky factor of A = X'FX, written to ih (p x p)
+__device__ void shrink_inv_hessian_w(const DesignS& d, int p, const ShrinkParams& prm, const int64_t* y, int64_t ld, double size,
+                                     double lsize, const double* beta, double* ih, ShrinkWs& ws) {
+    wfill(ws.A, p * (p + 1) / 2, 0.0);
+    for (int n0 = 0; n0 < d.N; n0 += 32) {
+        const int n = n0 + lane_id();
+        double w = 0.0;
+        if (n < d.N) {
+            const double* x = row_of(d, n);
+            const double yv = (double)y[(int64_t)n * ld];
+            const double dd = xdot(x, beta, p) + x[p + 1] - lsize;
+            const double t = exp(-fabs(dd));
+            w = (yv + size) * (t / ((1.0 + t) * (1.0 + t)));  // (y+s) q (1-q)
+        }
+        __syncwarp();
+        ws.cw[lane_id()] = w;
+        __syncwarp();
+        rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, ws.A);
+    }
+    chol_w(ws.A, p);
+    chol_inverse_w(ws.A, ws.Li, ws.A, p);  // A^-1 in ws.A
+    double *h = ws.t, *u = ws.r, *v = ws.q;  // the optimiser's vectors are free now
+    const double bk = beta[prm.k], den = prm.scale2 + bk * bk;
+    for (int j = lane_id(); j < p; j += 32) h[j] = (j == prm.k) ? 2.0 * (prm.scale2 - bk * bk) / (den * den) : prm.inv_var0;
+    __syncwarp();
+    for (int i = lane_id(); i < p; i += 32) {
+        double su = 0.0, sv = 0.0;
+        for (int j = 0; j < p; ++j) {
+            const double aij = ws.A[j <= i ? tri(i, j) : tri(j, i)];
+            su += aij;
+            sv = fma(aij, h[j], sv);
+        }
+        u[i] = su;
+        v[i] = sv;
+    }
+    __syncwarp();
+    const double inv = 1.0 / (1.0 + wdot(h, u, p));
+    for (int k = lane_id(); k < p * p; k += 32) {
+        const int i = k / p, j = k - i * p;
+        ih[k] = ws.A[j <= i ? tri(i, j) : tri(j, i)] - u[i] * v[j] * inv;
+    }
+}
+
+// z = x + (L-BFGS step), with an empty memory z = x - g / theta: lbfgs_point
+__device__ void lbfgs_point_w(int p, int col, int head, double theta, ShrinkWs& ws) {
+    const int lane = lane_id();
+    for (int j = lane; j < p; j += 32) ws.q[j] = -ws.g[j];
+    __syncwarp();
+    if (col == 0) {
+        for (int j = lane; j < p; j += 32) ws.z[j] = ws.x[j] + (1.0 / theta) * ws.q[j];
+        __syncwarp();
+        return;
+    }
+    for (int i = col - 1; i >= 0; --i) {  // newest -> oldest
+        const int s = (head + i) % kShrinkMem;
+        const double a = wdot(ws.S + s * p, ws.q, p) / ws.sy[s];
+        if (lane == 0) ws.al[i] = a;
+        for (int j = lane; j < p; j += 32) ws.q[j] = ws.q[j] - a * ws.Y[s * p + j];
+        __syncwarp();
+    }
+    for (int j = lane; j < p; j += 32) ws.q[j] = ws.q[j] / theta;
+    __syncwarp();
+    for (int i = 0; i < col; ++i) {  // oldest -> newest
+        const int s = (head + i) % kShrinkMem;
+        const double b = wdot(ws.Y + s * p, ws.q, p) / ws.sy[s];
+        for (int j = lane; j < p; j += 32) ws.q[j] = ws.q[j] + ws.S[s * p + j] * (ws.al[i] - b);
+        __syncwarp();
+    }
+    for (int j = lane; j < p; j += 32) ws.z[j] = ws.x[j] + ws.q[j];
+    __syncwarp();
+}
+
+struct ShrinkArgsW {
+    WideBase b;
+    ShrinkParams prm;
+    const int64_t* counts;
+    int64_t ld;
+    const double* size;
+    double *beta, *ih, *conv;
+    int* status;
+};
+
+// shrink_gene: beta_init +-0.1, scale max(f(0), 1), m = 10 two-loop direction, dcsrch with maxls 20, the update skip, the restarts,
+// ftol = gtol = 1e-8 and the evaluation budget; no grid fallback (two-column designs only)
+__global__ void __launch_bounds__(32) k_wide_lfc_shrink(const __grid_constant__ ShrinkArgsW a) {
+    extern __shared__ __align__(16) double wsm[];
+    const int g = blockIdx.x, p = a.b.p, lane = lane_id();
+    ShrinkWs ws = carve_shrink(wsm, p);
+    const DesignS d = design_of(a.b.pack, a.b.N, p);
+    const ShrinkParams prm = a.prm;
+    const int64_t* y = a.counts + g;
+    const double size = a.size[g], lsize = log(size);
+    const double ftol = 1e-8, gtol = 1e-8;
+    wfill(ws.x, p, 0.0);
+    __syncwarp();
+    double f = shrink_eval_w(d, p, prm, y, a.ld, size, lsize, ws.x, nullptr, ws);
+    const double cnst = (f < 1.0) ? 1.0 : f;  // np.maximum(scale_cnst, 1)
+    for (int j = lane; j < p; j += 32) ws.x[j] = (j & 1) ? -0.1 : 0.1;
+    __syncwarp();
+    f = shrink_eval_w(d, p, prm, y, a.ld, size, lsize, ws.x, ws.g, ws) / cnst;
+    for (int j = lane; j < p; j += 32) ws.g[j] = ws.g[j] / cnst;
+    __syncwarp();
+
+    int col = 0, head = 0;
+    double theta = 1.0;
+    LineSearch ls;
+    double fold = f, gdold = 0.0, stp = 1.0;
+    int nit = 0, iback = 0;
+    bool active = true, ok = false;
+
+    auto set_trial = [&]() {  // xt = t + stp dir (z itself at stp = 1)
+        for (int j = lane; j < p; j += 32) ws.xt[j] = (stp == 1.0) ? ws.z[j] : fma(stp, ws.dir[j], ws.t[j]);
+        __syncwarp();
+    };
+    // prepares the next line search from (x, f, g); returns false on ABNORMAL_TERMINATION_IN_LNSRCH
+    auto begin_iteration = [&]() -> bool {
+        for (;;) {
+            lbfgs_point_w(p, col, head, theta, ws);
+            for (int j = lane; j < p; j += 32) ws.dir[j] = ws.z[j] - ws.x[j];
+            __syncwarp();
+            const double dtd = wdot(ws.dir, ws.dir, p), gd = wdot(ws.g, ws.dir, p);
+            stp = (nit == 0) ? fmin(1.0 / sqrt(dtd), kLsStpMax) : 1.0;
+            wcopy(ws.t, ws.x, p);
+            wcopy(ws.r, ws.g, p);
+            __syncwarp();
+            fold = f;
+            gdold = gd;
+            iback = 0;
+            if (!(gd < 0.0)) {  // not a descent direction: drop the memory and retry, or give up
+                if (col == 0) return false;
+                col = 0;
+                head = 0;
+                theta = 1.0;
+                continue;
+            }
+            dcsrch_start(ls, stp, f, gd);
+            set_trial();
+            return true;
+        }
+    };
+
+    if (wmaxabs(ws.g, p) <= gtol) {
+        ok = true;
+        active = false;
+    }
+    if (active && !begin_iteration()) active = false;
+    for (int ev = 0; ev < kShrinkMaxEval && active; ++ev) {
+        const double ft = shrink_eval_w(d, p, prm, y, a.ld, size, lsize, ws.xt, ws.gt, ws);
+        f = ft / cnst;
+        for (int j = lane; j < p; j += 32) {
+            ws.g[j] = ws.gt[j] / cnst;
+            ws.x[j] = ws.xt[j];
+        }
+        __syncwarp();
+        const double gd = wdot(ws.g, ws.dir, p);
+        if (dcsrch_step(ls, stp, f, gd)) {  // another trial point
+            if (++iback >= kShrinkMaxLs) {  // line search failed: restore, restart from steepest descent or give up
+                wcopy(ws.x, ws.t, p);
+                wcopy(ws.g, ws.r, p);
+                __syncwarp();
+                f = fold;
+                if (col == 0) {
+                    active = false;
+                    continue;
+                }
+                col = 0;
+                head = 0;
+                theta = 1.0;
+                if (!begin_iteration()) active = false;
+                continue;
+            }
+            set_trial();
+            continue;
+        }
+        // ---- new iterate
+        ++nit;
+        if (wmaxabs(ws.g, p) <= gtol || (fold - f) <= ftol * fmax(fmax(fabs(fold), fabs(f)), 1.0)) {
+            ok = true;
+            active = false;
+            continue;
+        }
+        if (nit >= kShrinkMaxIter) {
+            active = false;
+            continue;
+        }
+        // memory update (skipped when the curvature s'y is not safely positive); y = g - r
+        double rr = 0.0;
+        for (int j = lane; j < p; j += 32) {
+            const double yj = ws.g[j] - ws.r[j];
+            rr = fma(yj, yj, rr);
+        }
+        rr = wsum(rr);
+        const double dr = (stp == 1.0) ? (gd - gdold) : (gd - gdold) * stp;
+        const double ddum = (stp == 1.0) ? -gdold : -gdold * stp;
+        if (dr > 2.220446049250313e-16 * ddum) {
+            int slot;
+            if (col < kShrinkMem) {
+                slot = (head + col) % kShrinkMem;
+                ++col;
+            } else {
+                slot = head;
+                head = (head + 1) % kShrinkMem;
+            }
+            double *Ss = ws.S + slot * p, *Ys = ws.Y + slot * p;
+            for (int j = lane; j < p; j += 32) {
+                Ss[j] = (stp == 1.0) ? ws.dir[j] : stp * ws.dir[j];
+                Ys[j] = ws.g[j] - ws.r[j];
+            }
+            __syncwarp();
+            const double sy = wdot(Ys, Ss, p);
+            if (lane == 0) ws.sy[slot] = sy;
+            __syncwarp();
+            theta = rr / dr;
+        }
+        if (!begin_iteration()) active = false;
+    }
+    // `active` still set: evaluation budget exhausted -> not converged
+    shrink_inv_hessian_w(d, p, prm, y, a.ld, size, lsize, ws.x, a.ih + (int64_t)g * p * p, ws);
+    for (int j = lane; j < p; j += 32) a.beta[(int64_t)g * p + j] = ws.x[j];
+    if (lane == 0) {
+        a.conv[g] = ok ? 1.0 : 0.0;
+        a.status[g] = kShrinkOk;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // launch helpers
 // ---------------------------------------------------------------------------------------------
 template <class K>
@@ -1127,6 +1445,19 @@ int launch_cooks_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* cou
                        outlier, replaced};
     if (int e = prep(k_wide_cooks, smem)) return e;
     k_wide_cooks<<<G, 32, smem, c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_lfc_shrink_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* size,
+                           double prior_no_shrink_scale, double prior_scale, int shrink_index, double* beta, double* inv_hessian,
+                           double* conv, int* status) {
+    if (shrink_index < 0 || shrink_index >= d.p) return PDQ_ERR_INVALID;
+    const ShrinkArgsW a{base_of(d, G), ShrinkParams{1.0 / (prior_no_shrink_scale * prior_no_shrink_scale), prior_scale * prior_scale, shrink_index},
+                        counts, ld, size, beta, inv_hessian, conv, status};
+    const size_t smem = shrink_ws_doubles(d.p) * sizeof(double);
+    if (int e = prep(k_wide_lfc_shrink, smem)) return e;
+    k_wide_lfc_shrink<<<G, 32, smem, c.stream>>>(a);
     if (int e = check_launch()) return e;
     return 1;
 }

@@ -112,7 +112,7 @@ def _rows(a, dtype, name):
 class _CudaOps:
     """Raw ops on numpy buffers through the C ABI (host-buffer entry points)."""
 
-    def __init__(self, device=0, lanes_per_gene=0, pinned_outputs=True, ctx=None, wide_designs=False):
+    def __init__(self, device=0, lanes_per_gene=0, pinned_outputs=True, ctx=None, wide_designs=False, wide_shrink=False):
         self.ctx = ctx if ctx is not None else _lib.Context(device)  # ctx: share an existing context (its device and stream)
         self.lib = self.ctx.lib
         self.pinned_outputs = pinned_outputs
@@ -122,6 +122,8 @@ class _CudaOps:
             self.ctx.check(self.lib.pdq_set_lanes_per_gene(self.ctx.h, int(lanes_per_gene)))
         if wide_designs:
             self.ctx.set_wide_designs(True)
+        if wide_shrink:
+            self.ctx.set_wide_shrink(True)
 
     @property
     def max_p(self):
@@ -264,17 +266,24 @@ class B200Inference(_InferenceBase):
     wide_designs : bool
         Also fit designs of 17 to 64 columns (paired designs such as ``~subject + condition``, factors with many levels) on the
         wide-design kernels.  Off by default: such designs then raise ``B200Error`` as before.  Designs of up to 16 columns run
-        the same kernels either way.  apeGLM shrinkage (``lfc_shrink_nbinom_glm``) of a wide design is not implemented.
+        the same kernels either way.
+    wide_shrink : bool
+        Also run apeGLM shrinkage (``lfc_shrink_nbinom_glm``, ``DeseqStats.lfc_shrink``) of such designs on the GPU.  Needs
+        ``wide_designs=True``.  Off by default: shrinking a wide design then raises ``B200Error`` ("not implemented"), so a
+        caller that shrinks those on the CPU keeps working unchanged.
     """
 
     _TRACED = ("lin_reg_mu", "irls", "alpha_mle", "wald_test", "wald_tests", "fit_rough_dispersions", "fit_moments_dispersions",
                "dispersion_trend_gamma_glm", "lfc_shrink_nbinom_glm", "size_factors", "calculate_cooks", "adjust_pvalues")
 
     def __init__(self, device: int = 0, n_cpus: int | None = None, lanes_per_gene: int = 0, _ops=None, trace: bool = False,
-                 pinned_outputs: bool = True, wide_designs: bool = False):
+                 pinned_outputs: bool = True, wide_designs: bool = False, wide_shrink: bool = False):
+        if wide_shrink and not wide_designs:
+            raise ValueError("wide_shrink=True needs wide_designs=True")
         # pinned_outputs: large results are returned in page-locked numpy blocks (full-rate device-to-host copies, and full-rate
         # uploads when the caller hands them back); False returns ordinary pageable arrays
-        self._ops = _ops if _ops is not None else _CudaOps(device, lanes_per_gene, pinned_outputs, wide_designs=wide_designs)
+        self._ops = _ops if _ops is not None else _CudaOps(device, lanes_per_gene, pinned_outputs, wide_designs=wide_designs,
+                                                                     wide_shrink=wide_shrink)
         self._n_cpus = n_cpus or 1
         self.last_irls_fallbacks = 0
         # per-call tracing (the reference prints wall-clock per phase to stderr, dds.py:626-711 ...; a backend is better served by

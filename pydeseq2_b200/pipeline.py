@@ -967,7 +967,8 @@ class ResidentFit:
     # -- apeGLM shrinkage on the resident counts ----------------------------------------------------------
     def lfc_shrink(self, result, coeff_idx: int, adapt: bool = True, se=None, prior_scale=None):
         """``DeseqStats.lfc_shrink`` (ds.py:363-443) after :meth:`run`: counts, design pack and dispersions are already in HBM,
-        so the call moves 8*G bytes up (size = 1/dispersion) and 8*G*(p*p+p+1) down.  ``result`` is what :meth:`run`
+        so the call moves 8*G bytes up (size = 1/dispersion) and 24*G down: the shrunk column, the [k, k] entries of the inverse
+        Hessians (the kernel writes all p*p of them on the device) and the convergence flags.  ``result`` is what :meth:`run`
         returned; the prior scale comes from its LFC column ``coeff_idx`` and ``se`` (default: the Wald SEs of that run, i.e.
         the run's contrast must have selected the same coefficient).  With gene shards pass ``prior_scale`` computed from the
         gathered tables (the prior is global over genes).  Returns a :class:`ShrinkResult` for this shard's genes."""
@@ -982,9 +983,8 @@ class ResidentFit:
                 prior_var = fit_shrink_prior_var(np.asarray(result["lfc"])[:, coeff_idx],
                                                  np.asarray(result["se"] if se is None else se, dtype=float))
                 prior_scale = float(np.minimum(np.sqrt(prior_var), 1))
-        host = ctx.pinned_empty((G * (1 + p + p * p + 1),))
-        size, lfcs = host[:G], host[G:G + G * p].reshape(G, p)
-        ih, conv = host[G + G * p:G + G * p + G * p * p].reshape(G, p, p), host[G + G * p + G * p * p:]
+        host = ctx.pinned_empty((4 * G,))
+        size, lfc_k, ih_kk, conv = host[:G], host[G:2 * G], host[2 * G:3 * G], host[3 * G:]
         disp_in = np.asarray(result["dispersions"])
         size[:] = 1.0 / (disp_in if self._perm is None else disp_in[self._perm])  # device gene order
         d_size, d_out = self._dev("shrink_size", G * 8), self._dev("shrink_out", G * (p + p * p + 1) * 8)
@@ -992,15 +992,18 @@ class ResidentFit:
         ctx.h2d(d_size, size)
         ctx.check(L.pdq_lfc_shrink_dev(h, self.design, c_d(self._main.counts), G, G, c_d(d_size), 15.0, float(prior_scale), int(coeff_idx),
                                        c_d(d_out), c_d(d_out + G * p * 8), c_d(d_out + G * (p + p * p) * 8), c_d(d_status)))
-        ctx.d2h(host[G:], d_out)
+        k = int(coeff_idx)
+        ctx.d2h_strided(lfc_k, d_out + k * 8, p * 8)
+        ctx.d2h_strided(ih_kk, d_out + (G * p + k * p + k) * 8, p * p * 8)
+        ctx.d2h(conv, d_out + G * (p + p * p) * 8)
         ctx.sync()
         lfc = np.array(result["lfc"], copy=True)
-        se_s, conv_s = np.sqrt(np.abs(ih[:, coeff_idx, coeff_idx])), conv.copy()
+        se_s, conv_s = np.sqrt(np.abs(ih_kk)), conv.copy()
         if self._perm is None:
-            lfc[:, coeff_idx] = lfcs[:, coeff_idx]
+            lfc[:, coeff_idx] = lfc_k
             return ShrinkResult(lfc, se_s, conv_s, float(prior_scale), prior_var)
         se_o, conv_o = np.empty(G), np.empty(G)  # back to the caller's gene order
-        lfc[self._perm, coeff_idx] = lfcs[:, coeff_idx]
+        lfc[self._perm, coeff_idx] = lfc_k
         se_o[self._perm], conv_o[self._perm] = se_s, conv_s
         return ShrinkResult(lfc, se_o, conv_o, float(prior_scale), prior_var)
 

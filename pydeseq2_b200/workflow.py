@@ -295,14 +295,16 @@ def _adjust(base_mean, pv, independent_filter, alpha, comm=None, inference=None)
 
 def deseq2_results_resident(rf, contrast=None, refit_cooks=True, min_replicates=7, cooks_filter=True, independent_filter=True,
                             alpha=0.05, lfc_null=0.0, alt_hypothesis=None, fit_type="parametric", non_zero=None,
-                            adjust=True) -> Deseq2Results:
+                            adjust=True, shrink_coeff=None, shrink_adapt=True) -> Deseq2Results:
     """:func:`deseq2_results` on a :class:`pipeline.ResidentFit` whose counts are already in HBM (``rf.upload(counts)``, all-zero
     genes dropped by the caller): the hot path, Cook's distances and their per-gene decisions run in ONE resident pass; only
     per-gene vectors come back.  For the few genes whose outlier counts get replaced (dds.py:1301-1358) the mu / hat columns are
     gathered on the device, the replacement is decided on the host (R columns), and the refit (dds.py:1360-1458) runs resident
     again on the compact matrix.  Multiple testing is G-length host work as in :func:`deseq2_results`.  ``non_zero``: boolean mask of
     the uploaded genes within the caller's full gene list (all-zero genes are not fitted but take part in the independent
-    filtering with base mean 0, ds.py:486-528); the returned tables then have the full length."""
+    filtering with base mean 0, ds.py:486-528); the returned tables then have the full length.  ``shrink_coeff`` /
+    ``shrink_adapt``: apeGLM shrinkage of that coefficient on the resident counts (:meth:`pipeline.ResidentFit.lfc_shrink`), as in
+    :func:`deseq2_results`."""
     from scipy.stats import f as f_dist
 
     X, N, p, G = rf.X, rf.N, rf.p, rf.G
@@ -349,6 +351,12 @@ def deseq2_results_resident(rf, contrast=None, refit_cooks=True, min_replicates=
             _merge_refit(tables, refitted, new_zero, q)
     if cooks_filter:
         pv[outlier] = np.nan
+    scale = None
+    if shrink_coeff is not None:   # DeseqStats.lfc_shrink (ds.py:363-443): LFC column and SE replaced, p-values untouched
+        k = int(shrink_coeff)
+        scale = float(np.minimum(np.sqrt(fit_shrink_prior_var(lfc[:, k], se)), 1)) if shrink_adapt else 1.0
+        sh = rf.lfc_shrink({"lfc": lfc, "se": se, "dispersions": disp}, k, prior_scale=scale)
+        lfc, se = sh.lfc, sh.se
     nz = np.ones(G, bool)
     if non_zero is not None:
         nz = np.asarray(non_zero, dtype=bool)
@@ -365,8 +373,11 @@ def deseq2_results_resident(rf, contrast=None, refit_cooks=True, min_replicates=
         replaced, refitted, outlier = full(replaced, False), full(refitted, False), full(outlier, False)
     # adjust=False stops where deseq2() + run_wald_test() + the Cook's filter stop (no independent filtering / BH: `padj` is NaN)
     padj = _adjust(base_mean, pv, independent_filter, alpha, None, _context_inference(rf.ctx)) if adjust else np.full(len(pv), np.nan)
-    return Deseq2Results(base_mean, lfc @ contrast / LN2, se / LN2, stat, pv, padj, lfc, disp, genewise, fitted, sf, nz, replaced, refitted,
-                         outlier, None, None)
+    res = Deseq2Results(base_mean, lfc @ contrast / LN2, se / LN2, stat, pv, padj, lfc, disp, genewise, fitted, sf, nz, replaced, refitted,
+                        outlier, None, None)
+    if scale is not None:
+        res.log2_fold_change, res.shrink_prior_scale = lfc[:, int(shrink_coeff)] / LN2, scale
+    return res
 
 
 def _context_inference(ctx):
