@@ -35,13 +35,14 @@ typedef enum pdq_status {
     PDQ_OK = 0,
     PDQ_ERR_CUDA = -1,        /* a CUDA runtime call failed */
     PDQ_ERR_INVALID = -2,     /* bad argument (null pointer, N<=0, p<1, ld<G, ...) */
-    PDQ_ERR_UNSUPPORTED = -3, /* p > PDQ_MAX_P (PDQ_MAX_P_WIDE with pdq_set_wide_designs) */
+    PDQ_ERR_UNSUPPORTED = -3, /* p > PDQ_MAX_P (PDQ_MAX_P_WIDE with pdq_set_wide_designs, PDQ_MAX_P_LARGE with pdq_set_large_designs as well) */
     PDQ_ERR_NCCL = -4,        /* NCCL missing or a collective failed */
     PDQ_ERR_NO_DEVICE = -5    /* no CUDA device / not an sm_90 part */
 } pdq_status;
 
 #define PDQ_MAX_P 16 /* design columns supported (p <= 8: register-resident p x p solvers; 9..16: the same code with the small matrices in local memory) */
 #define PDQ_MAX_P_WIDE 64 /* design columns of a context with pdq_set_wide_designs(ctx, 1): 17..64 run on the wide-design kernels */
+#define PDQ_MAX_P_LARGE 128 /* design columns of a context with pdq_set_large_designs(ctx, 1) as well: 65..128 run on the large-design kernels */
 
 /* alt_hypothesis codes of Inference.wald_test (utils.py:778-806) */
 #define PDQ_ALT_NONE 0
@@ -82,9 +83,19 @@ int pdq_set_wide_designs(pdq_ctx* ctx, int on);
  * has pdq_set_wide_designs on: otherwise the design is refused with the message of pdq_set_wide_designs (p <= PDQ_MAX_P), also
  * for a pack made while wide designs were on.  Outputs are those of the narrow path; no gene is refitted on a grid. */
 int pdq_set_wide_shrink(pdq_ctx* ctx, int on);
+/* Designs of PDQ_MAX_P_WIDE + 1 .. PDQ_MAX_P_LARGE columns (paired designs of up to 127 subjects): off by default.  It takes
+ * effect only on a context that also has pdq_set_wide_designs on; otherwise p > PDQ_MAX_P is refused with the message of
+ * pdq_set_wide_designs (p <= PDQ_MAX_P), and with wide designs on but large designs off every code and message is that of the
+ * wide tier (p <= PDQ_MAX_P_WIDE), also for a pack made while large designs were on.  Such designs run on kernels in which a
+ * block of several warps owns one gene.  Above PDQ_MAX_P_LARGE: PDQ_ERR_UNSUPPORTED, and the message names PDQ_MAX_P_LARGE.
+ * apeGLM shrinkage of these designs is not implemented (PDQ_ERR_UNSUPPORTED, "not implemented"), with or without
+ * pdq_set_wide_shrink. */
+int pdq_set_large_designs(pdq_ctx* ctx, int on);
 /* Host only, no device needed: (X^T X)^+ (p x p row-major) and whether X (N x p, row-major, p <= PDQ_MAX_P_WIDE) has full column
  * rank, from the one-sided Jacobi SVD every design pack is built with (numpy.linalg.matrix_rank's tolerance). */
 int pdq_design_pinv(const double* X, int N, int p, double* pinv_out, int* full_rank_out);
+/* The same for p <= PDQ_MAX_P_LARGE (the linear algebra every pack of a large design is built with). */
+int pdq_design_pinv_large(const double* X, int N, int p, double* pinv_out, int* full_rank_out);
 /* Measured FP64 FMA throughput of the context's device in TFLOP/s (dependent-free DFMA chains on every SM, CUDA-event timed):
  * the arithmetic roofline bench.py reports next to the HBM one -- the per-gene kernels are FP64-pipe bound (DESIGN.md §5). */
 int pdq_fp64_peak_tflops(pdq_ctx* ctx, double* tflops_out);

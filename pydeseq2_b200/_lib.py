@@ -22,6 +22,7 @@ i64p = C.POINTER(C.c_int64)
 
 PDQ_MAX_P = 16
 PDQ_MAX_P_WIDE = 64  # with pdq_set_wide_designs (B200Inference(wide_designs=True))
+PDQ_MAX_P_LARGE = 128  # with pdq_set_large_designs as well (B200Inference(wide_designs=True, large_designs=True))
 ALT_CODES = {None: 0, "greaterAbs": 1, "lessAbs": 2, "greater": 3, "less": 4}
 UNIQUE_ID_BYTES = 128
 PEER_HANDLE_BYTES = 64
@@ -45,7 +46,9 @@ _SIGNATURES = {
     "pdq_set_debug_flags": (C.c_int, [c_ctx, C.c_int]),
     "pdq_set_wide_designs": (C.c_int, [c_ctx, C.c_int]),
     "pdq_set_wide_shrink": (C.c_int, [c_ctx, C.c_int]),
+    "pdq_set_large_designs": (C.c_int, [c_ctx, C.c_int]),
     "pdq_design_pinv": (C.c_int, [f64p, C.c_int, C.c_int, f64p, C.POINTER(C.c_int)]),
+    "pdq_design_pinv_large": (C.c_int, [f64p, C.c_int, C.c_int, f64p, C.POINTER(C.c_int)]),
     "pdq_launch_count": (C.c_int64, [c_ctx]),
     "pdq_buffer_epoch": (C.c_int64, [c_ctx]),
     "pdq_residency_stats": (C.c_int, [c_ctx, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
@@ -191,6 +194,7 @@ class Context:
         self.device = int(device)
         self.wide_designs = False  # pdq_set_wide_designs: designs of up to PDQ_MAX_P_WIDE columns
         self.wide_shrink = False   # pdq_set_wide_shrink: apeGLM shrinkage of those designs
+        self.large_designs = False  # pdq_set_large_designs: designs of up to PDQ_MAX_P_LARGE columns (with wide_designs)
         self._pin_pool = {}  # nbytes -> [addresses] of released page-locked blocks (cudaHostAlloc is expensive)
 
     def set_wide_designs(self, on: bool = True):
@@ -203,6 +207,12 @@ class Context:
         :meth:`set_wide_designs` as well, or such designs are refused as without it)."""
         self.check(self.lib.pdq_set_wide_shrink(self.h, 1 if on else 0))
         self.wide_shrink = bool(on)
+
+    def set_large_designs(self, on: bool = True):
+        """Accept designs of PDQ_MAX_P_WIDE + 1 .. PDQ_MAX_P_LARGE columns on this context (off by default; needs
+        :meth:`set_wide_designs` as well, or designs wider than PDQ_MAX_P are refused as without it)."""
+        self.check(self.lib.pdq_set_large_designs(self.h, 1 if on else 0))
+        self.large_designs = bool(on)
 
     def check(self, rc: int):
         if rc != 0:

@@ -11,8 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libpydeseq2_b200.so")
 # translation units: (source, object tag, extra defines).  pdq_kernels.cu is compiled once for p = 1..8 and once per wide design
-# width p = 9..16 (see the note at its top); pdq_wide.cu holds the kernels of designs of 17..64 columns, one build for every width
-# (p is a run-time argument there).  The units are independent and compile in parallel.
+# width p = 9..16 (see the note at its top); pdq_wide.cu holds the kernels of designs of 17..128 columns, one build for every width
+# (p is a run-time argument there; 65..128 columns are its team-per-gene instantiations).  The units are independent and compile in parallel.
 WIDE_P = tuple(range(9, 17))
 UNITS = [("pdq_api.cu", "pdq_api", ()), ("pdq_dispatch.cu", "pdq_dispatch", ()), ("pdq_io.cpp", "pdq_io", ()), ("pdq_padj.cu", "pdq_padj", ()), ("pdq_wide.cu", "pdq_wide", ()),
          ("pdq_kernels.cu", "pdq_kernels_p1to8", ())] + \

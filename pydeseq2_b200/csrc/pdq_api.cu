@@ -163,6 +163,7 @@ struct pdq_ctx {
     int debug = 0;           // PDQ_DEBUG_* test hooks
     int wide = 0;            // designs of up to PDQ_MAX_P_WIDE columns (pdq_set_wide_designs)
     int wide_shrink = 0;     // apeGLM shrinkage of those designs (pdq_set_wide_shrink)
+    int large = 0;           // designs of up to PDQ_MAX_P_LARGE columns, with `wide` on as well (pdq_set_large_designs)
     int64_t launches_at_capture = 0;
     int64_t buf_epoch = 0;   // bumped whenever ensure() re-allocates a context-owned buffer (captured graphs hold those pointers)
     NcclApi nccl;
@@ -375,8 +376,20 @@ extern "C" int pdq_set_wide_shrink(pdq_ctx* c, int on) {
     return PDQ_OK;
 }
 
+extern "C" int pdq_set_large_designs(pdq_ctx* c, int on) {
+    if (!c) return PDQ_ERR_INVALID;
+    c->large = on != 0;
+    return PDQ_OK;
+}
+
 extern "C" int pdq_design_pinv(const double* X, int N, int p, double* pinv_out, int* full_rank_out) {
     if (!X || !pinv_out || !full_rank_out || N <= 0 || p < 1 || p > PDQ_MAX_P_WIDE) return PDQ_ERR_INVALID;
+    design_linear_algebra(X, N, p, pinv_out, full_rank_out);
+    return PDQ_OK;
+}
+
+extern "C" int pdq_design_pinv_large(const double* X, int N, int p, double* pinv_out, int* full_rank_out) {
+    if (!X || !pinv_out || !full_rank_out || N <= 0 || p < 1 || p > PDQ_MAX_P_LARGE) return PDQ_ERR_INVALID;
     design_linear_algebra(X, N, p, pinv_out, full_rank_out);
     return PDQ_OK;
 }
@@ -500,11 +513,14 @@ extern "C" void pdq_graph_destroy(pdq_ctx* c, pdq_graph* g) {
 }
 
 // --------------------------------------------------------------------------------------------- design pack
-// the design widths the context accepts: PDQ_MAX_P, or PDQ_MAX_P_WIDE after pdq_set_wide_designs(ctx, 1)
+// the widest design the context accepts: PDQ_MAX_P, PDQ_MAX_P_WIDE after pdq_set_wide_designs(ctx, 1), PDQ_MAX_P_LARGE after
+// pdq_set_large_designs(ctx, 1) as well
+static int max_p(const pdq_ctx* c) { return !c->wide ? PDQ_MAX_P : (c->large ? PDQ_MAX_P_LARGE : PDQ_MAX_P_WIDE); }
+
 static int check_width(pdq_ctx* c, int p) {
     if (p > PDQ_MAX_P && !c->wide) return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
-    if (p > PDQ_MAX_P_WIDE)
-        return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; wide designs support p <= %d", p, PDQ_MAX_P_WIDE);
+    if (p > max_p(c))
+        return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; wide designs support p <= %d", p, max_p(c));
     return PDQ_OK;
 }
 
@@ -532,11 +548,15 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
     if (p <= PDQ_MAX_P) {
         memcpy(dd.pinv, pinv.data(), pinv.size() * 8);
     } else if (cudaMalloc((void**)&dd.pinv_dev, pinv.size() * 8) != cudaSuccess ||
-               cudaMemcpy(dd.pinv_dev, pinv.data(), pinv.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) {
+               cudaMemcpy(dd.pinv_dev, pinv.data(), pinv.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess ||
+               (p > PDQ_MAX_P_WIDE && cudaMalloc((void**)&dd.wald_dev, ((size_t)p * (p + 1) / 2 + 1 + p) * 8) != cudaSuccess)) {
         if (dd.pinv_dev) cudaFree(dd.pinv_dev);
+        if (dd.wald_dev) cudaFree(dd.wald_dev);
         delete d;
         return fail(c, PDQ_ERR_CUDA, "cudaMalloc/cudaMemcpy(pseudo-inverse) failed");
     }
+    if (p > PDQ_MAX_P_WIDE)
+        if (const char* e = getenv("PDQ_LARGE_WARPS")) dd.warps = atoi(e);  // tuning hook (A/B runs): 2, 4 or 8 warps per gene
     dd.few_rows = design_distinct_rows(X, N, p, 16) <= 16;
     if (const char* e = getenv("PDQ_IRLS_MEMO")) dd.few_rows = dd.few_rows && atoi(e) != 0;  // tuning hook (A/B runs)
     {
@@ -549,6 +569,7 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
             cudaMemcpy(dd.cell_plan, plan.data(), plan.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess) {
             if (dd.cell_plan) cudaFree(dd.cell_plan);
             if (dd.pinv_dev) cudaFree(dd.pinv_dev);
+            if (dd.wald_dev) cudaFree(dd.wald_dev);
             delete d;
             return fail(c, PDQ_ERR_CUDA, "cudaMalloc/cudaMemcpy(cell plan) failed");
         }
@@ -556,6 +577,7 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
     if (cudaMalloc((void**)&dd.pack, pack.size() * 8) != cudaSuccess) {
         cudaFree(dd.cell_plan);
         if (dd.pinv_dev) cudaFree(dd.pinv_dev);
+        if (dd.wald_dev) cudaFree(dd.wald_dev);
         delete d;
         return fail(c, PDQ_ERR_CUDA, "cudaMalloc(design pack) failed");
     }
@@ -564,6 +586,7 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
         cudaFree(dd.pack);
         cudaFree(dd.cell_plan);
         if (dd.pinv_dev) cudaFree(dd.pinv_dev);
+        if (dd.wald_dev) cudaFree(dd.wald_dev);
         delete d;
         return fail(c, PDQ_ERR_CUDA, "cudaMemcpy(design pack) failed");
     }
@@ -581,6 +604,7 @@ extern "C" void pdq_design_destroy(pdq_ctx* c, pdq_design* d) {
     if (d->d.pack) cudaFree(d->d.pack);
     if (d->d.cell_plan) cudaFree(d->d.cell_plan);
     if (d->d.pinv_dev) cudaFree(d->d.pinv_dev);
+    if (d->d.wald_dev) cudaFree(d->d.wald_dev);
     delete d;
 }
 
@@ -623,7 +647,7 @@ static int cached_design(pdq_ctx* c, const double* X, const double* sf, int N, i
 static int done(pdq_ctx* c, int rc, const char* what) {
     if (rc < 0) {
         if (rc == PDQ_ERR_UNSUPPORTED)
-            return fail(c, rc, "%s: unsupported design (p=%d..%d, shared-memory stage <= %zu bytes)", what, 1, c->wide ? PDQ_MAX_P_WIDE : PDQ_MAX_P,
+            return fail(c, rc, "%s: unsupported design (p=%d..%d, shared-memory stage <= %zu bytes)", what, 1, max_p(c),
                         kMaxDynSmem);
         return fail(c, rc, "%s: kernel launch failed: %s", what, cudaGetErrorString(cudaGetLastError()));
     }
@@ -778,6 +802,9 @@ extern "C" int pdq_lfc_shrink_dev(pdq_ctx* c, const pdq_design* d, const int64_t
             return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
         if (int e = check_width(c, d->d.p)) return e;  // a pack made before the wide-design opt-in was turned off
     }
+    if (d->d.p > PDQ_MAX_P_WIDE)  // reached with wide shrinkage on only (refused above otherwise)
+        return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented",
+                    PDQ_MAX_P_WIDE);
     return done(c, launch_lfc_shrink(cfg(c, G, d->d.N), d->d, counts, ld, G, size, prior_no_shrink_scale, prior_scale, shrink_index, lfcs,
                                      inv_hessians, conv, status), "lfc_shrink");
 }
@@ -1478,8 +1505,8 @@ extern "C" int pdq_wald_contrasts(pdq_ctx* c, const double* X, const double* sf,
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: bad arguments");
     if (p > PDQ_MAX_P && !c->wide)
         return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
-    if (p > PDQ_MAX_P_WIDE)
-        return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; wide designs support p <= %d", p, PDQ_MAX_P_WIDE);
+    if (p > max_p(c))
+        return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; wide designs support p <= %d", p, max_p(c));
     std::vector<double> tab((size_t)K * (p + 2));
     if (const int k = wald_contrast_table(K, p, contrasts, lfc_null, alt, tab.data()); k >= 0)
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: unknown alternative %d (contrast %d)", alt[k], k);
@@ -1611,6 +1638,9 @@ extern "C" int pdq_lfc_shrink_nbinom_glm(pdq_ctx* c, const double* X, const int6
     if (int e = cached_design(c, X, offset, N, p, &d, true)) return e;
     if (p > PDQ_MAX_P && !c->wide_shrink)
         return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
+    if (p > PDQ_MAX_P_WIDE)  // with or without wide shrinkage
+        return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented",
+                    PDQ_MAX_P_WIDE);
     void *dc, *dsize, *dbeta, *dih, *dconv, *status;
     res_begin(c);
     bool up_c;

@@ -13,6 +13,9 @@
 #ifndef PDQ_MAX_P_WIDE
 #define PDQ_MAX_P_WIDE 64
 #endif
+#ifndef PDQ_MAX_P_LARGE
+#define PDQ_MAX_P_LARGE 128
+#endif
 
 namespace pdq {
 
@@ -51,7 +54,7 @@ inline int wald_contrast_table(int K, int p, const double* contrasts, const doub
     return -1;
 }
 
-// One-sided Jacobi SVD of X (N x p, p <= PDQ_MAX_P_WIDE): the right singular vectors V and singular values give
+// One-sided Jacobi SVD of X (N x p, p <= PDQ_MAX_P_LARGE): the right singular vectors V and singular values give
 //   rank(X)   with numpy.linalg.matrix_rank's tolerance  s_max * max(N, p) * eps     (utils.py:349)
 //   (X^T X)^+ = V diag(1/s_i^2 for s_i > tol) V^T        (least-squares / minimum-norm projector)
 // number of distinct rows of X (capped at `cap + 1`): categorical designs have a handful, continuous covariates ~N

@@ -1,20 +1,29 @@
 // pdq_wide.cu -- per-gene kernels for designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns (opt-in per context:
-// pdq_set_wide_designs).
+// pdq_set_wide_designs; launchers `_wide`) and of PDQ_MAX_P_WIDE + 1 .. PDQ_MAX_P_LARGE columns (a second opt-in on top of it:
+// pdq_set_large_designs; launchers `_large`).
 //
 // The kernels of pdq_kernels.cu keep one gene's p x p state per LANE: in registers for p <= 8, in local memory for 9..16.  At
-// p = 64 one packed symmetric matrix is 16.6 KB, so that layout does not scale.  Here one WARP owns one gene (one warp per block,
-// one gene per block), and the gene's matrices live once, in the block's dynamic shared memory (DESIGN.md §3):
-//   * per-sample work is split over the lanes: chunks of 32 samples, lane l takes sample n0 + l and stages its weight (and working
-//     response) in shared memory;
-//   * the rank-32 update of a packed matrix from one chunk is split over its entries (lane l owns entries l, l + 32, ...); vectors
-//     such as X^T W z are split over their components;
-//   * the Cholesky factorisation, the triangular solves and the inverse are cooperative, one warp barrier per column step.
+// p = 64 one packed symmetric matrix is 16.6 KB, so that layout does not scale.  Here one TEAM of W warps owns one gene (one team
+// per block, one gene per block), and the gene's matrices live once, in the block's dynamic shared memory (DESIGN.md §3):
+//   * per-sample work is split over the team's threads: chunks of 32 W samples, thread t takes sample n0 + t and stages its
+//     weight (and working response) in shared memory;
+//   * the rank-(32 W) update of a packed matrix from one chunk is split over its entries (thread t owns entries t, t + 32 W, ...);
+//     vectors such as X^T W z are split over their components;
+//   * the Cholesky factorisation, the triangular solves and the inverse are cooperative, one team barrier per column step;
+//   * sums and votes are warp butterflies, combined across the warps through per-warp slots in shared memory.
+// The 17..64 tier runs W = 1 (a warp barrier is enough, and the Wald ridge and contrast travel as kernel parameters).  At p = 128
+// the workspace is ~204 KB, so one block fits per SM: the 65..128 tier runs W = 2, 4 or 8 warps per gene (large_warps) to keep the SM's FP64
+// pipes busy, and reads the Wald ridge and contrast from a device buffer next to the design pack (DesignDev::wald_dev; they
+// exceed the 32 KB kernel-parameter limit there).  Passes whose work does not grow with p (moments, mu from LFCs, Cook's
+// distances) run the W = 1 kernels at every width.
 // The design pack is read from global memory (it stays in L1 / L2).  The per-gene semantics are those of pdq_gene.cuh -- start
 // values, ridge, stopping rules, optimiser branch, dispersion search and grid, Wald alternatives, Cook's distances -- written
 // against libdevice's exp / log and the series of pdq_math.cuh instead of the table-driven cores; parity is to the reference's
 // tolerances, not bit for bit with the narrow kernels (which never run the same designs).
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "pdq_gene.cuh"
 #include "pdq_internal.h"
@@ -26,17 +35,46 @@ namespace {
 constexpr int kMaxTri = PDQ_MAX_P_WIDE * (PDQ_MAX_P_WIDE + 1) / 2;
 constexpr int kVecs = 8;  // vectors of p doubles in the workspace
 
+// the cooperative primitives of one gene's team of W warps (the whole block)
+template <int W>
+struct Team {
+    static constexpr int NT = 32 * W;  // threads, and samples per chunk
+    static __device__ __forceinline__ int tid() { return W == 1 ? (int)(threadIdx.x & 31) : (int)threadIdx.x; }
+    static __device__ __forceinline__ void sync() {
+        if constexpr (W == 1) __syncwarp();
+        else __syncthreads();
+    }
+    // total over the team, bit-identical in every thread
+    static __device__ __forceinline__ double sum(double v) {
+        for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if constexpr (W > 1) {
+            __shared__ double slot[W];
+            if ((threadIdx.x & 31) == 0) slot[threadIdx.x >> 5] = v;
+            __syncthreads();
+            v = slot[0];
+            for (int w = 1; w < W; ++w) v += slot[w];
+            __syncthreads();  // the slots are free again
+        }
+        return v;
+    }
+    static __device__ __forceinline__ bool any(bool b) {
+        if constexpr (W == 1) return __any_sync(0xffffffffu, b) != 0;
+        else return __syncthreads_or(b) != 0;
+    }
+};
+
 __host__ __device__ constexpr int tri_count(int p) { return (p * (p + 1) / 2 + 1) & ~1; }
-// workspace of one gene: three packed p x p matrices, kVecs vectors of p, two chunk buffers of 32
-__host__ __device__ constexpr size_t wide_ws_doubles(int p) { return 3 * (size_t)tri_count(p) + (size_t)kVecs * p + 64; }
+// workspace of one gene: three packed p x p matrices, kVecs vectors of p, two chunk buffers of 32 W
+__host__ __device__ constexpr size_t wide_ws_doubles(int p, int W = 1) { return 3 * (size_t)tri_count(p) + (size_t)kVecs * p + 64 * W; }
 
 struct Ws {
     double *A, *L, *Li;  // packed lower triangles
     double* v[kVecs];
-    double *cw, *cz;     // per-chunk staging, one slot per lane
+    double *cw, *cz;     // per-chunk staging, one slot per thread
     int p, np;
 };
 
+template <int W = 1>
 __device__ __forceinline__ Ws carve(double* s, int p) {
     Ws w;
     w.p = p;
@@ -47,16 +85,12 @@ __device__ __forceinline__ Ws carve(double* s, int p) {
     w.Li = s + 2 * t;
     for (int k = 0; k < kVecs; ++k) w.v[k] = s + 3 * t + k * p;
     w.cw = s + 3 * t + kVecs * p;
-    w.cz = w.cw + 32;
+    w.cz = w.cw + Team<W>::NT;
     return w;
 }
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
-__device__ __forceinline__ double wsum(double v) {
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-__device__ __forceinline__ bool wany(bool b) { return __any_sync(0xffffffffu, b) != 0; }
+__device__ __forceinline__ double wsum(double v) { return Team<1>::sum(v); }
 
 __device__ __forceinline__ DesignS design_of(const double* pack, int N, int p) {
     DesignS d;
@@ -69,29 +103,35 @@ __device__ __forceinline__ DesignS design_of(const double* pack, int N, int p) {
 }
 __device__ __forceinline__ const double* row_of(const DesignS& d, int n) { return d.X + (size_t)n * d.RS; }
 
+template <int W = 1>
 __device__ __forceinline__ void wfill(double* a, int n, double v) {
-    for (int k = lane_id(); k < n; k += 32) a[k] = v;
+    using T = Team<W>;
+    for (int k = T::tid(); k < n; k += T::NT) a[k] = v;
 }
+template <int W = 1>
 __device__ __forceinline__ void wcopy(double* dst, const double* src, int n) {
-    for (int k = lane_id(); k < n; k += 32) dst[k] = src[k];
+    using T = Team<W>;
+    for (int k = T::tid(); k < n; k += T::NT) dst[k] = src[k];
 }
 
 // S += sum_{s < cnt} w[s] x_{n0+s} x_{n0+s}^T over the packed lower triangle, entries k = lane, lane + 32, ...
+template <int W = 1>
 __device__ void rank_chunk(const DesignS& d, int p, int n0, int cnt, const double* w, double* S) {
+    using T = Team<W>;
     const int np = p * (p + 1) / 2;
-    int i = 0, j = lane_id();
+    int i = 0, j = T::tid();
     while (j > i) {
         j -= i + 1;
         ++i;
     }
-    for (int k = lane_id(); k < np; k += 32) {
+    for (int k = T::tid(); k < np; k += T::NT) {
         double acc = S[k];
         for (int s = 0; s < cnt; ++s) {
             const double* x = row_of(d, n0 + s);
             acc = fma(w[s] * x[i], x[j], acc);
         }
         S[k] = acc;
-        j += 32;
+        j += T::NT;
         while (j > i) {
             j -= i + 1;
             ++i;
@@ -100,8 +140,10 @@ __device__ void rank_chunk(const DesignS& d, int p, int n0, int cnt, const doubl
 }
 
 // v += sum_{s < cnt} z[s] x_{n0+s}, components split over the lanes
+template <int W = 1>
 __device__ void vec_chunk(const DesignS& d, int p, int n0, int cnt, const double* z, double* v) {
-    for (int j = lane_id(); j < p; j += 32) {
+    using T = Team<W>;
+    for (int j = T::tid(); j < p; j += T::NT) {
         double acc = v[j];
         for (int s = 0; s < cnt; ++s) acc = fma(z[s], row_of(d, n0 + s)[j], acc);
         v[j] = acc;
@@ -115,48 +157,54 @@ __device__ __forceinline__ double xdot(const double* x, const double* b, int p) 
 }
 
 // in-place L L^T = L (packed); a non-positive pivot gives NaN through sqrt, as chol<P>
+template <int W = 1>
 __device__ void chol_w(double* L, int p) {
-    const int lane = lane_id();
+    using T = Team<W>;
+    const int lane = T::tid();
     for (int j = 0; j < p; ++j) {
-        __syncwarp();
+        T::sync();
         const double dj = sqrt(L[tri(j, j)]);
         const double inv = 1.0 / dj;
-        __syncwarp();
-        for (int i = j + 1 + lane; i < p; i += 32) L[tri(i, j)] *= inv;
+        T::sync();
+        for (int i = j + 1 + lane; i < p; i += T::NT) L[tri(i, j)] *= inv;
         if (lane == 0) L[tri(j, j)] = dj;
-        __syncwarp();
-        for (int i = j + 1 + lane; i < p; i += 32) {
+        T::sync();
+        for (int i = j + 1 + lane; i < p; i += T::NT) {
             const double lij = L[tri(i, j)];
             for (int k = j + 1; k <= i; ++k) L[tri(i, k)] = fma(-lij, L[tri(k, j)], L[tri(i, k)]);
         }
     }
-    __syncwarp();
+    T::sync();
 }
 
 // solve (L L^T) x = v in place
+template <int W = 1>
 __device__ void chol_solve_w(const double* L, double* v, int p) {
-    const int lane = lane_id();
+    using T = Team<W>;
+    const int lane = T::tid();
     for (int i = 0; i < p; ++i) {
-        __syncwarp();
+        T::sync();
         const double xi = v[i] / L[tri(i, i)];
-        __syncwarp();
+        T::sync();
         if (lane == 0) v[i] = xi;
-        for (int r = i + 1 + lane; r < p; r += 32) v[r] = fma(-L[tri(r, i)], xi, v[r]);
+        for (int r = i + 1 + lane; r < p; r += T::NT) v[r] = fma(-L[tri(r, i)], xi, v[r]);
     }
     for (int i = p - 1; i >= 0; --i) {
-        __syncwarp();
+        T::sync();
         const double xi = v[i] / L[tri(i, i)];
-        __syncwarp();
+        T::sync();
         if (lane == 0) v[i] = xi;
-        for (int r = lane; r < i; r += 32) v[r] = fma(-L[tri(i, r)], xi, v[r]);
+        for (int r = lane; r < i; r += T::NT) v[r] = fma(-L[tri(i, r)], xi, v[r]);
     }
-    __syncwarp();
+    T::sync();
 }
 
 // H = (L L^T)^-1; Li = L^-1 (scratch).  H may be L itself: the second phase reads Li only
+template <int W = 1>
 __device__ void chol_inverse_w(const double* L, double* Li, double* H, int p) {
-    __syncwarp();
-    for (int j = lane_id(); j < p; j += 32) {
+    using T = Team<W>;
+    T::sync();
+    for (int j = T::tid(); j < p; j += T::NT) {
         Li[tri(j, j)] = 1.0 / L[tri(j, j)];
         for (int i = j + 1; i < p; ++i) {
             double s = 0.0;
@@ -164,14 +212,14 @@ __device__ void chol_inverse_w(const double* L, double* Li, double* H, int p) {
             Li[tri(i, j)] = s / L[tri(i, i)];
         }
     }
-    __syncwarp();
-    for (int i = lane_id(); i < p; i += 32)
+    T::sync();
+    for (int i = T::tid(); i < p; i += T::NT)
         for (int j = 0; j <= i; ++j) {
             double s = 0.0;
             for (int k = i; k < p; ++k) s = fma(Li[tri(k, i)], Li[tri(k, j)], s);
             H[tri(i, j)] = s;
         }
-    __syncwarp();
+    T::sync();
 }
 
 // x^T S x (one lane, x a design row)
@@ -186,55 +234,63 @@ __device__ __forceinline__ double quad_w(const double* S, const double* x, int p
 }
 
 // y = S x, rows split over the lanes
+template <int W = 1>
 __device__ void matvec_w(const double* S, const double* x, double* y, int p) {
-    __syncwarp();
-    for (int i = lane_id(); i < p; i += 32) {
+    using T = Team<W>;
+    T::sync();
+    for (int i = T::tid(); i < p; i += T::NT) {
         double r = 0.0;
         for (int j = 0; j < p; ++j) r = fma(S[j <= i ? tri(i, j) : tri(j, i)], x[j], r);
         y[i] = r;
     }
-    __syncwarp();
+    T::sync();
 }
 
 // sum_ij S_ij T_ij
-__device__ double symdot_w(const double* S, const double* T, int p) {
+template <int W = 1>
+__device__ double symdot_w(const double* S, const double* U, int p) {
+    using T = Team<W>;
     double dg = 0.0, o = 0.0;
-    int i = 0, j = lane_id();
+    int i = 0, j = T::tid();
     while (j > i) {
         j -= i + 1;
         ++i;
     }
-    for (int k = lane_id(); k < p * (p + 1) / 2; k += 32) {
-        if (i == j) dg = fma(S[k], T[k], dg);
-        else o = fma(S[k], T[k], o);
-        j += 32;
+    for (int k = T::tid(); k < p * (p + 1) / 2; k += T::NT) {
+        if (i == j) dg = fma(S[k], U[k], dg);
+        else o = fma(S[k], U[k], o);
+        j += T::NT;
         while (j > i) {
             j -= i + 1;
             ++i;
         }
     }
-    return fma(2.0, wsum(o), wsum(dg));
+    return fma(2.0, T::sum(o), T::sum(dg));
 }
 
 // L = S + diag(ridge) / + the packed lower triangle `ridge_tri`, then factor
+template <int W = 1>
 __device__ void factor_ridged(const double* S, double* L, int p, double ridge, const double* ridge_tri) {
-    __syncwarp();
-    for (int k = lane_id(); k < p * (p + 1) / 2; k += 32) L[k] = S[k] + (ridge_tri ? ridge_tri[k] : 0.0);
-    __syncwarp();
+    using T = Team<W>;
+    T::sync();
+    for (int k = T::tid(); k < p * (p + 1) / 2; k += T::NT) L[k] = S[k] + (ridge_tri ? ridge_tri[k] : 0.0);
+    T::sync();
     if (!ridge_tri)
-        for (int i = lane_id(); i < p; i += 32) L[tri(i, i)] += ridge;
-    chol_w(L, p);
+        for (int i = T::tid(); i < p; i += T::NT) L[tri(i, i)] += ridge;
+    chol_w<W>(L, p);
 }
 
 // beta = (X^T X)^+ v (rows of pinv split over the lanes)
+template <int W = 1>
 __device__ void apply_pinv(const double* pinv, const double* v, double* beta, int p) {
-    __syncwarp();
-    for (int i = lane_id(); i < p; i += 32) {
+    using T = Team<W>;
+    T::sync();
+    for (int i = T::tid(); i < p; i += T::NT) {
         double s = 0.0;
         for (int j = 0; j < p; ++j) s = fma(pinv[(size_t)i * p + j], v[j], s);
         beta[i] = s;
     }
-    __syncwarp();
+    T::sync();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -246,6 +302,18 @@ struct WideWald {
     double lfc_null;
     int alt;
 };
+// the same parameters of a 65..128-column design: ridge and contrast in device memory (DesignDev::wald_dev, wald_dev_layout)
+struct WaldRef {
+    const double* ridge;
+    const double* contrast;
+    double lfc_null;
+    int alt;
+};
+template <int W>
+using WaldOf = std::conditional_t<W == 1, WideWald, WaldRef>;
+// the packed ridge of the K-contrast test: a kernel parameter at W = 1, a device pointer above
+template <int W>
+using RidgeOf = std::conditional_t<W == 1, double[kMaxTri], const double*>;
 
 // statistic and p-value of alternative `alt` given SE (every lane, replicated; the same expressions as wald_contrast)
 __device__ void wald_alt(const double* c, const double* b, int p, double se, double t0, int alt, double& pv, double& stat) {
@@ -283,27 +351,32 @@ __device__ void wald_alt(const double* c, const double* b, int p, double se, dou
 }
 
 // H = (M + ridge)^-1 into ws.L (ws.Li scratch); M in `M`
+template <int W = 1>
 __device__ void wald_inverse_w(const double* M, const double* ridge_tri, Ws& ws) {
-    factor_ridged(M, ws.L, ws.p, 0.0, ridge_tri);
-    chol_inverse_w(ws.L, ws.Li, ws.L, ws.p);
+    factor_ridged<W>(M, ws.L, ws.p, 0.0, ridge_tri);
+    chol_inverse_w<W>(ws.L, ws.Li, ws.L, ws.p);
 }
 
 // SE of contrast c (shared memory or parameter space) against M and H = ws.L; ws.v[6], ws.v[7] scratch
+template <int W = 1>
 __device__ double wald_se_w(const double* M, const double* c, Ws& ws) {
-    matvec_w(ws.L, c, ws.v[6], ws.p);
-    matvec_w(M, ws.v[6], ws.v[7], ws.p);
+    using T = Team<W>;
+    matvec_w<W>(ws.L, c, ws.v[6], ws.p);
+    matvec_w<W>(M, ws.v[6], ws.v[7], ws.p);
     double q = 0.0;
-    for (int j = lane_id(); j < ws.p; j += 32) q = fma(ws.v[6][j], ws.v[7][j], q);
-    return sqrt(wsum(q));
+    for (int j = T::tid(); j < ws.p; j += T::NT) q = fma(ws.v[6][j], ws.v[7][j], q);
+    return sqrt(T::sum(q));
 }
 
-__device__ void wald_finish_w(const double* M, const WideWald& w, const double* beta, Ws& ws, double* p_out, double* stat_out,
+template <int W, class WP>
+__device__ void wald_finish_w(const double* M, const WP& w, const double* beta, Ws& ws, double* p_out, double* stat_out,
                               double* se_out) {
-    wald_inverse_w(M, w.ridge, ws);
-    const double se = wald_se_w(M, w.contrast, ws);
+    using T = Team<W>;
+    wald_inverse_w<W>(M, w.ridge, ws);
+    const double se = wald_se_w<W>(M, w.contrast, ws);
     double pv, stat;
     wald_alt(w.contrast, beta, ws.p, se, w.lfc_null, w.alt, pv, stat);
-    if (lane_id() == 0) {
+    if (T::tid() == 0) {
         *p_out = pv;
         *stat_out = stat;
         *se_out = se;
@@ -311,7 +384,7 @@ __device__ void wald_finish_w(const double* M, const WideWald& w, const double* 
 }
 
 // ---------------------------------------------------------------------------------------------
-// kernels: one warp per block, one gene per block
+// kernels: one team of W warps per block, one gene per block
 // ---------------------------------------------------------------------------------------------
 struct WideBase {
     const double* pack;  // design pack (global)
@@ -329,31 +402,34 @@ struct LinArgs {
 };
 
 // v = X^T t with t = y / sf per sample (the projection lin_reg_mu / fit_rough_dispersions start from); returns sum t
-template <class Y>
+template <int W, class Y>
 __device__ double project(const DesignS& d, int p, const Y& yy, Ws& ws, double* v) {
-    wfill(v, p, 0.0);
+    using T = Team<W>;
+    wfill<W>(v, p, 0.0);
     double s = 0.0;
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
         const double t = n < d.N ? yy.at(d, n) : 0.0;
         s += t;
-        __syncwarp();
-        ws.cz[lane_id()] = t;
-        __syncwarp();
-        vec_chunk(d, p, n0, min(32, d.N - n0), ws.cz, v);
+        T::sync();
+        ws.cz[T::tid()] = t;
+        T::sync();
+        vec_chunk<W>(d, p, n0, min(T::NT, d.N - n0), ws.cz, v);
     }
-    __syncwarp();
-    return wsum(s);
+    T::sync();
+    return T::sum(s);
 }
 
-__global__ void __launch_bounds__(32) k_wide_lin_reg_mu(const __grid_constant__ LinArgs a) {
+template <int W>
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_lin_reg_mu(const __grid_constant__ LinArgs a) {
+    using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
-    Ws ws = carve(wsm, a.b.p);
+    Ws ws = carve<W>(wsm, a.b.p);
     const int g = blockIdx.x, p = a.b.p;
     const DesignS d = design_of(a.b.pack, a.b.N, p);
-    project(d, p, NormedFromCounts{a.counts + g, a.ld}, ws, ws.v[0]);
-    apply_pinv(a.b.pinv, ws.v[0], ws.v[1], p);
-    for (int n = lane_id(); n < d.N; n += 32) {
+    project<W>(d, p, NormedFromCounts{a.counts + g, a.ld}, ws, ws.v[0]);
+    apply_pinv<W>(a.b.pinv, ws.v[0], ws.v[1], p);
+    for (int n = T::tid(); n < d.N; n += T::NT) {
         const double m = d.sf[n * d.RS] * xdot(row_of(d, n), ws.v[1], p);
         a.mu[(int64_t)n * a.ld_out + g] = (m < a.min_mu) ? a.min_mu : m;  // np.maximum (NaN propagates)
     }
@@ -371,14 +447,15 @@ struct MomArgsW {
 };
 
 // fit_rough_dispersions (rough_disp_gene); `fit` receives nothing, beta stays in ws.v[1]
-template <class Y>
+template <int W, class Y>
 __device__ double rough_w(const DesignS& d, const double* pinv, int p, const Y& yy, Ws& ws, double* mean, double* mu_out,
                           int64_t ld_mu, double min_mu) {
-    const double s = project(d, p, yy, ws, ws.v[0]);
-    apply_pinv(pinv, ws.v[0], ws.v[1], p);
+    using T = Team<W>;
+    const double s = project<W>(d, p, yy, ws, ws.v[0]);
+    apply_pinv<W>(pinv, ws.v[0], ws.v[1], p);
     const double m = s / (double)d.N;
     double acc = 0.0, ss = 0.0;
-    for (int n = lane_id(); n < d.N; n += 32) {
+    for (int n = T::tid(); n < d.N; n += T::NT) {
         const double fit = xdot(row_of(d, n), ws.v[1], p);
         const double t = yy.at(d, n);
         const double yh = (fit < 1.0) ? 1.0 : fit;  // np.maximum(y_hat, 1)
@@ -391,18 +468,20 @@ __device__ double rough_w(const DesignS& d, const double* pinv, int p, const Y& 
             mu_out[(int64_t)n * ld_mu] = (mu < min_mu) ? min_mu : mu;
         }
     }
-    acc = wsum(acc) / (double)(d.N - p);
-    if (mean) *mean = wsum(ss);  // sum of squared deviations from the mean (mom_from_counts)
+    acc = T::sum(acc) / (double)(d.N - p);
+    if (mean) *mean = T::sum(ss);  // sum of squared deviations from the mean (mom_from_counts)
     return (acc < 0.0) ? 0.0 : acc;  // np.maximum(alpha_rde, 0)
 }
 
-__global__ void __launch_bounds__(32) k_wide_rough(const __grid_constant__ MomArgsW a) {
+template <int W>
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_rough(const __grid_constant__ MomArgsW a) {
+    using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
-    Ws ws = carve(wsm, a.b.p);
+    Ws ws = carve<W>(wsm, a.b.p);
     const int g = blockIdx.x;
     const DesignS d = design_of(a.b.pack, a.b.N, a.b.p);
-    const double r = rough_w(d, a.b.pinv, a.b.p, NormedF64{a.normed + g, a.ld}, ws, nullptr, nullptr, 0, 0.0);
-    if (lane_id() == 0) a.alpha[g] = r;
+    const double r = rough_w<W>(d, a.b.pinv, a.b.p, NormedF64{a.normed + g, a.ld}, ws, nullptr, nullptr, 0, 0.0);
+    if (T::tid() == 0) a.alpha[g] = r;
 }
 
 __global__ void __launch_bounds__(32) k_wide_moments(const __grid_constant__ MomArgsW a) {
@@ -419,22 +498,24 @@ __global__ void __launch_bounds__(32) k_wide_moments(const __grid_constant__ Mom
 }
 
 // rough + moments, their min / clip, the normalised mean and (lin_reg_mu branch) mu_hat: mom_fused_gene
-__global__ void __launch_bounds__(32) k_wide_mom_from_counts(const __grid_constant__ MomArgsW a) {
+template <int W>
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_mom_from_counts(const __grid_constant__ MomArgsW a) {
+    using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
-    Ws ws = carve(wsm, a.b.p);
+    Ws ws = carve<W>(wsm, a.b.p);
     const int g = blockIdx.x;
     const DesignS d = design_of(a.b.pack, a.b.N, a.b.p);
     double ss;
     const NormedFromCounts yy{a.counts + g, a.ld};
     // the mean is needed inside the sweep: one projection pass for it first (rough_w recomputes the same sums)
-    const double m = project(d, a.b.p, yy, ws, ws.v[0]) / (double)d.N;
-    const double rough = rough_w(d, a.b.pinv, a.b.p, yy, ws, &ss, a.mu ? a.mu + g : nullptr, a.ld_mu, a.min_mu);
+    const double m = project<W>(d, a.b.p, yy, ws, ws.v[0]) / (double)d.N;
+    const double rough = rough_w<W>(d, a.b.pinv, a.b.p, yy, ws, &ss, a.mu ? a.mu + g : nullptr, a.ld_mu, a.min_mu);
     const double var = ss / (double)(d.N - 1);
     double mde = (var - a.s_mean_inv * m) / (m * m);
     if (!(mde == mde)) mde = 0.0;  // np.nan_to_num
     else if (mde > 1.7976931348623157e308) mde = 1.7976931348623157e308;
     else if (mde < -1.7976931348623157e308) mde = -1.7976931348623157e308;
-    if (lane_id() == 0) {
+    if (T::tid() == 0) {
         double al = (mde < rough) ? mde : rough;                                    // np.minimum (dds.py:1158)
         al = (al < a.min_disp) ? a.min_disp : ((al > a.max_disp) ? a.max_disp : al);  // np.clip (dds.py:1161)
         a.alpha[g] = al;
@@ -459,6 +540,7 @@ __global__ void __launch_bounds__(32) k_wide_mu_from_lfc(const __grid_constant__
 // ---------------------------------------------------------------------------------------------
 // irls (irls_gene + irls_optimizer_gene)
 // ---------------------------------------------------------------------------------------------
+template <int W>
 struct IrlsArgsW {
     WideBase b;
     IrlsParams prm;
@@ -471,18 +553,20 @@ struct IrlsArgsW {
     int* n_fallback;
     int force;
     int with_wald;
-    WideWald wald;
+    WaldOf<W> wald;
     double *wald_p, *wald_stat, *wald_se;
 };
 
 // start value (utils.py:349-357) into `beta`; also returns sum lgamma(y + 1) - lgamma(y + r) through lgsum when asked
+template <int W = 1>
 __device__ void irls_start(const DesignS& d, const double* pinv, int p, int full_rank, const int64_t* y, int64_t ld, double r,
                            Ws& ws, double* beta, double* lgsum) {
+    using T = Team<W>;
     double* v = ws.v[0];
-    wfill(v, p, 0.0);
+    wfill<W>(v, p, 0.0);
     double logmean = 0.0, lg = 0.0;
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
         double t = 0.0;
         if (n < d.N) {
             const double yv = (double)y[(int64_t)n * ld];
@@ -491,33 +575,35 @@ __device__ void irls_start(const DesignS& d, const double* pinv, int p, int full
             else logmean += log(q);
             if (lgsum) lg += lgamma_pos(yv + 1.0) - lgamma_pos(yv + r);
         }
-        __syncwarp();
-        ws.cz[lane_id()] = t;
-        __syncwarp();
-        if (full_rank) vec_chunk(d, p, n0, min(32, d.N - n0), ws.cz, v);
+        T::sync();
+        ws.cz[T::tid()] = t;
+        T::sync();
+        if (full_rank) vec_chunk<W>(d, p, n0, min(T::NT, d.N - n0), ws.cz, v);
     }
-    __syncwarp();
-    if (lgsum) *lgsum = wsum(lg);
+    T::sync();
+    if (lgsum) *lgsum = T::sum(lg);
     if (full_rank) {
-        apply_pinv(pinv, v, beta, p);
+        apply_pinv<W>(pinv, v, beta, p);
     } else {
-        logmean = wsum(logmean);
-        wfill(beta, p, 0.0);
-        __syncwarp();
-        if (lane_id() == 0) beta[0] = logmean / (double)d.N;
-        __syncwarp();
+        logmean = T::sum(logmean);
+        wfill<W>(beta, p, 0.0);
+        T::sync();
+        if (T::tid() == 0) beta[0] = logmean / (double)d.N;
+        T::sync();
     }
 }
 
 // one IRLS sweep at `beta`: A = X^T W X, b = X^T W z (W, z from the clamped mu); returns S = sum (y + r) log(r + mu) - y log(mu)
+template <int W = 1>
 __device__ double irls_sweep_w(const DesignS& d, int p, const int64_t* y, int64_t ld, const double* beta, double alpha, double r,
                                double min_mu, double log_min_mu, Ws& ws, double* A, double* b) {
-    wfill(A, p * (p + 1) / 2, 0.0);
-    wfill(b, p, 0.0);
+    using T = Team<W>;
+    wfill<W>(A, p * (p + 1) / 2, 0.0);
+    wfill<W>(b, p, 0.0);
     double S = 0.0;
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
-        double W = 0.0, Wz = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
+        double wt = 0.0, Wz = 0.0;
         if (n < d.N) {
             const double* x = row_of(d, n);
             const double yv = (double)y[(int64_t)n * ld];
@@ -528,28 +614,30 @@ __device__ double irls_sweep_w(const DesignS& d, int p, const int64_t* y, int64_
             const double mu = cl ? min_mu : mu_raw;
             const double lmu = cl ? log_min_mu : (eta + lsfn);
             const double iden = 1.0 / fma(mu, alpha, 1.0);
-            W = mu * iden;
-            Wz = fma(yv - mu, iden, W * (lmu - lsfn));
+            wt = mu * iden;
+            Wz = fma(yv - mu, iden, wt * (lmu - lsfn));
             S += fma(yv + r, log(r + mu), -yv * lmu);
         }
-        __syncwarp();
-        ws.cw[lane_id()] = W;
-        ws.cz[lane_id()] = Wz;
-        __syncwarp();
-        const int cnt = min(32, d.N - n0);
-        rank_chunk(d, p, n0, cnt, ws.cw, A);
-        vec_chunk(d, p, n0, cnt, ws.cz, b);
+        T::sync();
+        ws.cw[T::tid()] = wt;
+        ws.cz[T::tid()] = Wz;
+        T::sync();
+        const int cnt = min(T::NT, d.N - n0);
+        rank_chunk<W>(d, p, n0, cnt, ws.cw, A);
+        vec_chunk<W>(d, p, n0, cnt, ws.cz, b);
     }
-    __syncwarp();
-    return wsum(S);
+    T::sync();
+    return T::sum(S);
 }
 
 // mu (unclamped) and hat = W x^T H x with H = (A + ridge)^-1 (A: W from the clamped mu of `beta`); H ends in ws.L
+template <int W = 1>
 __device__ void irls_outputs(const DesignS& d, int p, const double* beta, double alpha, double min_mu, Ws& ws, const double* A,
                              double* mu_out, double* hat_out, int64_t ld_out) {
-    factor_ridged(A, ws.L, p, kRidge, nullptr);
-    chol_inverse_w(ws.L, ws.Li, ws.L, p);
-    for (int n = lane_id(); n < d.N; n += 32) {
+    using T = Team<W>;
+    factor_ridged<W>(A, ws.L, p, kRidge, nullptr);
+    chol_inverse_w<W>(ws.L, ws.Li, ws.L, p);
+    for (int n = T::tid(); n < d.N; n += T::NT) {
         const double* x = row_of(d, n);
         const double mu_raw = x[p] * exp(xdot(x, beta, p));
         const double mu = (mu_raw < min_mu) ? min_mu : mu_raw;
@@ -559,34 +647,38 @@ __device__ void irls_outputs(const DesignS& d, int p, const double* beta, double
 }
 
 // M = sum w x x^T with w = mu / (1 + mu alpha) of the UNCLAMPED (clamped = false) or clamped mu of `beta`
+template <int W = 1>
 __device__ void weight_matrix(const DesignS& d, int p, const double* beta, double alpha, double min_mu, bool clamp, Ws& ws,
                               double* M) {
-    wfill(M, p * (p + 1) / 2, 0.0);
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
-        double W = 0.0;
+    using T = Team<W>;
+    wfill<W>(M, p * (p + 1) / 2, 0.0);
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
+        double wt = 0.0;
         if (n < d.N) {
             const double* x = row_of(d, n);
             const double mu_raw = x[p] * exp(xdot(x, beta, p));
             const double mu = (clamp && mu_raw < min_mu) ? min_mu : mu_raw;
-            W = mu / fma(mu, alpha, 1.0);
+            wt = mu / fma(mu, alpha, 1.0);
         }
-        __syncwarp();
-        ws.cw[lane_id()] = W;
-        __syncwarp();
-        rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, M);
+        T::sync();
+        ws.cw[T::tid()] = wt;
+        T::sync();
+        rank_chunk<W>(d, p, n0, min(T::NT, d.N - n0), ws.cw, M);
     }
-    __syncwarp();
+    T::sync();
 }
 
 // f(beta) = nb_nll (mu-dependent part) + 0.5 ridge |beta|^2, its gradient g and Hessian H (irls_obj_sweep)
+template <int W = 1>
 __device__ double obj_sweep_w(const DesignS& d, int p, const int64_t* y, int64_t ld, const double* beta, double alpha, double r,
                               double min_mu, double log_min_mu, Ws& ws, double* g, double* H) {
-    wfill(H, p * (p + 1) / 2, 0.0);
-    wfill(g, p, 0.0);
+    using T = Team<W>;
+    wfill<W>(H, p * (p + 1) / 2, 0.0);
+    wfill<W>(g, p, 0.0);
     double f = 0.0;
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
         double gi = 0.0, hi = 0.0;
         if (n < d.N) {
             const double* x = row_of(d, n);
@@ -601,38 +693,40 @@ __device__ double obj_sweep_w(const DesignS& d, int p, const int64_t* y, int64_t
             gi = t - yv;
             hi = t * r / (r + mu);
         }
-        __syncwarp();
-        ws.cw[lane_id()] = hi;
-        ws.cz[lane_id()] = gi;
-        __syncwarp();
-        const int cnt = min(32, d.N - n0);
-        rank_chunk(d, p, n0, cnt, ws.cw, H);
-        vec_chunk(d, p, n0, cnt, ws.cz, g);
+        T::sync();
+        ws.cw[T::tid()] = hi;
+        ws.cz[T::tid()] = gi;
+        T::sync();
+        const int cnt = min(T::NT, d.N - n0);
+        rank_chunk<W>(d, p, n0, cnt, ws.cw, H);
+        vec_chunk<W>(d, p, n0, cnt, ws.cz, g);
     }
-    __syncwarp();
-    f = wsum(f);
+    T::sync();
+    f = T::sum(f);
     for (int j = 0; j < p; ++j) f = fma(0.5 * kRidge * beta[j], beta[j], f);
-    for (int j = lane_id(); j < p; j += 32) {
+    for (int j = T::tid(); j < p; j += T::NT) {
         g[j] = fma(kRidge, beta[j], g[j]);
         H[tri(j, j)] += kRidge;
     }
-    __syncwarp();
+    T::sync();
     return f;
 }
 
 __device__ __forceinline__ bool is_fixed(double b, double g, double lo, double hi) { return (b <= lo && g > 0.0) || (b >= hi && g < 0.0); }
 
 // the reference's L-BFGS-B branch (utils.py:374-413) as projected Newton: irls_optimizer_gene, every output written here
-__device__ void irls_optimizer_w(const IrlsArgsW& a, const DesignS& d, Ws& ws, int g) {
-    const int p = a.b.p, lane = lane_id();
+template <int W = 1>
+__device__ void irls_optimizer_w(const IrlsArgsW<W>& a, const DesignS& d, Ws& ws, int g) {
+    using T = Team<W>;
+    const int p = a.b.p, lane = T::tid();
     const IrlsParams& prm = a.prm;
     const int64_t* y = a.counts + g;
     const double alpha = a.disp[g], r = 1.0 / alpha, log_min_mu = log(prm.min_mu);
     double *beta = ws.v[1], *dir = ws.v[2], *gr = ws.v[3], *bt = ws.v[4], *gt = ws.v[5];
-    irls_start(d, a.b.pinv, p, prm.full_rank, y, a.ld, r, ws, beta, nullptr);
-    for (int j = lane; j < p; j += 32) beta[j] = fmin(fmax(beta[j], prm.min_beta), prm.max_beta);
-    __syncwarp();
-    double f = obj_sweep_w(d, p, y, a.ld, beta, alpha, r, prm.min_mu, log_min_mu, ws, gr, ws.A);
+    irls_start<W>(d, a.b.pinv, p, prm.full_rank, y, a.ld, r, ws, beta, nullptr);
+    for (int j = lane; j < p; j += T::NT) beta[j] = fmin(fmax(beta[j], prm.min_beta), prm.max_beta);
+    T::sync();
+    double f = obj_sweep_w<W>(d, p, y, a.ld, beta, alpha, r, prm.min_mu, log_min_mu, ws, gr, ws.A);
     bool ok = false;
     for (int it = 0; it < 100; ++it) {
         double pg = 0.0;
@@ -643,8 +737,8 @@ __device__ void irls_optimizer_w(const IrlsArgsW& a, const DesignS& d, Ws& ws, i
             break;
         }
         // Newton direction on the free set: fixed rows / columns of H replaced by the identity
-        __syncwarp();
-        for (int i = lane; i < p; i += 32) {
+        T::sync();
+        for (int i = lane; i < p; i += T::NT) {
             const bool fi = is_fixed(beta[i], gr[i], prm.min_beta, prm.max_beta);
             dir[i] = fi ? 0.0 : -gr[i];
             for (int j = 0; j <= i; ++j) {
@@ -652,25 +746,25 @@ __device__ void irls_optimizer_w(const IrlsArgsW& a, const DesignS& d, Ws& ws, i
                 ws.L[tri(i, j)] = (i == j) ? (fi ? 1.0 : ws.A[tri(i, i)]) : ((fi || fj) ? 0.0 : ws.A[tri(i, j)]);
             }
         }
-        chol_w(ws.L, p);
-        chol_solve_w(ws.L, dir, p);
+        chol_w<W>(ws.L, p);
+        chol_solve_w<W>(ws.L, dir, p);
         double slope = 0.0;
         for (int j = 0; j < p; ++j) slope = fma(gr[j], dir[j], slope);
         if (!(slope < 0.0)) {  // not a descent direction (indefinite / NaN): steepest descent on the free set
-            __syncwarp();
-            for (int j = lane; j < p; j += 32) dir[j] = is_fixed(beta[j], gr[j], prm.min_beta, prm.max_beta) ? 0.0 : -gr[j];
-            __syncwarp();
+            T::sync();
+            for (int j = lane; j < p; j += T::NT) dir[j] = is_fixed(beta[j], gr[j], prm.min_beta, prm.max_beta) ? 0.0 : -gr[j];
+            T::sync();
         }
         // backtracking line search with projection onto the box; the trial Hessian goes to ws.Li
         double step = 1.0, fn = f;
         bool accepted = false;
         for (int ls = 0; ls < 30; ++ls) {
-            __syncwarp();
-            for (int j = lane; j < p; j += 32) bt[j] = fmin(fmax(fma(step, dir[j], beta[j]), prm.min_beta), prm.max_beta);
-            __syncwarp();
+            T::sync();
+            for (int j = lane; j < p; j += T::NT) bt[j] = fmin(fmax(fma(step, dir[j], beta[j]), prm.min_beta), prm.max_beta);
+            T::sync();
             double dec = 0.0;
             for (int j = 0; j < p; ++j) dec = fma(gr[j], bt[j] - beta[j], dec);
-            const double ft = obj_sweep_w(d, p, y, a.ld, bt, alpha, r, prm.min_mu, log_min_mu, ws, gt, ws.Li);
+            const double ft = obj_sweep_w<W>(d, p, y, a.ld, bt, alpha, r, prm.min_mu, log_min_mu, ws, gt, ws.Li);
             if (ft <= f + 1e-4 * dec) {
                 accepted = true;
                 fn = ft;
@@ -684,10 +778,10 @@ __device__ void irls_optimizer_w(const IrlsArgsW& a, const DesignS& d, Ws& ws, i
         }
         const double df = f - fn;
         f = fn;
-        wcopy(ws.A, ws.Li, p * (p + 1) / 2);
-        wcopy(gr, gt, p);
-        wcopy(beta, bt, p);
-        __syncwarp();
+        wcopy<W>(ws.A, ws.Li, p * (p + 1) / 2);
+        wcopy<W>(gr, gt, p);
+        wcopy<W>(beta, bt, p);
+        T::sync();
         if (df <= 1e-15 * (1.0 + fabs(f))) {  // no further decrease possible in FP64
             ok = true;
             break;
@@ -696,32 +790,34 @@ __device__ void irls_optimizer_w(const IrlsArgsW& a, const DesignS& d, Ws& ws, i
     if (prm.fail_optimizer) ok = false;
     // (the two-column grid_fit_beta of utils.py:402-409 is never reached: p > 16 here)
     if (a.with_wald) {
-        weight_matrix(d, p, beta, alpha, prm.min_mu, false, ws, ws.A);
-        wald_finish_w(ws.A, a.wald, beta, ws, a.wald_p + g, a.wald_stat + g, a.wald_se + g);
+        weight_matrix<W>(d, p, beta, alpha, prm.min_mu, false, ws, ws.A);
+        wald_finish_w<W>(ws.A, a.wald, beta, ws, a.wald_p + g, a.wald_stat + g, a.wald_se + g);
     }
-    weight_matrix(d, p, beta, alpha, prm.min_mu, true, ws, ws.A);
-    irls_outputs(d, p, beta, alpha, prm.min_mu, ws, ws.A, a.mu + g, a.hat + g, a.ld_out);
-    for (int j = lane; j < p; j += 32) a.beta[(int64_t)g * p + j] = beta[j];
+    weight_matrix<W>(d, p, beta, alpha, prm.min_mu, true, ws, ws.A);
+    irls_outputs<W>(d, p, beta, alpha, prm.min_mu, ws, ws.A, a.mu + g, a.hat + g, a.ld_out);
+    for (int j = lane; j < p; j += T::NT) a.beta[(int64_t)g * p + j] = beta[j];
     if (lane == 0) a.conv[g] = ok ? 1.0 : 0.0;
 }
 
-__global__ void __maxnreg__(224) k_wide_irls(const __grid_constant__ IrlsArgsW a) {
+template <int W>
+__global__ void __maxnreg__(224) k_wide_irls(const __grid_constant__ IrlsArgsW<W> a) {
+    using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
-    Ws ws = carve(wsm, a.b.p);
-    const int g = blockIdx.x, p = a.b.p, lane = lane_id();
+    Ws ws = carve<W>(wsm, a.b.p);
+    const int g = blockIdx.x, p = a.b.p, lane = T::tid();
     const DesignS d = design_of(a.b.pack, a.b.N, p);
     const IrlsParams& prm = a.prm;
     const int64_t* y = a.counts + g;
     const double alpha = a.disp[g], r = 1.0 / alpha, Nd = (double)d.N, log_min_mu = log(prm.min_mu);
     double *b = ws.v[0], *beta = ws.v[1], *bh = ws.v[2];
     double lgsum;
-    irls_start(d, a.b.pinv, p, prm.full_rank, y, a.ld, r, ws, beta, &lgsum);
+    irls_start<W>(d, a.b.pinv, p, prm.full_rank, y, a.ld, r, ws, beta, &lgsum);
     const double C = Nd * r * log(alpha) + Nd * lgamma_pos(r) + lgsum;  // nb_nll = C + S(mu)
     double dev = 1000.0, ratio = 1.0;
     int it = 0, status = kIrlsOk;
     bool first = true;
     for (;;) {
-        const double S = irls_sweep_w(d, p, y, a.ld, beta, alpha, r, prm.min_mu, log_min_mu, ws, ws.A, b);
+        const double S = irls_sweep_w<W>(d, p, y, a.ld, beta, alpha, r, prm.min_mu, log_min_mu, ws, ws.A, b);
         if (!first) {
             const double old = dev;
             dev = -2.0 * (C + S);
@@ -729,18 +825,18 @@ __global__ void __maxnreg__(224) k_wide_irls(const __grid_constant__ IrlsArgsW a
         }
         first = false;
         if (!(ratio > prm.beta_tol)) break;  // `while dev_ratio > beta_tol` (NaN exits)
-        factor_ridged(ws.A, ws.L, p, kRidge, nullptr);
-        wcopy(bh, b, p);
-        chol_solve_w(ws.L, bh, p);
+        factor_ridged<W>(ws.A, ws.L, p, kRidge, nullptr);
+        wcopy<W>(bh, b, p);
+        chol_solve_w<W>(ws.L, bh, p);
         ++it;
         bool div = false;
-        for (int j = lane; j < p; j += 32) div = div || (fabs(bh[j]) > prm.max_beta);
-        if (wany(div) || it >= prm.maxiter) {
+        for (int j = lane; j < p; j += T::NT) div = div || (fabs(bh[j]) > prm.max_beta);
+        if (T::any(div) || it >= prm.maxiter) {
             status = kIrlsNeedsOptimizer;
             break;
         }
-        wcopy(beta, bh, p);
-        __syncwarp();
+        wcopy<W>(beta, bh, p);
+        T::sync();
     }
     if (a.force) status = kIrlsNeedsOptimizer;
     if (status != kIrlsOk) {
@@ -748,13 +844,13 @@ __global__ void __maxnreg__(224) k_wide_irls(const __grid_constant__ IrlsArgsW a
             a.status[g] = status;
             if (a.n_fallback) atomicAdd(a.n_fallback, 1);
         }
-        irls_optimizer_w(a, d, ws, g);
+        irls_optimizer_w<W>(a, d, ws, g);
         return;
     }
-    irls_outputs(d, p, beta, alpha, prm.min_mu, ws, ws.A, a.mu + g, a.hat + g, a.ld_out);
+    irls_outputs<W>(d, p, beta, alpha, prm.min_mu, ws, ws.A, a.mu + g, a.hat + g, a.ld_out);
     if (a.with_wald) {
         // run_wald_test uses the UNCLAMPED mu (ds.py:320-324): A + the correction of the samples on the min_mu clamp
-        for (int n0 = 0; n0 < d.N; n0 += 32) {
+        for (int n0 = 0; n0 < d.N; n0 += T::NT) {
             const int n = n0 + lane;
             double wd = 0.0;
             if (n < d.N) {
@@ -762,16 +858,16 @@ __global__ void __maxnreg__(224) k_wide_irls(const __grid_constant__ IrlsArgsW a
                 const double mu_raw = x[p] * exp(xdot(x, beta, p));
                 if (mu_raw < prm.min_mu) wd = mu_raw / fma(mu_raw, alpha, 1.0) - prm.min_mu / fma(prm.min_mu, alpha, 1.0);
             }
-            if (!wany(wd != 0.0)) continue;
-            __syncwarp();
+            if (!T::any(wd != 0.0)) continue;
+            T::sync();
             ws.cw[lane] = wd;
-            __syncwarp();
-            rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, ws.A);
+            T::sync();
+            rank_chunk<W>(d, p, n0, min(T::NT, d.N - n0), ws.cw, ws.A);
         }
-        __syncwarp();
-        wald_finish_w(ws.A, a.wald, beta, ws, a.wald_p + g, a.wald_stat + g, a.wald_se + g);
+        T::sync();
+        wald_finish_w<W>(ws.A, a.wald, beta, ws, a.wald_p + g, a.wald_stat + g, a.wald_se + g);
     }
-    for (int j = lane; j < p; j += 32) a.beta[(int64_t)g * p + j] = beta[j];
+    for (int j = lane; j < p; j += T::NT) a.beta[(int64_t)g * p + j] = beta[j];
     if (lane == 0) {
         a.conv[g] = 1.0;  // IRLS exits are "converged" (utils.py:365)
         a.status[g] = kIrlsOk;
@@ -798,167 +894,183 @@ struct AlphaArgsW {
 };
 
 // d loss / d log(alpha) at x (curv: also the NB part's curvature, see alpha_dloss)
+template <int W = 1>
 __device__ double dloss_w(const DesignS& d, int p, const AlphaParams& prm, const int64_t* y, int64_t ld, const double* mu,
                           int64_t ld_mu, double x, double xhat, double* curv, Ws& ws) {
+    using T = Team<W>;
     const double a = exp(x), r = 1.0 / a, Nd = (double)d.N;
     const bool cr = prm.cr_reg != 0;
     if (cr) {
-        wfill(ws.A, p * (p + 1) / 2, 0.0);
-        wfill(ws.Li, p * (p + 1) / 2, 0.0);
+        wfill<W>(ws.A, p * (p + 1) / 2, 0.0);
+        wfill<W>(ws.Li, p * (p + 1) / 2, 0.0);
     }
     double Sg = 0.0, S2 = 0.0;
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
-        double W = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
+        double wt = 0.0;
         if (n < d.N) {
             const double yv = (double)y[(int64_t)n * ld], m = mu[(int64_t)n * ld_mu];
             const double inv = 1.0 / (r + m);
             Sg += log(r + m) - digamma_pos(yv + r) + (yv - m) * inv;
             if (curv) S2 += fma(-(yv - m) * inv, inv, inv - trigamma_pos(yv + r));
-            W = m * r * inv;
+            wt = m * r * inv;
         }
         if (!cr) continue;
-        __syncwarp();
-        ws.cw[lane_id()] = W;
-        ws.cz[lane_id()] = W * W;
-        __syncwarp();
-        const int cnt = min(32, d.N - n0);
-        rank_chunk(d, p, n0, cnt, ws.cw, ws.A);
-        rank_chunk(d, p, n0, cnt, ws.cz, ws.Li);
+        T::sync();
+        ws.cw[T::tid()] = wt;
+        ws.cz[T::tid()] = wt * wt;
+        T::sync();
+        const int cnt = min(T::NT, d.N - n0);
+        rank_chunk<W>(d, p, n0, cnt, ws.cw, ws.A);
+        rank_chunk<W>(d, p, n0, cnt, ws.cz, ws.Li);
     }
-    __syncwarp();
-    Sg = wsum(Sg);
+    T::sync();
+    Sg = T::sum(Sg);
     const double F = Nd * (digamma_pos(r) + x) + Sg;
     double g = -r * F;
     if (curv) {
-        S2 = wsum(S2);
+        S2 = T::sum(S2);
         const double Fp = Nd * (trigamma_pos(r) - a) + S2;
         *curv = r * (F + r * Fp) + (prm.prior_reg ? 1.0 / prm.prior_var : 0.0);
     }
     if (cr) {
         // tr((X^T W X)^-1 X^T W^2 X): A is factored in ws.L and inverted back into ws.L; ws.Li holds X^T W^2 X, so A's own buffer
         // is the inverse's scratch
-        wcopy(ws.L, ws.A, p * (p + 1) / 2);
-        chol_w(ws.L, p);
-        chol_inverse_w(ws.L, ws.A, ws.L, p);
-        g -= 0.5 * a * symdot_w(ws.L, ws.Li, p);
+        wcopy<W>(ws.L, ws.A, p * (p + 1) / 2);
+        chol_w<W>(ws.L, p);
+        chol_inverse_w<W>(ws.L, ws.A, ws.L, p);
+        g -= 0.5 * a * symdot_w<W>(ws.L, ws.Li, p);
     }
     if (prm.prior_reg) g += (x - xhat) / prm.prior_var;
     return g;
 }
 
 // loss up to an alpha-independent constant, cr_reg on, no prior (the grid's objective, alpha_loss)
+template <int W = 1>
 __device__ double loss_w(const DesignS& d, int p, const int64_t* y, int64_t ld, const double* mu, int64_t ld_mu, double x, Ws& ws) {
+    using T = Team<W>;
     const double a = exp(x), r = 1.0 / a, Nd = (double)d.N;
-    wfill(ws.A, p * (p + 1) / 2, 0.0);
+    wfill<W>(ws.A, p * (p + 1) / 2, 0.0);
     double Sf = 0.0;
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
-        double W = 0.0;
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
+        double wt = 0.0;
         if (n < d.N) {
             const double yv = (double)y[(int64_t)n * ld], m = mu[(int64_t)n * ld_mu];
             const double rm = r + m;
             Sf += fma(yv + r, log(rm), -lgamma_pos(yv + r));
-            W = m * r / rm;
+            wt = m * r / rm;
         }
-        __syncwarp();
-        ws.cw[lane_id()] = W;
-        __syncwarp();
-        rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, ws.A);
+        T::sync();
+        ws.cw[T::tid()] = wt;
+        T::sync();
+        rank_chunk<W>(d, p, n0, min(T::NT, d.N - n0), ws.cw, ws.A);
     }
-    __syncwarp();
-    double f = Nd * (r * x + lgamma_pos(r)) + wsum(Sf);
-    chol_w(ws.A, p);
+    T::sync();
+    double f = Nd * (r * x + lgamma_pos(r)) + T::sum(Sf);
+    chol_w<W>(ws.A, p);
     double ld2 = 0.0;
     for (int i = 0; i < p; ++i) ld2 += log(ws.A[tri(i, i)]);
     return f + 0.5 * (2.0 * ld2);
 }
 
-__global__ void __launch_bounds__(32) k_wide_alpha_mle(const __grid_constant__ AlphaArgsW a) {
+template <int W>
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_alpha_mle(const __grid_constant__ AlphaArgsW a) {
+    using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
-    Ws ws = carve(wsm, a.b.p);
+    Ws ws = carve<W>(wsm, a.b.p);
     const int g = blockIdx.x, p = a.b.p;
     const DesignS d = design_of(a.b.pack, a.b.N, p);
     AlphaParams prm = a.prm;
     if (a.prior_var_dev) prm.prior_var = *a.prior_var_dev;
     const int64_t* y = a.counts + g;
     const double* mu = a.mu + g;
-    const Group grp{lane_id(), 32, 1};
+    // alpha_search / alpha_grid_search vote through Group::any (a single-warp __any_sync) and write through grp.si == 0 (thread
+    // 0 of the block).  At W > 1 that is right only because every value dloss_w / loss_w return is a Team<W>::sum, bit-identical
+    // in every thread of the block, so every warp takes the same branches and reaches the __syncthreads inside T::sum together.
+    // A change that lets a per-thread value reach the search's control flow breaks that uniformity.
+    const Group grp{T::tid(), T::NT, 1};
     alpha_search(grp, prm, a.alpha_hat[g],
-                 [&](double x, double xhat, double* curv) { return dloss_w(d, p, prm, y, a.ld, mu, a.ld_mu, x, xhat, curv, ws); },
+                 [&](double x, double xhat, double* curv) { return dloss_w<W>(d, p, prm, y, a.ld, mu, a.ld_mu, x, xhat, curv, ws); },
                  a.alpha + g, a.conv + g, a.status + g, true, a.hint_in ? a.hint_in + 2 * (int64_t)g : nullptr,
                  a.hint_out ? a.hint_out + 2 * (int64_t)g : nullptr);
-    __syncwarp();
-    if (a.force && lane_id() == 0) {
+    T::sync();
+    if (a.force && T::tid() == 0) {
         a.status[g] = kAlphaNeedsGrid;
         a.conv[g] = 0.0;
     }
-    __syncwarp();
+    T::sync();
     if (a.status[g] == kAlphaNeedsGrid)
-        alpha_grid_search(grp, prm.lo, prm.hi, [&](double x) { return loss_w(d, p, y, a.ld, mu, a.ld_mu, x, ws); }, a.alpha + g, true);
+        alpha_grid_search(grp, prm.lo, prm.hi, [&](double x) { return loss_w<W>(d, p, y, a.ld, mu, a.ld_mu, x, ws); }, a.alpha + g, true);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Wald tests
 // ---------------------------------------------------------------------------------------------
+template <int W>
 struct WaldArgsW {
     WideBase b;
-    WideWald w;
+    WaldOf<W> w;
     const double *disp, *lfc, *mu;
     int64_t ld_mu;
     double *pv, *stat, *se;
 };
 
-__global__ void __launch_bounds__(32) k_wide_wald(const __grid_constant__ WaldArgsW a) {
+template <int W>
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_wald(const __grid_constant__ WaldArgsW<W> a) {
+    using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
-    Ws ws = carve(wsm, a.b.p);
+    Ws ws = carve<W>(wsm, a.b.p);
     const int g = blockIdx.x, p = a.b.p;
     const DesignS d = design_of(a.b.pack, a.b.N, p);
     const double disp = a.disp[g];
-    wfill(ws.A, p * (p + 1) / 2, 0.0);
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
-        double W = 0.0;
+    wfill<W>(ws.A, p * (p + 1) / 2, 0.0);
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
+        double wt = 0.0;
         if (n < d.N) {
             const double m = a.mu[(int64_t)n * a.ld_mu + g];
-            W = m / fma(m, disp, 1.0);
+            wt = m / fma(m, disp, 1.0);
         }
-        __syncwarp();
-        ws.cw[lane_id()] = W;
-        __syncwarp();
-        rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, ws.A);
+        T::sync();
+        ws.cw[T::tid()] = wt;
+        T::sync();
+        rank_chunk<W>(d, p, n0, min(T::NT, d.N - n0), ws.cw, ws.A);
     }
-    __syncwarp();
-    wcopy(ws.v[1], a.lfc + (int64_t)g * p, p);
-    __syncwarp();
-    wald_finish_w(ws.A, a.w, ws.v[1], ws, a.pv + g, a.stat + g, a.se + g);
+    T::sync();
+    wcopy<W>(ws.v[1], a.lfc + (int64_t)g * p, p);
+    T::sync();
+    wald_finish_w<W>(ws.A, a.w, ws.v[1], ws, a.pv + g, a.stat + g, a.se + g);
 }
 
+template <int W>
 struct WaldKArgsW {
     WideBase b;
-    double ridge[kMaxTri];
+    RidgeOf<W> ridge;
     const double *disp, *lfc, *tab;  // tab (K, p + 2): contrast | lfc_null | alt
     int K;
     double *pv, *stat, *se;
     int64_t ld_out;
 };
 
-__global__ void __launch_bounds__(32) k_wide_wald_contrasts(const __grid_constant__ WaldKArgsW a) {
+template <int W>
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_wald_contrasts(const __grid_constant__ WaldKArgsW<W> a) {
+    using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
-    Ws ws = carve(wsm, a.b.p);
+    Ws ws = carve<W>(wsm, a.b.p);
     const int g = blockIdx.x, p = a.b.p;
     const DesignS d = design_of(a.b.pack, a.b.N, p);
     double* beta = ws.v[1];
-    wcopy(beta, a.lfc + (int64_t)g * p, p);
-    __syncwarp();
-    weight_matrix(d, p, beta, a.disp[g], 0.0, false, ws, ws.A);  // mu = sf exp(x'beta), as k_mu_from_lfc writes it
-    wald_inverse_w(ws.A, a.ridge, ws);
+    wcopy<W>(beta, a.lfc + (int64_t)g * p, p);
+    T::sync();
+    weight_matrix<W>(d, p, beta, a.disp[g], 0.0, false, ws, ws.A);  // mu = sf exp(x'beta), as k_mu_from_lfc writes it
+    wald_inverse_w<W>(ws.A, a.ridge, ws);
     for (int k = 0; k < a.K; ++k) {
         const double* row = a.tab + (int64_t)k * (p + 2);
-        const double se = wald_se_w(ws.A, row, ws);
+        const double se = wald_se_w<W>(ws.A, row, ws);
         double pv, stat;
         wald_alt(row, beta, p, se, row[p], (int)row[p + 1], pv, stat);
-        if (lane_id() == 0) {
+        if (T::tid() == 0) {
             a.pv[(int64_t)k * a.ld_out + g] = pv;
             a.stat[(int64_t)k * a.ld_out + g] = stat;
             a.se[(int64_t)k * a.ld_out + g] = se;
@@ -1322,7 +1434,7 @@ int prep(K kernel, size_t smem) {
 }
 
 inline int check_launch() { return cudaGetLastError() == cudaSuccess ? 0 : PDQ_ERR_CUDA; }
-inline size_t ws_bytes(int p) { return wide_ws_doubles(p) * sizeof(double); }
+inline size_t ws_bytes(int p, int W = 1) { return wide_ws_doubles(p, W) * sizeof(double); }
 inline WideBase base_of(const DesignDev& d, int G) { return WideBase{d.pack, d.pinv_dev, d.N, d.p, G}; }
 
 void pack_lower(const double* full, int p, double* tri_out) {
@@ -1337,21 +1449,81 @@ void wide_wald(const WaldHost& h, int p, WideWald& w) {
     w.alt = h.alt;
 }
 
-}  // namespace
+// host values -> device memory as kernel parameters, in chunks that fit the parameter space: stream-ordered behind the kernels
+// that read the previous values, and a captured graph keeps the values of its capture
+constexpr int kPutChunk = 3968;
+struct PutArgs {
+    double v[kPutChunk];
+    double* dst;
+    int n;
+};
+__global__ void __launch_bounds__(256) k_large_put(const __grid_constant__ PutArgs a) {
+    for (int i = threadIdx.x; i < a.n; i += blockDim.x) a.dst[i] = a.v[i];
+}
 
-int launch_lin_reg_mu_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
-                           int64_t ld_out) {
+// uploads `n` doubles; returns the number of launches or a negative pdq_status
+int put_dev(const LaunchCfg& c, const double* h, int n, double* dst) {
+    int launches = 0;
+    for (int o = 0; o < n; o += kPutChunk) {
+        PutArgs a;
+        a.n = (n - o < kPutChunk) ? n - o : kPutChunk;
+        a.dst = dst + o;
+        for (int i = 0; i < a.n; ++i) a.v[i] = h[o + i];
+        k_large_put<<<1, 256, 0, c.stream>>>(a);
+        if (int e = check_launch()) return e;
+        ++launches;
+    }
+    return launches;
+}
+
+// ridge (packed lower triangle) and contrast of a 65..128-column design into DesignDev::wald_dev; contrast may be null
+int put_wald(const LaunchCfg& c, const DesignDev& d, const double* ridge, const double* contrast, WaldRef& w) {
+    const int p = d.p, t = tri_count(p);
+    double buf[PDQ_MAX_P_LARGE * (PDQ_MAX_P_LARGE + 1) / 2 + 1 + PDQ_MAX_P_LARGE];
+    pack_lower(ridge, p, buf);
+    if (t > p * (p + 1) / 2) buf[t - 1] = 0.0;  // the pad slot of an odd p(p+1)/2: never read, uploaded as zero
+    if (contrast)
+        for (int j = 0; j < p; ++j) buf[t + j] = contrast[j];
+    w.ridge = d.wald_dev;
+    w.contrast = d.wald_dev + t;
+    return put_dev(c, buf, contrast ? t + p : t, d.wald_dev);
+}
+
+// warps per gene of the 65..128 tier: the fewest of 2, 4, 8 that keep 8 warps on an SM, given how many blocks the workspace lets
+// share one (228 KB of shared memory per SM, 1 KB of it reserved per block).  That is 2 at p = 65 (four blocks), 4 at p = 81 (two)
+// and 8 from p = 101 on (one): the fastest of the three at each of those widths (DESIGN.md §5)
+int large_warps(int p) {
+    for (int W = 2; W < 8; W *= 2)
+        if ((int)(228 * 1024 / (ws_bytes(p, W) + 1024)) * W >= 8) return W;
+    return 8;
+}
+
+// the 65..128 tier's team width: DesignDev::warps (a tuning hook) or large_warps
+template <class F>
+int with_warps(const DesignDev& d, F&& f) {
+    switch (d.warps ? d.warps : large_warps(d.p)) {
+        case 2: return f(std::integral_constant<int, 2>{});
+        case 4: return f(std::integral_constant<int, 4>{});
+        default: return f(std::integral_constant<int, 8>{});
+    }
+}
+
+template <int W>
+int lin_reg_mu_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
+                 int64_t ld_out) {
     const LinArgs a{base_of(d, G), counts, ld, min_mu, mu_out, ld_out};
-    if (int e = prep(k_wide_lin_reg_mu, ws_bytes(d.p))) return e;
-    k_wide_lin_reg_mu<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = prep(k_wide_lin_reg_mu<W>, ws_bytes(d.p, W))) return e;
+    k_wide_lin_reg_mu<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
     if (int e = check_launch()) return e;
     return 1;
 }
 
-int launch_irls_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
-                     double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
+template <int W>
+int irls_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
+           double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
     if (n_fallback && cudaMemsetAsync(n_fallback, 0, sizeof(int), c.stream) != cudaSuccess) return PDQ_ERR_CUDA;
-    IrlsArgsW a{};
+    int puts = 0;
+    IrlsArgsW<W> a{};
     a.b = base_of(d, G);
     a.prm = IrlsParams{h.min_mu, h.beta_tol, h.min_beta, h.max_beta, h.maxiter, d.full_rank, d.few_rows,
                        (c.debug & PDQ_DEBUG_FAIL_IRLS_OPTIMIZER) ? 1 : 0};
@@ -1361,58 +1533,125 @@ int launch_irls_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* coun
     a.force = (c.debug & PDQ_DEBUG_FORCE_IRLS_OPTIMIZER) ? 1 : 0;
     a.with_wald = w ? 1 : 0;
     if (w) {
-        wide_wald(*w, d.p, a.wald);
+        if constexpr (W == 1) {
+            wide_wald(*w, d.p, a.wald);
+        } else {
+            if ((puts = put_wald(c, d, w->ridge, w->contrast, a.wald)) < 0) return puts;
+            a.wald.lfc_null = w->lfc_null;
+            a.wald.alt = w->alt;
+        }
         a.wald_p = w->pv; a.wald_stat = w->stat; a.wald_se = w->se;
     }
-    if (int e = prep(k_wide_irls, ws_bytes(d.p))) return e;
-    k_wide_irls<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
+    if (int e = prep(k_wide_irls<W>, ws_bytes(d.p, W))) return e;
+    k_wide_irls<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1 + puts;
+}
+
+template <int W>
+int alpha_mle_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
+                const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
+                int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
+    const AlphaArgsW a{base_of(d, G), AlphaParams{log(min_disp), log(max_disp), prior_var, cr_reg, prior_reg}, counts, ld, mu, ld_mu,
+                       alpha_hat, alpha, conv, status, prior_var_dev, (c.debug & PDQ_DEBUG_FORCE_ALPHA_GRID) ? 1 : 0, hint_in, hint_out};
+    if (int e = prep(k_wide_alpha_mle<W>, ws_bytes(d.p, W))) return e;
+    k_wide_alpha_mle<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
     if (int e = check_launch()) return e;
     return 1;
+}
+
+template <int W>
+int wald_t(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu, int64_t ld_mu, int G,
+           const double* ridge, const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
+    int puts = 0;
+    WaldArgsW<W> a{};
+    a.b = base_of(d, G);
+    if constexpr (W == 1) {
+        wide_wald(WaldHost{ridge, contrast, lfc_null, alt, pv, stat, se}, d.p, a.w);
+    } else {
+        if ((puts = put_wald(c, d, ridge, contrast, a.w)) < 0) return puts;
+        a.w.lfc_null = lfc_null;
+        a.w.alt = alt;
+    }
+    a.disp = disp; a.lfc = lfc; a.mu = mu; a.ld_mu = ld_mu;
+    a.pv = pv; a.stat = stat; a.se = se;
+    if (int e = prep(k_wide_wald<W>, ws_bytes(d.p, W))) return e;
+    k_wide_wald<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1 + puts;
+}
+
+template <int W>
+int wald_contrasts_t(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
+                     const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
+    int puts = 0;
+    WaldKArgsW<W> a{};
+    a.b = base_of(d, G);
+    if constexpr (W == 1) {
+        pack_lower(ridge, d.p, a.ridge);
+    } else {
+        WaldRef w;
+        if ((puts = put_wald(c, d, ridge, nullptr, w)) < 0) return puts;
+        a.ridge = w.ridge;
+    }
+    a.disp = disp; a.lfc = lfc; a.tab = tab; a.K = K;
+    a.pv = pv; a.stat = stat; a.se = se; a.ld_out = ld_out;
+    if (int e = prep(k_wide_wald_contrasts<W>, ws_bytes(d.p, W))) return e;
+    k_wide_wald_contrasts<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1 + puts;
+}
+
+template <int W>
+int rough_t(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {
+    const MomArgsW a{base_of(d, G), normed, nullptr, ld, d.s_mean_inv, 0.0, 0.0, 0.0, alpha, nullptr, nullptr, 0};
+    if (int e = prep(k_wide_rough<W>, ws_bytes(d.p, W))) return e;
+    k_wide_rough<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+template <int W>
+int mom_from_counts_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp, double max_disp,
+                      double* alpha, double* normed_mean, double min_mu, double* mu_hat, int64_t ld_mu) {
+    const MomArgsW a{base_of(d, G), nullptr, counts, ld, d.s_mean_inv, min_disp, max_disp, min_mu, alpha, normed_mean, mu_hat, ld_mu};
+    if (int e = prep(k_wide_mom_from_counts<W>, ws_bytes(d.p, W))) return e;
+    k_wide_mom_from_counts<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+}  // namespace
+
+int launch_lin_reg_mu_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
+                           int64_t ld_out) {
+    return lin_reg_mu_t<1>(c, d, counts, ld, G, min_mu, mu_out, ld_out);
+}
+
+int launch_irls_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
+                     double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
+    return irls_t<1>(c, d, counts, ld, G, disp, h, beta, mu, hat, ld_out, conv, status, n_fallback, w);
 }
 
 int launch_alpha_mle_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
                           const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
                           int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
-    const AlphaArgsW a{base_of(d, G), AlphaParams{log(min_disp), log(max_disp), prior_var, cr_reg, prior_reg}, counts, ld, mu, ld_mu,
-                       alpha_hat, alpha, conv, status, prior_var_dev, (c.debug & PDQ_DEBUG_FORCE_ALPHA_GRID) ? 1 : 0, hint_in, hint_out};
-    if (int e = prep(k_wide_alpha_mle, ws_bytes(d.p))) return e;
-    k_wide_alpha_mle<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
+    return alpha_mle_t<1>(c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_var, prior_var_dev, cr_reg, prior_reg, alpha,
+                          conv, status, hint_in, hint_out);
 }
 
 int launch_wald_wide(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu, int64_t ld_mu, int G,
                      const double* ridge, const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
-    WaldArgsW a{};
-    a.b = base_of(d, G);
-    wide_wald(WaldHost{ridge, contrast, lfc_null, alt, pv, stat, se}, d.p, a.w);
-    a.disp = disp; a.lfc = lfc; a.mu = mu; a.ld_mu = ld_mu;
-    a.pv = pv; a.stat = stat; a.se = se;
-    if (int e = prep(k_wide_wald, ws_bytes(d.p))) return e;
-    k_wide_wald<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
+    return wald_t<1>(c, d, disp, lfc, mu, ld_mu, G, ridge, contrast, lfc_null, alt, pv, stat, se);
 }
 
 int launch_wald_contrasts_wide(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
                                const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
-    WaldKArgsW a{};
-    a.b = base_of(d, G);
-    pack_lower(ridge, d.p, a.ridge);
-    a.disp = disp; a.lfc = lfc; a.tab = tab; a.K = K;
-    a.pv = pv; a.stat = stat; a.se = se; a.ld_out = ld_out;
-    if (int e = prep(k_wide_wald_contrasts, ws_bytes(d.p))) return e;
-    k_wide_wald_contrasts<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
+    return wald_contrasts_t<1>(c, d, disp, lfc, G, ridge, K, tab, pv, stat, se, ld_out);
 }
 
 int launch_rough_wide(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {
-    const MomArgsW a{base_of(d, G), normed, nullptr, ld, d.s_mean_inv, 0.0, 0.0, 0.0, alpha, nullptr, nullptr, 0};
-    if (int e = prep(k_wide_rough, ws_bytes(d.p))) return e;
-    k_wide_rough<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
+    return rough_t<1>(c, d, normed, ld, G, alpha);
 }
 
 int launch_moments_wide(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha, double* all_zero) {
@@ -1424,11 +1663,7 @@ int launch_moments_wide(const LaunchCfg& c, const DesignDev& d, const double* no
 
 int launch_mom_from_counts_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp,
                                 double max_disp, double* alpha, double* normed_mean, double min_mu, double* mu_hat, int64_t ld_mu) {
-    const MomArgsW a{base_of(d, G), nullptr, counts, ld, d.s_mean_inv, min_disp, max_disp, min_mu, alpha, normed_mean, mu_hat, ld_mu};
-    if (int e = prep(k_wide_mom_from_counts, ws_bytes(d.p))) return e;
-    k_wide_mom_from_counts<<<G, 32, ws_bytes(d.p), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
+    return mom_from_counts_t<1>(c, d, counts, ld, G, min_disp, max_disp, alpha, normed_mean, min_mu, mu_hat, ld_mu);
 }
 
 int launch_mu_from_lfc_wide(const LaunchCfg& c, const DesignDev& d, const double* lfc, int G, double* mu, int64_t ld_out) {
@@ -1447,6 +1682,69 @@ int launch_cooks_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* cou
     k_wide_cooks<<<G, 32, smem, c.stream>>>(a);
     if (int e = check_launch()) return e;
     return 1;
+}
+
+// ---- 65..128 columns: the same kernels with a team of W warps per gene; the passes whose work does not grow with p (moments,
+// mu from LFCs, Cook's distances) are the one-warp kernels above
+int launch_lin_reg_mu_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
+                            int64_t ld_out) {
+    return with_warps(d, [&](auto w) { return lin_reg_mu_t<decltype(w)::value>(c, d, counts, ld, G, min_mu, mu_out, ld_out); });
+}
+
+int launch_irls_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
+                      double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
+    return with_warps(d, [&](auto tw) {
+        return irls_t<decltype(tw)::value>(c, d, counts, ld, G, disp, h, beta, mu, hat, ld_out, conv, status, n_fallback, w);
+    });
+}
+
+int launch_alpha_mle_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
+                           const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
+                           int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
+    return with_warps(d, [&](auto w) {
+        return alpha_mle_t<decltype(w)::value>(c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_var, prior_var_dev, cr_reg, prior_reg,
+                                alpha, conv, status, hint_in, hint_out);
+    });
+}
+
+int launch_wald_large(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu, int64_t ld_mu, int G,
+                      const double* ridge, const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
+    return with_warps(d, [&](auto w) { return wald_t<decltype(w)::value>(c, d, disp, lfc, mu, ld_mu, G, ridge, contrast, lfc_null, alt, pv, stat, se); });
+}
+
+int launch_wald_contrasts_large(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
+                                const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
+    return with_warps(d, [&](auto w) { return wald_contrasts_t<decltype(w)::value>(c, d, disp, lfc, G, ridge, K, tab, pv, stat, se, ld_out); });
+}
+
+int launch_rough_large(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {
+    return with_warps(d, [&](auto w) { return rough_t<decltype(w)::value>(c, d, normed, ld, G, alpha); });
+}
+
+int launch_moments_large(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha, double* all_zero) {
+    return launch_moments_wide(c, d, normed, ld, G, alpha, all_zero);
+}
+
+int launch_mom_from_counts_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp,
+                                 double max_disp, double* alpha, double* normed_mean, double min_mu, double* mu_hat, int64_t ld_mu) {
+    return with_warps(d, [&](auto w) {
+        return mom_from_counts_t<decltype(w)::value>(c, d, counts, ld, G, min_disp, max_disp, alpha, normed_mean, min_mu, mu_hat, ld_mu);
+    });
+}
+
+int launch_mu_from_lfc_large(const LaunchCfg& c, const DesignDev& d, const double* lfc, int G, double* mu, int64_t ld_out) {
+    return launch_mu_from_lfc_wide(c, d, lfc, G, mu, ld_out);
+}
+
+int launch_cooks_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
+                       int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced) {
+    return launch_cooks_wide(c, d, counts, ld, G, mu, hat, ld2, cutoff, cooks, ld_out, disp, outlier, replaced);
+}
+
+// apeGLM shrinkage above PDQ_MAX_P_WIDE columns is not implemented (refused in pdq_api.cu before it gets here)
+int launch_lfc_shrink_large(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, const double*, double, double, int, double*,
+                            double*, double*, int*) {
+    return PDQ_ERR_UNSUPPORTED;
 }
 
 int launch_lfc_shrink_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* size,
