@@ -549,7 +549,7 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
         memcpy(dd.pinv, pinv.data(), pinv.size() * 8);
     } else if (cudaMalloc((void**)&dd.pinv_dev, pinv.size() * 8) != cudaSuccess ||
                cudaMemcpy(dd.pinv_dev, pinv.data(), pinv.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess ||
-               (p > PDQ_MAX_P_WIDE && cudaMalloc((void**)&dd.wald_dev, ((size_t)p * (p + 1) / 2 + 1 + p) * 8) != cudaSuccess)) {
+               cudaMalloc((void**)&dd.wald_dev, ((size_t)p * (p + 1) / 2 + 1 + p) * 8) != cudaSuccess) {
         if (dd.pinv_dev) cudaFree(dd.pinv_dev);
         if (dd.wald_dev) cudaFree(dd.wald_dev);
         delete d;

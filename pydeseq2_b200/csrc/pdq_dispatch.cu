@@ -2,11 +2,11 @@
 //
 // pdq_kernels.cu is compiled once for p = 1..8 (p x p algebra unrolled in registers) and once per wide width p = 9..16
 // (same source, the small matrices in local memory): see the note at the top of that file and pydeseq2_b200/build.py.  Every
-// unit exports its launchers under a suffixed name; the functions declared in pdq_internal.h live here.  Designs of 17..64
-// columns (only created on contexts that opted in) go to pdq_wide.cu's launchers (`_wide`), designs of 65..128 columns (a second
-// opt-in) to its team-per-gene launchers (`_large`).  The fused MAP -> LFC pair has neither and reports PDQ_ERR_UNSUPPORTED for
-// them; apeGLM shrinkage reaches its wide launcher only on a context that also opted in to wide shrinkage (pdq_set_wide_shrink,
-// checked in pdq_api.cu), and has no large one.
+// unit exports its launchers under a suffixed name; the functions declared in pdq_internal.h live here.  Designs of 17..128
+// columns (only created on contexts that opted in: 65..128 columns are a second opt-in) go to pdq_wide.cu's launchers (`_wide`),
+// which pick the team width from the design.  The fused MAP -> LFC pair has none and reports PDQ_ERR_UNSUPPORTED for them;
+// apeGLM shrinkage reaches its wide launcher only on a context that also opted in to wide shrinkage (pdq_set_wide_shrink,
+// checked in pdq_api.cu), and only up to PDQ_MAX_P_WIDE columns.
 #include "pdq_internal.h"
 
 namespace pdq {
@@ -28,12 +28,11 @@ namespace pdq {
         default: return PDQ_ERR_UNSUPPORTED;                      \
     }
 
-#define PDQ_ROUTE_WIDE(name, p, ...)                                                     \
-    if ((p) > PDQ_MAX_P_WIDE) return (p) <= PDQ_MAX_P_LARGE ? name##_large(__VA_ARGS__) : PDQ_ERR_UNSUPPORTED; \
-    if ((p) > PDQ_MAX_P) return name##_wide(__VA_ARGS__); \
+#define PDQ_ROUTE_WIDE(name, p, ...)                                                                     \
+    if ((p) > PDQ_MAX_P) return (p) <= PDQ_MAX_P_LARGE ? name##_wide(__VA_ARGS__) : PDQ_ERR_UNSUPPORTED; \
     PDQ_ROUTE(name, p, __VA_ARGS__)
 
-#define PDQ_UNITS_ALL(X) PDQ_UNITS(X) X(_wide) X(_large)
+#define PDQ_UNITS_ALL(X) PDQ_UNITS(X) X(_wide)
 
 #define DECL_LIN(sfx) int launch_lin_reg_mu##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, double, double*, int64_t);
 PDQ_UNITS_ALL(DECL_LIN)

@@ -15,8 +15,9 @@ struct DesignDev {
     int few_rows;       // X has at most 16 distinct rows (categorical design): k_irls reuses exp(x'beta) across equal rows
     double pinv[PDQ_MAX_P * PDQ_MAX_P];  // (X^T X)^+ row-major p x p (host copy, passed by value to kernels), p <= PDQ_MAX_P
     double* pinv_dev = nullptr;          // device copy of (X^T X)^+ for wide designs (p > PDQ_MAX_P), read by pdq_wide.cu
-    double* wald_dev = nullptr;          // p > PDQ_MAX_P_WIDE: the Wald ridge (packed) and contrast of the latest launch, pdq_wide.cu
-    int warps = 0;                       // p > PDQ_MAX_P_WIDE: warps per gene (0: the built-in choice; PDQ_LARGE_WARPS tuning hook)
+    double* wald_dev = nullptr;          // p > PDQ_MAX_P: the Wald ridge (packed) and contrast of the latest launch, read by pdq_wide.cu
+    int warps = 0;                       // p > PDQ_MAX_P_WIDE: warps per gene (0: the built-in choice; PDQ_LARGE_WARPS tuning hook);
+                                         // unused below, where with_warps (pdq_wide.cu) always picks one
     double s_mean_inv;  // mean(1 / size_factors)  (utils.py:880)
     int staged;         // the pack is small enough to be copied into shared memory by every block (else read from global / L1)
     size_t smem_bytes;  // dynamic shared memory the kernels need for the design: staged pack + mbarrier, or the mbarrier alone

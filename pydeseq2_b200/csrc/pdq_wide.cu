@@ -1,6 +1,6 @@
-// pdq_wide.cu -- per-gene kernels for designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns (opt-in per context:
-// pdq_set_wide_designs; launchers `_wide`) and of PDQ_MAX_P_WIDE + 1 .. PDQ_MAX_P_LARGE columns (a second opt-in on top of it:
-// pdq_set_large_designs; launchers `_large`).
+// pdq_wide.cu -- per-gene kernels and their launchers (`_wide`) for designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns (opt-in
+// per context: pdq_set_wide_designs) and of PDQ_MAX_P_WIDE + 1 .. PDQ_MAX_P_LARGE columns (a second opt-in on top of it:
+// pdq_set_large_designs).
 //
 // The kernels of pdq_kernels.cu keep one gene's p x p state per LANE: in registers for p <= 8, in local memory for 9..16.  At
 // p = 64 one packed symmetric matrix is 16.6 KB, so that layout does not scale.  Here one TEAM of W warps owns one gene (one team
@@ -11,11 +11,11 @@
 //     vectors such as X^T W z are split over their components;
 //   * the Cholesky factorisation, the triangular solves and the inverse are cooperative, one team barrier per column step;
 //   * sums and votes are warp butterflies, combined across the warps through per-warp slots in shared memory.
-// The 17..64 tier runs W = 1 (a warp barrier is enough, and the Wald ridge and contrast travel as kernel parameters).  At p = 128
-// the workspace is ~204 KB, so one block fits per SM: the 65..128 tier runs W = 2, 4 or 8 warps per gene (large_warps) to keep the SM's FP64
-// pipes busy, and reads the Wald ridge and contrast from a device buffer next to the design pack (DesignDev::wald_dev; they
-// exceed the 32 KB kernel-parameter limit there).  Passes whose work does not grow with p (moments, mu from LFCs, Cook's
-// distances) run the W = 1 kernels at every width.
+// The 17..64 tier runs W = 1 (a warp barrier is enough).  At p = 128 the workspace is ~204 KB, so one block fits per SM: the
+// 65..128 tier runs W = 2, 4 or 8 warps per gene (large_warps) to keep the SM's FP64 pipes busy.  with_warps picks W for a design.
+// At every width the kernels read the Wald ridge and contrast from a device buffer next to the design pack
+// (DesignDev::wald_dev; at 128 columns they exceed the 32 KB kernel-parameter limit).  Passes whose work does not grow with p
+// (moments, mu from LFCs, Cook's distances) run the W = 1 kernels at every width.
 // The design pack is read from global memory (it stays in L1 / L2).  The per-gene semantics are those of pdq_gene.cuh -- start
 // values, ridge, stopping rules, optimiser branch, dispersion search and grid, Wald alternatives, Cook's distances -- written
 // against libdevice's exp / log and the series of pdq_math.cuh instead of the table-driven cores; parity is to the reference's
@@ -32,7 +32,6 @@
 namespace pdq {
 namespace {
 
-constexpr int kMaxTri = PDQ_MAX_P_WIDE * (PDQ_MAX_P_WIDE + 1) / 2;
 constexpr int kVecs = 8;  // vectors of p doubles in the workspace
 
 // the cooperative primitives of one gene's team of W warps (the whole block)
@@ -296,24 +295,14 @@ __device__ void apply_pinv(const double* pinv, const double* v, double* beta, in
 // ---------------------------------------------------------------------------------------------
 // Wald test from M = X^T W X (wald_inverse + wald_contrast of pdq_gene.cuh)
 // ---------------------------------------------------------------------------------------------
-struct WideWald {
-    double ridge[kMaxTri];             // lower triangle of the caller's p x p ridge matrix, packed (the only part wald_inverse reads)
-    double contrast[PDQ_MAX_P_WIDE];
-    double lfc_null;
-    int alt;
-};
-// the same parameters of a 65..128-column design: ridge and contrast in device memory (DesignDev::wald_dev, wald_dev_layout)
+// ridge (lower triangle of the caller's p x p matrix, packed: the only part wald_inverse reads) and contrast in device memory
+// (DesignDev::wald_dev, written by put_wald)
 struct WaldRef {
     const double* ridge;
     const double* contrast;
     double lfc_null;
     int alt;
 };
-template <int W>
-using WaldOf = std::conditional_t<W == 1, WideWald, WaldRef>;
-// the packed ridge of the K-contrast test: a kernel parameter at W = 1, a device pointer above
-template <int W>
-using RidgeOf = std::conditional_t<W == 1, double[kMaxTri], const double*>;
 
 // statistic and p-value of alternative `alt` given SE (every lane, replicated; the same expressions as wald_contrast)
 __device__ void wald_alt(const double* c, const double* b, int p, double se, double t0, int alt, double& pv, double& stat) {
@@ -368,8 +357,8 @@ __device__ double wald_se_w(const double* M, const double* c, Ws& ws) {
     return sqrt(T::sum(q));
 }
 
-template <int W, class WP>
-__device__ void wald_finish_w(const double* M, const WP& w, const double* beta, Ws& ws, double* p_out, double* stat_out,
+template <int W>
+__device__ void wald_finish_w(const double* M, const WaldRef& w, const double* beta, Ws& ws, double* p_out, double* stat_out,
                               double* se_out) {
     using T = Team<W>;
     wald_inverse_w<W>(M, w.ridge, ws);
@@ -540,7 +529,6 @@ __global__ void __launch_bounds__(32) k_wide_mu_from_lfc(const __grid_constant__
 // ---------------------------------------------------------------------------------------------
 // irls (irls_gene + irls_optimizer_gene)
 // ---------------------------------------------------------------------------------------------
-template <int W>
 struct IrlsArgsW {
     WideBase b;
     IrlsParams prm;
@@ -553,7 +541,7 @@ struct IrlsArgsW {
     int* n_fallback;
     int force;
     int with_wald;
-    WaldOf<W> wald;
+    WaldRef wald;
     double *wald_p, *wald_stat, *wald_se;
 };
 
@@ -716,7 +704,7 @@ __device__ __forceinline__ bool is_fixed(double b, double g, double lo, double h
 
 // the reference's L-BFGS-B branch (utils.py:374-413) as projected Newton: irls_optimizer_gene, every output written here
 template <int W = 1>
-__device__ void irls_optimizer_w(const IrlsArgsW<W>& a, const DesignS& d, Ws& ws, int g) {
+__device__ void irls_optimizer_w(const IrlsArgsW& a, const DesignS& d, Ws& ws, int g) {
     using T = Team<W>;
     const int p = a.b.p, lane = T::tid();
     const IrlsParams& prm = a.prm;
@@ -800,7 +788,7 @@ __device__ void irls_optimizer_w(const IrlsArgsW<W>& a, const DesignS& d, Ws& ws
 }
 
 template <int W>
-__global__ void __maxnreg__(224) k_wide_irls(const __grid_constant__ IrlsArgsW<W> a) {
+__global__ void __maxnreg__(224) k_wide_irls(const __grid_constant__ IrlsArgsW a) {
     using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
     Ws ws = carve<W>(wsm, a.b.p);
@@ -1007,17 +995,16 @@ __global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_alpha_mle(const
 // ---------------------------------------------------------------------------------------------
 // Wald tests
 // ---------------------------------------------------------------------------------------------
-template <int W>
 struct WaldArgsW {
     WideBase b;
-    WaldOf<W> w;
+    WaldRef w;
     const double *disp, *lfc, *mu;
     int64_t ld_mu;
     double *pv, *stat, *se;
 };
 
 template <int W>
-__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_wald(const __grid_constant__ WaldArgsW<W> a) {
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_wald(const __grid_constant__ WaldArgsW a) {
     using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
     Ws ws = carve<W>(wsm, a.b.p);
@@ -1043,10 +1030,9 @@ __global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_wald(const __gr
     wald_finish_w<W>(ws.A, a.w, ws.v[1], ws, a.pv + g, a.stat + g, a.se + g);
 }
 
-template <int W>
 struct WaldKArgsW {
     WideBase b;
-    RidgeOf<W> ridge;
+    const double* ridge;  // packed, DesignDev::wald_dev
     const double *disp, *lfc, *tab;  // tab (K, p + 2): contrast | lfc_null | alt
     int K;
     double *pv, *stat, *se;
@@ -1054,7 +1040,7 @@ struct WaldKArgsW {
 };
 
 template <int W>
-__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_wald_contrasts(const __grid_constant__ WaldKArgsW<W> a) {
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_wald_contrasts(const __grid_constant__ WaldKArgsW a) {
     using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
     Ws ws = carve<W>(wsm, a.b.p);
@@ -1442,13 +1428,6 @@ void pack_lower(const double* full, int p, double* tri_out) {
         for (int j = 0; j <= i; ++j) tri_out[tri(i, j)] = full[i * p + j];
 }
 
-void wide_wald(const WaldHost& h, int p, WideWald& w) {
-    pack_lower(h.ridge, p, w.ridge);
-    for (int j = 0; j < p; ++j) w.contrast[j] = h.contrast[j];
-    w.lfc_null = h.lfc_null;
-    w.alt = h.alt;
-}
-
 // host values -> device memory as kernel parameters, in chunks that fit the parameter space: stream-ordered behind the kernels
 // that read the previous values, and a captured graph keeps the values of its capture
 constexpr int kPutChunk = 3968;
@@ -1457,7 +1436,7 @@ struct PutArgs {
     double* dst;
     int n;
 };
-__global__ void __launch_bounds__(256) k_large_put(const __grid_constant__ PutArgs a) {
+__global__ void __launch_bounds__(256) k_wide_put(const __grid_constant__ PutArgs a) {
     for (int i = threadIdx.x; i < a.n; i += blockDim.x) a.dst[i] = a.v[i];
 }
 
@@ -1469,14 +1448,16 @@ int put_dev(const LaunchCfg& c, const double* h, int n, double* dst) {
         a.n = (n - o < kPutChunk) ? n - o : kPutChunk;
         a.dst = dst + o;
         for (int i = 0; i < a.n; ++i) a.v[i] = h[o + i];
-        k_large_put<<<1, 256, 0, c.stream>>>(a);
+        k_wide_put<<<1, 256, 0, c.stream>>>(a);
         if (int e = check_launch()) return e;
         ++launches;
     }
     return launches;
 }
 
-// ridge (packed lower triangle) and contrast of a 65..128-column design into DesignDev::wald_dev; contrast may be null
+// ridge (packed lower triangle) and contrast into DesignDev::wald_dev; contrast may be null.  The host-buffer calls launch once
+// per gene block, and with the gene-block pipeline the upload of block b + 1 (on the other stream) can write wald_dev while block
+// b's kernel reads it.  That is safe because every upload within one call writes the same bytes.
 int put_wald(const LaunchCfg& c, const DesignDev& d, const double* ridge, const double* contrast, WaldRef& w) {
     const int p = d.p, t = tri_count(p);
     double buf[PDQ_MAX_P_LARGE * (PDQ_MAX_P_LARGE + 1) / 2 + 1 + PDQ_MAX_P_LARGE];
@@ -1498,9 +1479,10 @@ int large_warps(int p) {
     return 8;
 }
 
-// the 65..128 tier's team width: DesignDev::warps (a tuning hook) or large_warps
+// the team width of a design: one warp up to PDQ_MAX_P_WIDE columns, above that DesignDev::warps (a tuning hook) or large_warps
 template <class F>
 int with_warps(const DesignDev& d, F&& f) {
+    if (d.p <= PDQ_MAX_P_WIDE) return f(std::integral_constant<int, 1>{});
     switch (d.warps ? d.warps : large_warps(d.p)) {
         case 2: return f(std::integral_constant<int, 2>{});
         case 4: return f(std::integral_constant<int, 4>{});
@@ -1508,22 +1490,29 @@ int with_warps(const DesignDev& d, F&& f) {
     }
 }
 
-template <int W>
-int lin_reg_mu_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
-                 int64_t ld_out) {
-    const LinArgs a{base_of(d, G), counts, ld, min_mu, mu_out, ld_out};
-    if (int e = prep(k_wide_lin_reg_mu<W>, ws_bytes(d.p, W))) return e;
-    k_wide_lin_reg_mu<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
+// one block of W warps per gene with its workspace; returns the number of launches, the `puts` Wald uploads included
+template <int W, class A>
+int launch_team(const LaunchCfg& c, const DesignDev& d, int G, void (*kernel)(A), const A& a, int puts = 0) {
+    const size_t smem = ws_bytes(d.p, W);
+    if (int e = prep(kernel, smem)) return e;
+    kernel<<<G, 32 * W, smem, c.stream>>>(a);
     if (int e = check_launch()) return e;
-    return 1;
+    return 1 + puts;
 }
 
-template <int W>
-int irls_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
-           double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
+}  // namespace
+
+int launch_lin_reg_mu_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
+                           int64_t ld_out) {
+    const LinArgs a{base_of(d, G), counts, ld, min_mu, mu_out, ld_out};
+    return with_warps(d, [&](auto w) { return launch_team<decltype(w)::value>(c, d, G, k_wide_lin_reg_mu<decltype(w)::value>, a); });
+}
+
+int launch_irls_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
+                     double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
     if (n_fallback && cudaMemsetAsync(n_fallback, 0, sizeof(int), c.stream) != cudaSuccess) return PDQ_ERR_CUDA;
     int puts = 0;
-    IrlsArgsW<W> a{};
+    IrlsArgsW a{};
     a.b = base_of(d, G);
     a.prm = IrlsParams{h.min_mu, h.beta_tol, h.min_beta, h.max_beta, h.maxiter, d.full_rank, d.few_rows,
                        (c.debug & PDQ_DEBUG_FAIL_IRLS_OPTIMIZER) ? 1 : 0};
@@ -1533,127 +1522,50 @@ int irls_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_
     a.force = (c.debug & PDQ_DEBUG_FORCE_IRLS_OPTIMIZER) ? 1 : 0;
     a.with_wald = w ? 1 : 0;
     if (w) {
-        if constexpr (W == 1) {
-            wide_wald(*w, d.p, a.wald);
-        } else {
-            if ((puts = put_wald(c, d, w->ridge, w->contrast, a.wald)) < 0) return puts;
-            a.wald.lfc_null = w->lfc_null;
-            a.wald.alt = w->alt;
-        }
+        if ((puts = put_wald(c, d, w->ridge, w->contrast, a.wald)) < 0) return puts;
+        a.wald.lfc_null = w->lfc_null;
+        a.wald.alt = w->alt;
         a.wald_p = w->pv; a.wald_stat = w->stat; a.wald_se = w->se;
     }
-    if (int e = prep(k_wide_irls<W>, ws_bytes(d.p, W))) return e;
-    k_wide_irls<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1 + puts;
-}
-
-template <int W>
-int alpha_mle_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
-                const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
-                int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
-    const AlphaArgsW a{base_of(d, G), AlphaParams{log(min_disp), log(max_disp), prior_var, cr_reg, prior_reg}, counts, ld, mu, ld_mu,
-                       alpha_hat, alpha, conv, status, prior_var_dev, (c.debug & PDQ_DEBUG_FORCE_ALPHA_GRID) ? 1 : 0, hint_in, hint_out};
-    if (int e = prep(k_wide_alpha_mle<W>, ws_bytes(d.p, W))) return e;
-    k_wide_alpha_mle<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
-}
-
-template <int W>
-int wald_t(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu, int64_t ld_mu, int G,
-           const double* ridge, const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
-    int puts = 0;
-    WaldArgsW<W> a{};
-    a.b = base_of(d, G);
-    if constexpr (W == 1) {
-        wide_wald(WaldHost{ridge, contrast, lfc_null, alt, pv, stat, se}, d.p, a.w);
-    } else {
-        if ((puts = put_wald(c, d, ridge, contrast, a.w)) < 0) return puts;
-        a.w.lfc_null = lfc_null;
-        a.w.alt = alt;
-    }
-    a.disp = disp; a.lfc = lfc; a.mu = mu; a.ld_mu = ld_mu;
-    a.pv = pv; a.stat = stat; a.se = se;
-    if (int e = prep(k_wide_wald<W>, ws_bytes(d.p, W))) return e;
-    k_wide_wald<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1 + puts;
-}
-
-template <int W>
-int wald_contrasts_t(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
-                     const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
-    int puts = 0;
-    WaldKArgsW<W> a{};
-    a.b = base_of(d, G);
-    if constexpr (W == 1) {
-        pack_lower(ridge, d.p, a.ridge);
-    } else {
-        WaldRef w;
-        if ((puts = put_wald(c, d, ridge, nullptr, w)) < 0) return puts;
-        a.ridge = w.ridge;
-    }
-    a.disp = disp; a.lfc = lfc; a.tab = tab; a.K = K;
-    a.pv = pv; a.stat = stat; a.se = se; a.ld_out = ld_out;
-    if (int e = prep(k_wide_wald_contrasts<W>, ws_bytes(d.p, W))) return e;
-    k_wide_wald_contrasts<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1 + puts;
-}
-
-template <int W>
-int rough_t(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {
-    const MomArgsW a{base_of(d, G), normed, nullptr, ld, d.s_mean_inv, 0.0, 0.0, 0.0, alpha, nullptr, nullptr, 0};
-    if (int e = prep(k_wide_rough<W>, ws_bytes(d.p, W))) return e;
-    k_wide_rough<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
-}
-
-template <int W>
-int mom_from_counts_t(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp, double max_disp,
-                      double* alpha, double* normed_mean, double min_mu, double* mu_hat, int64_t ld_mu) {
-    const MomArgsW a{base_of(d, G), nullptr, counts, ld, d.s_mean_inv, min_disp, max_disp, min_mu, alpha, normed_mean, mu_hat, ld_mu};
-    if (int e = prep(k_wide_mom_from_counts<W>, ws_bytes(d.p, W))) return e;
-    k_wide_mom_from_counts<W><<<G, 32 * W, ws_bytes(d.p, W), c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
-}
-
-}  // namespace
-
-int launch_lin_reg_mu_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
-                           int64_t ld_out) {
-    return lin_reg_mu_t<1>(c, d, counts, ld, G, min_mu, mu_out, ld_out);
-}
-
-int launch_irls_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
-                     double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
-    return irls_t<1>(c, d, counts, ld, G, disp, h, beta, mu, hat, ld_out, conv, status, n_fallback, w);
+    return with_warps(d, [&](auto tw) { return launch_team<decltype(tw)::value>(c, d, G, k_wide_irls<decltype(tw)::value>, a, puts); });
 }
 
 int launch_alpha_mle_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
                           const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
                           int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
-    return alpha_mle_t<1>(c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_var, prior_var_dev, cr_reg, prior_reg, alpha,
-                          conv, status, hint_in, hint_out);
+    const AlphaArgsW a{base_of(d, G), AlphaParams{log(min_disp), log(max_disp), prior_var, cr_reg, prior_reg}, counts, ld, mu, ld_mu,
+                       alpha_hat, alpha, conv, status, prior_var_dev, (c.debug & PDQ_DEBUG_FORCE_ALPHA_GRID) ? 1 : 0, hint_in, hint_out};
+    return with_warps(d, [&](auto w) { return launch_team<decltype(w)::value>(c, d, G, k_wide_alpha_mle<decltype(w)::value>, a); });
 }
 
 int launch_wald_wide(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu, int64_t ld_mu, int G,
                      const double* ridge, const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
-    return wald_t<1>(c, d, disp, lfc, mu, ld_mu, G, ridge, contrast, lfc_null, alt, pv, stat, se);
+    WaldArgsW a{};
+    a.b = base_of(d, G);
+    const int puts = put_wald(c, d, ridge, contrast, a.w);
+    if (puts < 0) return puts;
+    a.w.lfc_null = lfc_null;
+    a.w.alt = alt;
+    a.disp = disp; a.lfc = lfc; a.mu = mu; a.ld_mu = ld_mu;
+    a.pv = pv; a.stat = stat; a.se = se;
+    return with_warps(d, [&](auto w) { return launch_team<decltype(w)::value>(c, d, G, k_wide_wald<decltype(w)::value>, a, puts); });
 }
 
 int launch_wald_contrasts_wide(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
                                const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
-    return wald_contrasts_t<1>(c, d, disp, lfc, G, ridge, K, tab, pv, stat, se, ld_out);
+    WaldRef r;
+    const int puts = put_wald(c, d, ridge, nullptr, r);
+    if (puts < 0) return puts;
+    const WaldKArgsW a{base_of(d, G), r.ridge, disp, lfc, tab, K, pv, stat, se, ld_out};
+    return with_warps(d, [&](auto w) { return launch_team<decltype(w)::value>(c, d, G, k_wide_wald_contrasts<decltype(w)::value>, a, puts); });
 }
 
 int launch_rough_wide(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {
-    return rough_t<1>(c, d, normed, ld, G, alpha);
+    const MomArgsW a{base_of(d, G), normed, nullptr, ld, d.s_mean_inv, 0.0, 0.0, 0.0, alpha, nullptr, nullptr, 0};
+    return with_warps(d, [&](auto w) { return launch_team<decltype(w)::value>(c, d, G, k_wide_rough<decltype(w)::value>, a); });
 }
 
+// the passes whose work does not grow with p (moments, mu from LFCs, Cook's distances) run one warp per gene at every width
 int launch_moments_wide(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha, double* all_zero) {
     const MomArgsW a{base_of(d, G), normed, nullptr, ld, d.s_mean_inv, 0.0, 0.0, 0.0, alpha, all_zero, nullptr, 0};
     k_wide_moments<<<G, 32, 0, c.stream>>>(a);
@@ -1663,7 +1575,8 @@ int launch_moments_wide(const LaunchCfg& c, const DesignDev& d, const double* no
 
 int launch_mom_from_counts_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp,
                                 double max_disp, double* alpha, double* normed_mean, double min_mu, double* mu_hat, int64_t ld_mu) {
-    return mom_from_counts_t<1>(c, d, counts, ld, G, min_disp, max_disp, alpha, normed_mean, min_mu, mu_hat, ld_mu);
+    const MomArgsW a{base_of(d, G), nullptr, counts, ld, d.s_mean_inv, min_disp, max_disp, min_mu, alpha, normed_mean, mu_hat, ld_mu};
+    return with_warps(d, [&](auto w) { return launch_team<decltype(w)::value>(c, d, G, k_wide_mom_from_counts<decltype(w)::value>, a); });
 }
 
 int launch_mu_from_lfc_wide(const LaunchCfg& c, const DesignDev& d, const double* lfc, int G, double* mu, int64_t ld_out) {
@@ -1684,72 +1597,10 @@ int launch_cooks_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* cou
     return 1;
 }
 
-// ---- 65..128 columns: the same kernels with a team of W warps per gene; the passes whose work does not grow with p (moments,
-// mu from LFCs, Cook's distances) are the one-warp kernels above
-int launch_lin_reg_mu_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_mu, double* mu_out,
-                            int64_t ld_out) {
-    return with_warps(d, [&](auto w) { return lin_reg_mu_t<decltype(w)::value>(c, d, counts, ld, G, min_mu, mu_out, ld_out); });
-}
-
-int launch_irls_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp, const IrlsHost& h,
-                      double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback, const WaldHost* w) {
-    return with_warps(d, [&](auto tw) {
-        return irls_t<decltype(tw)::value>(c, d, counts, ld, G, disp, h, beta, mu, hat, ld_out, conv, status, n_fallback, w);
-    });
-}
-
-int launch_alpha_mle_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
-                           const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
-                           int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
-    return with_warps(d, [&](auto w) {
-        return alpha_mle_t<decltype(w)::value>(c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_var, prior_var_dev, cr_reg, prior_reg,
-                                alpha, conv, status, hint_in, hint_out);
-    });
-}
-
-int launch_wald_large(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, const double* mu, int64_t ld_mu, int G,
-                      const double* ridge, const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
-    return with_warps(d, [&](auto w) { return wald_t<decltype(w)::value>(c, d, disp, lfc, mu, ld_mu, G, ridge, contrast, lfc_null, alt, pv, stat, se); });
-}
-
-int launch_wald_contrasts_large(const LaunchCfg& c, const DesignDev& d, const double* disp, const double* lfc, int G, const double* ridge, int K,
-                                const double* tab, double* pv, double* stat, double* se, int64_t ld_out) {
-    return with_warps(d, [&](auto w) { return wald_contrasts_t<decltype(w)::value>(c, d, disp, lfc, G, ridge, K, tab, pv, stat, se, ld_out); });
-}
-
-int launch_rough_large(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha) {
-    return with_warps(d, [&](auto w) { return rough_t<decltype(w)::value>(c, d, normed, ld, G, alpha); });
-}
-
-int launch_moments_large(const LaunchCfg& c, const DesignDev& d, const double* normed, int64_t ld, int G, double* alpha, double* all_zero) {
-    return launch_moments_wide(c, d, normed, ld, G, alpha, all_zero);
-}
-
-int launch_mom_from_counts_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp,
-                                 double max_disp, double* alpha, double* normed_mean, double min_mu, double* mu_hat, int64_t ld_mu) {
-    return with_warps(d, [&](auto w) {
-        return mom_from_counts_t<decltype(w)::value>(c, d, counts, ld, G, min_disp, max_disp, alpha, normed_mean, min_mu, mu_hat, ld_mu);
-    });
-}
-
-int launch_mu_from_lfc_large(const LaunchCfg& c, const DesignDev& d, const double* lfc, int G, double* mu, int64_t ld_out) {
-    return launch_mu_from_lfc_wide(c, d, lfc, G, mu, ld_out);
-}
-
-int launch_cooks_large(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
-                       int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced) {
-    return launch_cooks_wide(c, d, counts, ld, G, mu, hat, ld2, cutoff, cooks, ld_out, disp, outlier, replaced);
-}
-
-// apeGLM shrinkage above PDQ_MAX_P_WIDE columns is not implemented (refused in pdq_api.cu before it gets here)
-int launch_lfc_shrink_large(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, const double*, double, double, int, double*,
-                            double*, double*, int*) {
-    return PDQ_ERR_UNSUPPORTED;
-}
-
 int launch_lfc_shrink_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* size,
                            double prior_no_shrink_scale, double prior_scale, int shrink_index, double* beta, double* inv_hessian,
                            double* conv, int* status) {
+    if (d.p > PDQ_MAX_P_WIDE) return PDQ_ERR_UNSUPPORTED;  // one warp per gene only (pdq_api.cu refuses these designs first)
     if (shrink_index < 0 || shrink_index >= d.p) return PDQ_ERR_INVALID;
     const ShrinkArgsW a{base_of(d, G), ShrinkParams{1.0 / (prior_no_shrink_scale * prior_no_shrink_scale), prior_scale * prior_scale, shrink_index},
                         counts, ld, size, beta, inv_hessian, conv, status};

@@ -279,6 +279,46 @@ def test_large_opt_in_leaves_a_resident_pass_byte_identical():
             np.testing.assert_array_equal(v0, v1, err_msg=name)
 
 
+@pytest.mark.parametrize("subjects", [20, 100], ids=["p21", "p101"])
+def test_pipelined_wald_tests_are_byte_identical(monkeypatch, subjects):
+    """wald_tests (K = 4) and wald_test through the gene-block pipeline and without it: byte-equal.  The pipeline uploads the
+    Wald ridge and contrast into the design's device buffer once per gene block, on that block's stream, so an upload may
+    overwrite the buffer while the previous block's kernel reads it; every upload of one call writes the same bytes.
+    pipe_begin splits a call when G >= 4096, staging is on and every large host buffer is page-locked: here the (K, G) outputs
+    of wald_tests (K G = 65 536 elements, from which the backend hands out page-locked outputs) and the (N, G) mu of wald_test.
+    G = 16 384 gives four blocks of 4 096 genes, so the pipelined context counts four times the launches of the other."""
+    from pydeseq2_b200.inference import B200Inference
+
+    X = paired(subjects)
+    N, p = X.shape
+    G, K = 16384, 4
+    rng = np.random.default_rng(subjects)
+    lfc = np.c_[rng.normal(5.0, 1.0, G), rng.normal(0.0, 0.3, (G, p - 1))]
+    disp = np.exp(rng.uniform(np.log(0.05), np.log(0.5), G))
+    sf = np.exp(rng.normal(0.0, 0.2, N))
+    cs = np.eye(p)[[p - 1, 1, 2, p - 1]] - np.eye(p)[[0, 2, 3, 1]]
+    alts = [None, "greaterAbs", "greater", "lessAbs"]
+    monkeypatch.delenv("PDQ_PIPELINE", raising=False)
+    infs = [B200Inference(device=0, wide_designs=True, large_designs=True)]
+    monkeypatch.setenv("PDQ_PIPELINE", "0")  # read when the context is created
+    infs.append(B200Inference(device=0, wide_designs=True, large_designs=True))
+    outs, launches = [], []
+    for inf in infs:
+        ctx = inf._ops.ctx
+        mu = ctx.pinned_empty((N, G))
+        mu[:] = sf[:, None] * np.exp(X @ lfc.T)
+        n0 = ctx.launches()
+        many = inf.wald_tests(X, sf, disp, lfc, cs, lfc_null=0.1, alt_hypothesis=alts)
+        n1 = ctx.launches()
+        one = inf.wald_test(X, disp, lfc, mu, np.diag(np.repeat(1e-6, p)), cs[0], 0.1, "greaterAbs")
+        launches.append((n1 - n0, ctx.launches() - n1))
+        outs.append(list(many) + list(one))
+    assert launches[0] == (4 * launches[1][0], 4 * launches[1][1])
+    assert np.isfinite(outs[1][0]).mean() > 0.99
+    for name, a, b in zip(["pvalue", "stat", "se"] * 2, *outs):
+        np.testing.assert_array_equal(a.view(np.uint64), b.view(np.uint64), err_msg=name)
+
+
 @pytest.mark.parametrize("resident", [False, True])
 @pytest.mark.parametrize("name", [n if n in ("large_paired_p101", "large_levels_p70_outliers") else
                                   pytest.param(n, marks=pytest.mark.xfail(strict=True, reason=MULTIMODAL_REASON)) for n in LARGE_E2E])
