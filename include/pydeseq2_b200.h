@@ -81,16 +81,23 @@ int pdq_set_debug_flags(pdq_ctx* ctx, int flags);
 int pdq_set_wide_designs(pdq_ctx* ctx, int on);
 /* apeGLM shrinkage of designs of PDQ_MAX_P + 1 .. PDQ_MAX_P_WIDE columns (off by default).  It runs only on a context that also
  * has pdq_set_wide_designs on: otherwise the design is refused with the message of pdq_set_wide_designs (p <= PDQ_MAX_P), also
- * for a pack made while wide designs were on.  Outputs are those of the narrow path; no gene is refitted on a grid. */
+ * for a pack made while wide designs were on.  Outputs are those of the narrow path; no gene is refitted on a grid.  Designs
+ * of more than PDQ_MAX_P_WIDE columns need pdq_set_large_shrink as well. */
 int pdq_set_wide_shrink(pdq_ctx* ctx, int on);
 /* Designs of PDQ_MAX_P_WIDE + 1 .. PDQ_MAX_P_LARGE columns (paired designs of up to 127 subjects): off by default.  It takes
  * effect only on a context that also has pdq_set_wide_designs on; otherwise p > PDQ_MAX_P is refused with the message of
  * pdq_set_wide_designs (p <= PDQ_MAX_P), and with wide designs on but large designs off every code and message is that of the
  * wide tier (p <= PDQ_MAX_P_WIDE), also for a pack made while large designs were on.  Such designs run on kernels in which a
  * block of several warps owns one gene.  Above PDQ_MAX_P_LARGE: PDQ_ERR_UNSUPPORTED, and the message names PDQ_MAX_P_LARGE.
- * apeGLM shrinkage of these designs is not implemented (PDQ_ERR_UNSUPPORTED, "not implemented"), with or without
- * pdq_set_wide_shrink. */
+ * apeGLM shrinkage of these designs is a fourth opt-in, pdq_set_large_shrink; without it such calls report
+ * PDQ_ERR_UNSUPPORTED ("not implemented"), with or without pdq_set_wide_shrink. */
 int pdq_set_large_designs(pdq_ctx* ctx, int on);
+/* apeGLM shrinkage of designs of PDQ_MAX_P_WIDE + 1 .. PDQ_MAX_P_LARGE columns (off by default), on kernels in which a block of
+ * several warps owns one gene.  It runs only on a context that also has pdq_set_wide_designs, pdq_set_wide_shrink and
+ * pdq_set_large_designs on; with any of them off every code and message is the one that context gives without this opt-in,
+ * also for a pack made while they were on.  Designs of up to PDQ_MAX_P_WIDE columns are not affected.  Outputs are those of the
+ * wide path: shrunk LFCs, the full (G, p, p) inverse Hessians and the converged flags. */
+int pdq_set_large_shrink(pdq_ctx* ctx, int on);
 /* Host only, no device needed: (X^T X)^+ (p x p row-major) and whether X (N x p, row-major, p <= PDQ_MAX_P_WIDE) has full column
  * rank, from the one-sided Jacobi SVD every design pack is built with (numpy.linalg.matrix_rank's tolerance). */
 int pdq_design_pinv(const double* X, int N, int p, double* pinv_out, int* full_rank_out);

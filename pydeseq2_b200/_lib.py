@@ -47,6 +47,7 @@ _SIGNATURES = {
     "pdq_set_wide_designs": (C.c_int, [c_ctx, C.c_int]),
     "pdq_set_wide_shrink": (C.c_int, [c_ctx, C.c_int]),
     "pdq_set_large_designs": (C.c_int, [c_ctx, C.c_int]),
+    "pdq_set_large_shrink": (C.c_int, [c_ctx, C.c_int]),
     "pdq_design_pinv": (C.c_int, [f64p, C.c_int, C.c_int, f64p, C.POINTER(C.c_int)]),
     "pdq_design_pinv_large": (C.c_int, [f64p, C.c_int, C.c_int, f64p, C.POINTER(C.c_int)]),
     "pdq_launch_count": (C.c_int64, [c_ctx]),
@@ -195,6 +196,7 @@ class Context:
         self.wide_designs = False  # pdq_set_wide_designs: designs of up to PDQ_MAX_P_WIDE columns
         self.wide_shrink = False   # pdq_set_wide_shrink: apeGLM shrinkage of those designs
         self.large_designs = False  # pdq_set_large_designs: designs of up to PDQ_MAX_P_LARGE columns (with wide_designs)
+        self.large_shrink = False   # pdq_set_large_shrink: apeGLM shrinkage of those (with the three above)
         self._pin_pool = {}  # nbytes -> [addresses] of released page-locked blocks (cudaHostAlloc is expensive)
 
     def set_wide_designs(self, on: bool = True):
@@ -213,6 +215,13 @@ class Context:
         :meth:`set_wide_designs` as well, or designs wider than PDQ_MAX_P are refused as without it)."""
         self.check(self.lib.pdq_set_large_designs(self.h, 1 if on else 0))
         self.large_designs = bool(on)
+
+    def set_large_shrink(self, on: bool = True):
+        """Run apeGLM shrinkage of designs of PDQ_MAX_P_WIDE + 1 .. PDQ_MAX_P_LARGE columns on this context (off by default;
+        needs :meth:`set_wide_designs`, :meth:`set_wide_shrink` and :meth:`set_large_designs` as well, or such calls are
+        refused as without it)."""
+        self.check(self.lib.pdq_set_large_shrink(self.h, 1 if on else 0))
+        self.large_shrink = bool(on)
 
     def check(self, rc: int):
         if rc != 0:

@@ -164,6 +164,7 @@ struct pdq_ctx {
     int wide = 0;            // designs of up to PDQ_MAX_P_WIDE columns (pdq_set_wide_designs)
     int wide_shrink = 0;     // apeGLM shrinkage of those designs (pdq_set_wide_shrink)
     int large = 0;           // designs of up to PDQ_MAX_P_LARGE columns, with `wide` on as well (pdq_set_large_designs)
+    int large_shrink = 0;    // apeGLM shrinkage of those, with `wide_shrink` and `large` on as well (pdq_set_large_shrink)
     int64_t launches_at_capture = 0;
     int64_t buf_epoch = 0;   // bumped whenever ensure() re-allocates a context-owned buffer (captured graphs hold those pointers)
     NcclApi nccl;
@@ -379,6 +380,12 @@ extern "C" int pdq_set_wide_shrink(pdq_ctx* c, int on) {
 extern "C" int pdq_set_large_designs(pdq_ctx* c, int on) {
     if (!c) return PDQ_ERR_INVALID;
     c->large = on != 0;
+    return PDQ_OK;
+}
+
+extern "C" int pdq_set_large_shrink(pdq_ctx* c, int on) {
+    if (!c) return PDQ_ERR_INVALID;
+    c->large_shrink = on != 0;
     return PDQ_OK;
 }
 
@@ -802,7 +809,7 @@ extern "C" int pdq_lfc_shrink_dev(pdq_ctx* c, const pdq_design* d, const int64_t
             return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
         if (int e = check_width(c, d->d.p)) return e;  // a pack made before the wide-design opt-in was turned off
     }
-    if (d->d.p > PDQ_MAX_P_WIDE)  // reached with wide shrinkage on only (refused above otherwise)
+    if (d->d.p > PDQ_MAX_P_WIDE && !c->large_shrink)  // reached with wide shrinkage and large designs on only (refused above otherwise)
         return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented",
                     PDQ_MAX_P_WIDE);
     return done(c, launch_lfc_shrink(cfg(c, G, d->d.N), d->d, counts, ld, G, size, prior_no_shrink_scale, prior_scale, shrink_index, lfcs,
@@ -1638,7 +1645,7 @@ extern "C" int pdq_lfc_shrink_nbinom_glm(pdq_ctx* c, const double* X, const int6
     if (int e = cached_design(c, X, offset, N, p, &d, true)) return e;
     if (p > PDQ_MAX_P && !c->wide_shrink)
         return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
-    if (p > PDQ_MAX_P_WIDE)  // with or without wide shrinkage
+    if (p > PDQ_MAX_P_WIDE && !c->large_shrink)  // with or without wide shrinkage
         return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented",
                     PDQ_MAX_P_WIDE);
     void *dc, *dsize, *dbeta, *dih, *dconv, *status;

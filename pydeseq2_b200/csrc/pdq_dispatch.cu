@@ -6,7 +6,7 @@
 // columns (only created on contexts that opted in: 65..128 columns are a second opt-in) go to pdq_wide.cu's launchers (`_wide`),
 // which pick the team width from the design.  The fused MAP -> LFC pair has none and reports PDQ_ERR_UNSUPPORTED for them;
 // apeGLM shrinkage reaches its wide launcher only on a context that also opted in to wide shrinkage (pdq_set_wide_shrink,
-// checked in pdq_api.cu), and only up to PDQ_MAX_P_WIDE columns.
+// checked in pdq_api.cu), and above PDQ_MAX_P_WIDE columns only with large shrinkage on as well (pdq_set_large_shrink).
 #include "pdq_internal.h"
 
 namespace pdq {

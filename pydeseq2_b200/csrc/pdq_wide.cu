@@ -12,7 +12,8 @@
 //   * the Cholesky factorisation, the triangular solves and the inverse are cooperative, one team barrier per column step;
 //   * sums and votes are warp butterflies, combined across the warps through per-warp slots in shared memory.
 // The 17..64 tier runs W = 1 (a warp barrier is enough).  At p = 128 the workspace is ~204 KB, so one block fits per SM: the
-// 65..128 tier runs W = 2, 4 or 8 warps per gene (large_warps) to keep the SM's FP64 pipes busy.  with_warps picks W for a design.
+// 65..128 tier runs W = 2, 4 or 8 warps per gene (large_warps, from each kernel's workspace) to keep the SM's FP64 pipes busy.
+// with_warps picks W for a design.  apeGLM shrinkage of that tier is a further opt-in (pdq_set_large_shrink).
 // At every width the kernels read the Wald ridge and contrast from a device buffer next to the design pack
 // (DesignDev::wald_dev; at 128 columns they exceed the 32 KB kernel-parameter limit).  Passes whose work does not grow with p
 // (moments, mu from LFCs, Cook's distances) run the W = 1 kernels at every width.
@@ -56,6 +57,19 @@ struct Team {
         }
         return v;
     }
+    // maximum over the team, bit-identical in every thread
+    static __device__ __forceinline__ double max(double v) {
+        for (int o = 16; o; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+        if constexpr (W > 1) {
+            __shared__ double slot[W];
+            if ((threadIdx.x & 31) == 0) slot[threadIdx.x >> 5] = v;
+            __syncthreads();
+            v = slot[0];
+            for (int w = 1; w < W; ++w) v = fmax(v, slot[w]);
+            __syncthreads();
+        }
+        return v;
+    }
     static __device__ __forceinline__ bool any(bool b) {
         if constexpr (W == 1) return __any_sync(0xffffffffu, b) != 0;
         else return __syncthreads_or(b) != 0;
@@ -89,7 +103,6 @@ __device__ __forceinline__ Ws carve(double* s, int p) {
 }
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
-__device__ __forceinline__ double wsum(double v) { return Team<1>::sum(v); }
 
 __device__ __forceinline__ DesignS design_of(const double* pack, int N, int p) {
     DesignS d;
@@ -1096,14 +1109,16 @@ __global__ void __launch_bounds__(32) k_wide_cooks(const __grid_constant__ Cooks
 // ---------------------------------------------------------------------------------------------
 // The narrow driver keeps its vectors in per-lane register arrays indexed by unrolled loops; here they are shared-memory vectors
 // split over the lanes, so the driver below restates shrink_gene step for step (the line search, dcsrch_start / dcsrch_step /
-// dcstep, is shared as is).  Every scalar of the optimiser is computed redundantly on all lanes from butterfly sums or shared
-// vectors, so all branches are warp-uniform.
+// dcstep, is shared as is).  One team of W warps owns one gene, as in the fit kernels: W = 1 for 17..64 columns, W = 2, 4 or 8
+// above.  Every scalar of the optimiser (line-search state, theta, the memory's head and size, the convergence tests) is computed
+// redundantly in every thread of the team from Team<W>::sum / max totals or shared vectors, so it is bit-identical everywhere
+// and all branches are team-uniform; that is what lets the W > 1 barriers inside those totals be reached by the whole block.
 //
 // Workspace of one gene: two packed p x p matrices (X'FX and its inverse's scratch), kShrinkVecs vectors of p, the L-BFGS memory
-// S, Y (2 kShrinkMem p) with s'y and the two-loop's alphas (kShrinkMem each), two chunk buffers of 32.
+// S, Y (2 kShrinkMem p) with s'y and the two-loop's alphas (kShrinkMem each), two chunk buffers of 32 W.
 constexpr int kShrinkVecs = 9;
-__host__ __device__ constexpr size_t shrink_ws_doubles(int p) {
-    return 2 * (size_t)tri_count(p) + (size_t)(kShrinkVecs + 2 * kShrinkMem) * p + 2 * kShrinkMem + 64;
+__host__ __device__ constexpr size_t shrink_ws_doubles(int p, int W = 1) {
+    return 2 * (size_t)tri_count(p) + (size_t)(kShrinkVecs + 2 * kShrinkMem) * p + 2 * kShrinkMem + 64 * W;
 }
 
 struct ShrinkWs {
@@ -1113,6 +1128,7 @@ struct ShrinkWs {
     double *cw, *cz;
 };
 
+template <int W>
 __device__ __forceinline__ ShrinkWs carve_shrink(double* s, int p) {
     ShrinkWs w;
     const int t = tri_count(p);
@@ -1126,30 +1142,35 @@ __device__ __forceinline__ ShrinkWs carve_shrink(double* s, int p) {
     w.sy = w.Y + kShrinkMem * p;
     w.al = w.sy + kShrinkMem;
     w.cw = w.al + kShrinkMem;
-    w.cz = w.cw + 32;
+    w.cz = w.cw + Team<W>::NT;
     return w;
 }
 
-// sum_j a[j] b[j], lanes over the components, butterfly total (bit-identical on every lane)
+// sum_j a[j] b[j], threads over the components, team total (bit-identical in every thread)
+template <int W>
 __device__ __forceinline__ double wdot(const double* a, const double* b, int p) {
+    using T = Team<W>;
     double s = 0.0;
-    for (int j = lane_id(); j < p; j += 32) s = fma(a[j], b[j], s);
-    return wsum(s);
+    for (int j = T::tid(); j < p; j += T::NT) s = fma(a[j], b[j], s);
+    return T::sum(s);
 }
+template <int W>
 __device__ __forceinline__ double wmaxabs(const double* a, int p) {
+    using T = Team<W>;
     double m = 0.0;
-    for (int j = lane_id(); j < p; j += 32) m = fmax(m, fabs(a[j]));
-    for (int o = 16; o; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-    return m;
+    for (int j = T::tid(); j < p; j += T::NT) m = fmax(m, fabs(a[j]));
+    return T::max(m);
 }
 
 // unscaled f (returned) and, when `grad`, its gradient: shrink_eval
+template <int W>
 __device__ double shrink_eval_w(const DesignS& d, int p, const ShrinkParams& prm, const int64_t* y, int64_t ld, double size,
                                 double lsize, const double* beta, double* grad, ShrinkWs& ws) {
-    if (grad) wfill(grad, p, 0.0);
+    using T = Team<W>;
+    if (grad) wfill<W>(grad, p, 0.0);
     double nll = 0.0;
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
         double gi = 0.0;
         if (n < d.N) {
             const double* x = row_of(d, n);
@@ -1165,30 +1186,32 @@ __device__ double shrink_eval_w(const DesignS& d, int p, const ShrinkParams& prm
             gi = ys * q - yv;
         }
         if (!grad) continue;
-        __syncwarp();
-        ws.cz[lane_id()] = gi;
-        __syncwarp();
-        vec_chunk(d, p, n0, min(32, d.N - n0), ws.cz, grad);
+        T::sync();
+        ws.cz[T::tid()] = gi;
+        T::sync();
+        vec_chunk<W>(d, p, n0, min(T::NT, d.N - n0), ws.cz, grad);
     }
-    nll = wsum(nll);
+    nll = T::sum(nll);
     double prior = 0.0;
     for (int j = 0; j < p; ++j)
         prior += (j == prm.k) ? log1p(beta[j] * beta[j] / prm.scale2) : 0.5 * beta[j] * beta[j] * prm.inv_var0;
     if (grad) {
-        __syncwarp();
-        for (int j = lane_id(); j < p; j += 32)
+        T::sync();
+        for (int j = T::tid(); j < p; j += T::NT)
             grad[j] += (j == prm.k) ? 2.0 * beta[j] / (prm.scale2 + beta[j] * beta[j]) : beta[j] * prm.inv_var0;
     }
-    __syncwarp();
+    T::sync();
     return prior - nll;
 }
 
 // shrink_inv_hessian: (X'FX + 1 h')^-1 through Sherman-Morrison on the Cholesky factor of A = X'FX, written to ih (p x p)
+template <int W>
 __device__ void shrink_inv_hessian_w(const DesignS& d, int p, const ShrinkParams& prm, const int64_t* y, int64_t ld, double size,
                                      double lsize, const double* beta, double* ih, ShrinkWs& ws) {
-    wfill(ws.A, p * (p + 1) / 2, 0.0);
-    for (int n0 = 0; n0 < d.N; n0 += 32) {
-        const int n = n0 + lane_id();
+    using T = Team<W>;
+    wfill<W>(ws.A, p * (p + 1) / 2, 0.0);
+    for (int n0 = 0; n0 < d.N; n0 += T::NT) {
+        const int n = n0 + T::tid();
         double w = 0.0;
         if (n < d.N) {
             const double* x = row_of(d, n);
@@ -1197,18 +1220,18 @@ __device__ void shrink_inv_hessian_w(const DesignS& d, int p, const ShrinkParams
             const double t = exp(-fabs(dd));
             w = (yv + size) * (t / ((1.0 + t) * (1.0 + t)));  // (y+s) q (1-q)
         }
-        __syncwarp();
-        ws.cw[lane_id()] = w;
-        __syncwarp();
-        rank_chunk(d, p, n0, min(32, d.N - n0), ws.cw, ws.A);
+        T::sync();
+        ws.cw[T::tid()] = w;
+        T::sync();
+        rank_chunk<W>(d, p, n0, min(T::NT, d.N - n0), ws.cw, ws.A);
     }
-    chol_w(ws.A, p);
-    chol_inverse_w(ws.A, ws.Li, ws.A, p);  // A^-1 in ws.A
+    chol_w<W>(ws.A, p);
+    chol_inverse_w<W>(ws.A, ws.Li, ws.A, p);  // A^-1 in ws.A
     double *h = ws.t, *u = ws.r, *v = ws.q;  // the optimiser's vectors are free now
     const double bk = beta[prm.k], den = prm.scale2 + bk * bk;
-    for (int j = lane_id(); j < p; j += 32) h[j] = (j == prm.k) ? 2.0 * (prm.scale2 - bk * bk) / (den * den) : prm.inv_var0;
-    __syncwarp();
-    for (int i = lane_id(); i < p; i += 32) {
+    for (int j = T::tid(); j < p; j += T::NT) h[j] = (j == prm.k) ? 2.0 * (prm.scale2 - bk * bk) / (den * den) : prm.inv_var0;
+    T::sync();
+    for (int i = T::tid(); i < p; i += T::NT) {
         double su = 0.0, sv = 0.0;
         for (int j = 0; j < p; ++j) {
             const double aij = ws.A[j <= i ? tri(i, j) : tri(j, i)];
@@ -1218,41 +1241,43 @@ __device__ void shrink_inv_hessian_w(const DesignS& d, int p, const ShrinkParams
         u[i] = su;
         v[i] = sv;
     }
-    __syncwarp();
-    const double inv = 1.0 / (1.0 + wdot(h, u, p));
-    for (int k = lane_id(); k < p * p; k += 32) {
+    T::sync();
+    const double inv = 1.0 / (1.0 + wdot<W>(h, u, p));
+    for (int k = T::tid(); k < p * p; k += T::NT) {
         const int i = k / p, j = k - i * p;
         ih[k] = ws.A[j <= i ? tri(i, j) : tri(j, i)] - u[i] * v[j] * inv;
     }
 }
 
 // z = x + (L-BFGS step), with an empty memory z = x - g / theta: lbfgs_point
+template <int W>
 __device__ void lbfgs_point_w(int p, int col, int head, double theta, ShrinkWs& ws) {
-    const int lane = lane_id();
-    for (int j = lane; j < p; j += 32) ws.q[j] = -ws.g[j];
-    __syncwarp();
+    using T = Team<W>;
+    const int lane = T::tid();
+    for (int j = lane; j < p; j += T::NT) ws.q[j] = -ws.g[j];
+    T::sync();
     if (col == 0) {
-        for (int j = lane; j < p; j += 32) ws.z[j] = ws.x[j] + (1.0 / theta) * ws.q[j];
-        __syncwarp();
+        for (int j = lane; j < p; j += T::NT) ws.z[j] = ws.x[j] + (1.0 / theta) * ws.q[j];
+        T::sync();
         return;
     }
     for (int i = col - 1; i >= 0; --i) {  // newest -> oldest
         const int s = (head + i) % kShrinkMem;
-        const double a = wdot(ws.S + s * p, ws.q, p) / ws.sy[s];
+        const double a = wdot<W>(ws.S + s * p, ws.q, p) / ws.sy[s];
         if (lane == 0) ws.al[i] = a;
-        for (int j = lane; j < p; j += 32) ws.q[j] = ws.q[j] - a * ws.Y[s * p + j];
-        __syncwarp();
+        for (int j = lane; j < p; j += T::NT) ws.q[j] = ws.q[j] - a * ws.Y[s * p + j];
+        T::sync();
     }
-    for (int j = lane; j < p; j += 32) ws.q[j] = ws.q[j] / theta;
-    __syncwarp();
+    for (int j = lane; j < p; j += T::NT) ws.q[j] = ws.q[j] / theta;
+    T::sync();
     for (int i = 0; i < col; ++i) {  // oldest -> newest
         const int s = (head + i) % kShrinkMem;
-        const double b = wdot(ws.Y + s * p, ws.q, p) / ws.sy[s];
-        for (int j = lane; j < p; j += 32) ws.q[j] = ws.q[j] + ws.S[s * p + j] * (ws.al[i] - b);
-        __syncwarp();
+        const double b = wdot<W>(ws.Y + s * p, ws.q, p) / ws.sy[s];
+        for (int j = lane; j < p; j += T::NT) ws.q[j] = ws.q[j] + ws.S[s * p + j] * (ws.al[i] - b);
+        T::sync();
     }
-    for (int j = lane; j < p; j += 32) ws.z[j] = ws.x[j] + ws.q[j];
-    __syncwarp();
+    for (int j = lane; j < p; j += T::NT) ws.z[j] = ws.x[j] + ws.q[j];
+    T::sync();
 }
 
 struct ShrinkArgsW {
@@ -1267,24 +1292,26 @@ struct ShrinkArgsW {
 
 // shrink_gene: beta_init +-0.1, scale max(f(0), 1), m = 10 two-loop direction, dcsrch with maxls 20, the update skip, the restarts,
 // ftol = gtol = 1e-8 and the evaluation budget; no grid fallback (two-column designs only)
-__global__ void __launch_bounds__(32) k_wide_lfc_shrink(const __grid_constant__ ShrinkArgsW a) {
+template <int W>
+__global__ void __launch_bounds__(32 * W, W == 1 ? 0 : 1) k_wide_lfc_shrink(const __grid_constant__ ShrinkArgsW a) {
+    using T = Team<W>;
     extern __shared__ __align__(16) double wsm[];
-    const int g = blockIdx.x, p = a.b.p, lane = lane_id();
-    ShrinkWs ws = carve_shrink(wsm, p);
+    const int g = blockIdx.x, p = a.b.p, lane = T::tid();
+    ShrinkWs ws = carve_shrink<W>(wsm, p);
     const DesignS d = design_of(a.b.pack, a.b.N, p);
     const ShrinkParams prm = a.prm;
     const int64_t* y = a.counts + g;
     const double size = a.size[g], lsize = log(size);
     const double ftol = 1e-8, gtol = 1e-8;
-    wfill(ws.x, p, 0.0);
-    __syncwarp();
-    double f = shrink_eval_w(d, p, prm, y, a.ld, size, lsize, ws.x, nullptr, ws);
+    wfill<W>(ws.x, p, 0.0);
+    T::sync();
+    double f = shrink_eval_w<W>(d, p, prm, y, a.ld, size, lsize, ws.x, nullptr, ws);
     const double cnst = (f < 1.0) ? 1.0 : f;  // np.maximum(scale_cnst, 1)
-    for (int j = lane; j < p; j += 32) ws.x[j] = (j & 1) ? -0.1 : 0.1;
-    __syncwarp();
-    f = shrink_eval_w(d, p, prm, y, a.ld, size, lsize, ws.x, ws.g, ws) / cnst;
-    for (int j = lane; j < p; j += 32) ws.g[j] = ws.g[j] / cnst;
-    __syncwarp();
+    for (int j = lane; j < p; j += T::NT) ws.x[j] = (j & 1) ? -0.1 : 0.1;
+    T::sync();
+    f = shrink_eval_w<W>(d, p, prm, y, a.ld, size, lsize, ws.x, ws.g, ws) / cnst;
+    for (int j = lane; j < p; j += T::NT) ws.g[j] = ws.g[j] / cnst;
+    T::sync();
 
     int col = 0, head = 0;
     double theta = 1.0;
@@ -1294,20 +1321,20 @@ __global__ void __launch_bounds__(32) k_wide_lfc_shrink(const __grid_constant__ 
     bool active = true, ok = false;
 
     auto set_trial = [&]() {  // xt = t + stp dir (z itself at stp = 1)
-        for (int j = lane; j < p; j += 32) ws.xt[j] = (stp == 1.0) ? ws.z[j] : fma(stp, ws.dir[j], ws.t[j]);
-        __syncwarp();
+        for (int j = lane; j < p; j += T::NT) ws.xt[j] = (stp == 1.0) ? ws.z[j] : fma(stp, ws.dir[j], ws.t[j]);
+        T::sync();
     };
     // prepares the next line search from (x, f, g); returns false on ABNORMAL_TERMINATION_IN_LNSRCH
     auto begin_iteration = [&]() -> bool {
         for (;;) {
-            lbfgs_point_w(p, col, head, theta, ws);
-            for (int j = lane; j < p; j += 32) ws.dir[j] = ws.z[j] - ws.x[j];
-            __syncwarp();
-            const double dtd = wdot(ws.dir, ws.dir, p), gd = wdot(ws.g, ws.dir, p);
+            lbfgs_point_w<W>(p, col, head, theta, ws);
+            for (int j = lane; j < p; j += T::NT) ws.dir[j] = ws.z[j] - ws.x[j];
+            T::sync();
+            const double dtd = wdot<W>(ws.dir, ws.dir, p), gd = wdot<W>(ws.g, ws.dir, p);
             stp = (nit == 0) ? fmin(1.0 / sqrt(dtd), kLsStpMax) : 1.0;
-            wcopy(ws.t, ws.x, p);
-            wcopy(ws.r, ws.g, p);
-            __syncwarp();
+            wcopy<W>(ws.t, ws.x, p);
+            wcopy<W>(ws.r, ws.g, p);
+            T::sync();
             fold = f;
             gdold = gd;
             iback = 0;
@@ -1324,25 +1351,25 @@ __global__ void __launch_bounds__(32) k_wide_lfc_shrink(const __grid_constant__ 
         }
     };
 
-    if (wmaxabs(ws.g, p) <= gtol) {
+    if (wmaxabs<W>(ws.g, p) <= gtol) {
         ok = true;
         active = false;
     }
     if (active && !begin_iteration()) active = false;
     for (int ev = 0; ev < kShrinkMaxEval && active; ++ev) {
-        const double ft = shrink_eval_w(d, p, prm, y, a.ld, size, lsize, ws.xt, ws.gt, ws);
+        const double ft = shrink_eval_w<W>(d, p, prm, y, a.ld, size, lsize, ws.xt, ws.gt, ws);
         f = ft / cnst;
-        for (int j = lane; j < p; j += 32) {
+        for (int j = lane; j < p; j += T::NT) {
             ws.g[j] = ws.gt[j] / cnst;
             ws.x[j] = ws.xt[j];
         }
-        __syncwarp();
-        const double gd = wdot(ws.g, ws.dir, p);
+        T::sync();
+        const double gd = wdot<W>(ws.g, ws.dir, p);
         if (dcsrch_step(ls, stp, f, gd)) {  // another trial point
             if (++iback >= kShrinkMaxLs) {  // line search failed: restore, restart from steepest descent or give up
-                wcopy(ws.x, ws.t, p);
-                wcopy(ws.g, ws.r, p);
-                __syncwarp();
+                wcopy<W>(ws.x, ws.t, p);
+                wcopy<W>(ws.g, ws.r, p);
+                T::sync();
                 f = fold;
                 if (col == 0) {
                     active = false;
@@ -1359,7 +1386,7 @@ __global__ void __launch_bounds__(32) k_wide_lfc_shrink(const __grid_constant__ 
         }
         // ---- new iterate
         ++nit;
-        if (wmaxabs(ws.g, p) <= gtol || (fold - f) <= ftol * fmax(fmax(fabs(fold), fabs(f)), 1.0)) {
+        if (wmaxabs<W>(ws.g, p) <= gtol || (fold - f) <= ftol * fmax(fmax(fabs(fold), fabs(f)), 1.0)) {
             ok = true;
             active = false;
             continue;
@@ -1370,11 +1397,11 @@ __global__ void __launch_bounds__(32) k_wide_lfc_shrink(const __grid_constant__ 
         }
         // memory update (skipped when the curvature s'y is not safely positive); y = g - r
         double rr = 0.0;
-        for (int j = lane; j < p; j += 32) {
+        for (int j = lane; j < p; j += T::NT) {
             const double yj = ws.g[j] - ws.r[j];
             rr = fma(yj, yj, rr);
         }
-        rr = wsum(rr);
+        rr = T::sum(rr);
         const double dr = (stp == 1.0) ? (gd - gdold) : (gd - gdold) * stp;
         const double ddum = (stp == 1.0) ? -gdold : -gdold * stp;
         if (dr > 2.220446049250313e-16 * ddum) {
@@ -1387,26 +1414,29 @@ __global__ void __launch_bounds__(32) k_wide_lfc_shrink(const __grid_constant__ 
                 head = (head + 1) % kShrinkMem;
             }
             double *Ss = ws.S + slot * p, *Ys = ws.Y + slot * p;
-            for (int j = lane; j < p; j += 32) {
+            for (int j = lane; j < p; j += T::NT) {
                 Ss[j] = (stp == 1.0) ? ws.dir[j] : stp * ws.dir[j];
                 Ys[j] = ws.g[j] - ws.r[j];
             }
-            __syncwarp();
-            const double sy = wdot(Ys, Ss, p);
+            T::sync();
+            const double sy = wdot<W>(Ys, Ss, p);
             if (lane == 0) ws.sy[slot] = sy;
-            __syncwarp();
+            T::sync();
             theta = rr / dr;
         }
         if (!begin_iteration()) active = false;
     }
     // `active` still set: evaluation budget exhausted -> not converged
-    shrink_inv_hessian_w(d, p, prm, y, a.ld, size, lsize, ws.x, a.ih + (int64_t)g * p * p, ws);
-    for (int j = lane; j < p; j += 32) a.beta[(int64_t)g * p + j] = ws.x[j];
+    shrink_inv_hessian_w<W>(d, p, prm, y, a.ld, size, lsize, ws.x, a.ih + (int64_t)g * p * p, ws);
+    for (int j = lane; j < p; j += T::NT) a.beta[(int64_t)g * p + j] = ws.x[j];
     if (lane == 0) {
         a.conv[g] = ok ? 1.0 : 0.0;
         a.status[g] = kShrinkOk;
     }
 }
+// instantiated here, not at its launcher, so that the module lists the kernels in the order ptxas was given them before the team
+// widths existed: ptxas's register assignment depends on that order, and with it every other kernel keeps its code
+template __global__ void k_wide_lfc_shrink<1>(const __grid_constant__ ShrinkArgsW a);
 
 // ---------------------------------------------------------------------------------------------
 // launch helpers
@@ -1470,20 +1500,26 @@ int put_wald(const LaunchCfg& c, const DesignDev& d, const double* ridge, const 
     return put_dev(c, buf, contrast ? t + p : t, d.wald_dev);
 }
 
-// warps per gene of the 65..128 tier: the fewest of 2, 4, 8 that keep 8 warps on an SM, given how many blocks the workspace lets
-// share one (228 KB of shared memory per SM, 1 KB of it reserved per block).  That is 2 at p = 65 (four blocks), 4 at p = 81 (two)
-// and 8 from p = 101 on (one): the fastest of the three at each of those widths (DESIGN.md §5)
-int large_warps(int p) {
+inline size_t shrink_ws_bytes(int p, int W) { return shrink_ws_doubles(p, W) * sizeof(double); }
+using WsBytes = size_t (*)(int p, int W);
+
+// warps per gene of the 65..128 tier for a kernel whose workspace takes ws(p, W) bytes: the fewest of 2, 4, 8 that keep 8 warps
+// on an SM, given how many blocks the workspace lets share one (228 KB of shared memory per SM, 1 KB of it reserved per block).
+// For the fit kernels (ws_bytes) that is 2 at p = 65 (four blocks), 4 at p = 81 (two) and 8 from p = 101 on (one): the fastest of
+// the three at each of those widths (DESIGN.md §5).  For apeGLM shrinkage (shrink_ws_bytes) it is 2 at p = 65, 4 at 81 and 101,
+// 8 at 128.
+int large_warps(int p, WsBytes ws) {
     for (int W = 2; W < 8; W *= 2)
-        if ((int)(228 * 1024 / (ws_bytes(p, W) + 1024)) * W >= 8) return W;
+        if ((int)(228 * 1024 / (ws(p, W) + 1024)) * W >= 8) return W;
     return 8;
 }
 
 // the team width of a design: one warp up to PDQ_MAX_P_WIDE columns, above that DesignDev::warps (a tuning hook) or large_warps
+// for the kernel's workspace
 template <class F>
-int with_warps(const DesignDev& d, F&& f) {
+int with_warps(const DesignDev& d, F&& f, WsBytes ws = ws_bytes) {
     if (d.p <= PDQ_MAX_P_WIDE) return f(std::integral_constant<int, 1>{});
-    switch (d.warps ? d.warps : large_warps(d.p)) {
+    switch (d.warps ? d.warps : large_warps(d.p, ws)) {
         case 2: return f(std::integral_constant<int, 2>{});
         case 4: return f(std::integral_constant<int, 4>{});
         default: return f(std::integral_constant<int, 8>{});
@@ -1600,15 +1636,20 @@ int launch_cooks_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* cou
 int launch_lfc_shrink_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* size,
                            double prior_no_shrink_scale, double prior_scale, int shrink_index, double* beta, double* inv_hessian,
                            double* conv, int* status) {
-    if (d.p > PDQ_MAX_P_WIDE) return PDQ_ERR_UNSUPPORTED;  // one warp per gene only (pdq_api.cu refuses these designs first)
     if (shrink_index < 0 || shrink_index >= d.p) return PDQ_ERR_INVALID;
     const ShrinkArgsW a{base_of(d, G), ShrinkParams{1.0 / (prior_no_shrink_scale * prior_no_shrink_scale), prior_scale * prior_scale, shrink_index},
                         counts, ld, size, beta, inv_hessian, conv, status};
-    const size_t smem = shrink_ws_doubles(d.p) * sizeof(double);
-    if (int e = prep(k_wide_lfc_shrink, smem)) return e;
-    k_wide_lfc_shrink<<<G, 32, smem, c.stream>>>(a);
-    if (int e = check_launch()) return e;
-    return 1;
+    return with_warps(
+        d,
+        [&](auto tw) {
+            constexpr int W = decltype(tw)::value;
+            const size_t smem = shrink_ws_bytes(d.p, W);
+            if (int e = prep(k_wide_lfc_shrink<W>, smem)) return e;
+            k_wide_lfc_shrink<W><<<G, 32 * W, smem, c.stream>>>(a);
+            if (int e = check_launch()) return e;
+            return 1;
+        },
+        shrink_ws_bytes);
 }
 
 }  // namespace pdq

@@ -113,7 +113,7 @@ class _CudaOps:
     """Raw ops on numpy buffers through the C ABI (host-buffer entry points)."""
 
     def __init__(self, device=0, lanes_per_gene=0, pinned_outputs=True, ctx=None, wide_designs=False, wide_shrink=False,
-                 large_designs=False):
+                 large_designs=False, large_shrink=False):
         self.ctx = ctx if ctx is not None else _lib.Context(device)  # ctx: share an existing context (its device and stream)
         self.lib = self.ctx.lib
         self.pinned_outputs = pinned_outputs
@@ -127,6 +127,8 @@ class _CudaOps:
             self.ctx.set_wide_shrink(True)
         if large_designs:
             self.ctx.set_large_designs(True)
+        if large_shrink:
+            self.ctx.set_large_shrink(True)
 
     @property
     def max_p(self):
@@ -279,22 +281,30 @@ class B200Inference(_InferenceBase):
     large_designs : bool
         Also fit designs of 65 to 128 columns (paired designs of up to 127 subjects) on the large-design kernels.  Needs
         ``wide_designs=True``.  Off by default: such designs then raise ``B200Error`` ("p <= 64") as before.  apeGLM
-        shrinkage of these designs is not implemented and raises ``B200Error`` either way.
+        shrinkage of these designs needs ``large_shrink=True`` as well, and raises ``B200Error`` ("not implemented") without it.
+    large_shrink : bool
+        Also run apeGLM shrinkage of designs of 65 to 128 columns on the GPU, on a kernel in which several warps own one gene.
+        Needs ``wide_designs=True``, ``wide_shrink=True`` and ``large_designs=True``.  Off by default: shrinking such a design
+        then raises ``B200Error`` ("not implemented") as before.  Designs of up to 64 columns are not affected.
     """
 
     _TRACED = ("lin_reg_mu", "irls", "alpha_mle", "wald_test", "wald_tests", "fit_rough_dispersions", "fit_moments_dispersions",
                "dispersion_trend_gamma_glm", "lfc_shrink_nbinom_glm", "size_factors", "calculate_cooks", "adjust_pvalues")
 
     def __init__(self, device: int = 0, n_cpus: int | None = None, lanes_per_gene: int = 0, _ops=None, trace: bool = False,
-                 pinned_outputs: bool = True, wide_designs: bool = False, wide_shrink: bool = False, large_designs: bool = False):
+                 pinned_outputs: bool = True, wide_designs: bool = False, wide_shrink: bool = False, large_designs: bool = False,
+                 large_shrink: bool = False):
         if wide_shrink and not wide_designs:
             raise ValueError("wide_shrink=True needs wide_designs=True")
         if large_designs and not wide_designs:
             raise ValueError("large_designs=True needs wide_designs=True")
+        if large_shrink and not (wide_shrink and large_designs):
+            raise ValueError("large_shrink=True needs wide_designs=True, wide_shrink=True and large_designs=True")
         # pinned_outputs: large results are returned in page-locked numpy blocks (full-rate device-to-host copies, and full-rate
         # uploads when the caller hands them back); False returns ordinary pageable arrays
         self._ops = _ops if _ops is not None else _CudaOps(device, lanes_per_gene, pinned_outputs, wide_designs=wide_designs,
-                                                                     wide_shrink=wide_shrink, large_designs=large_designs)
+                                                                     wide_shrink=wide_shrink, large_designs=large_designs,
+                                                                     large_shrink=large_shrink)
         self._n_cpus = n_cpus or 1
         self.last_irls_fallbacks = 0
         # per-call tracing (the reference prints wall-clock per phase to stderr, dds.py:626-711 ...; a backend is better served by

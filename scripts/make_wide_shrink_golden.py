@@ -1,5 +1,6 @@
 """Generate tests/golden/wide_shrink_*.npz from the REAL reference: apeGLM shrinkage (``lfc_shrink_nbinom_glm``) of designs of 17..64
-columns.  TEST INFRASTRUCTURE: writes only the ``wide_shrink_*`` fixtures, every other golden stays untouched.
+columns.  TEST INFRASTRUCTURE: writes only the ``wide_shrink_*`` fixtures, every other golden stays untouched.  ``gen_calls`` and
+``gen_tape`` take the output prefix, so scripts/make_large_shrink_golden.py writes the ``large_shrink*`` fixtures with them.
 
     PYDESEQ2_SRC=<PyDESeq2 0.5.3 checkout> python scripts/make_wide_shrink_golden.py
 
@@ -49,7 +50,7 @@ def _counted_minimize():
     return seen, lambda: setattr(ut, "minimize", inner)
 
 
-def gen_calls(name, source, shrink_index, adapt=True):
+def gen_calls(name, source, shrink_index, adapt=True, prefix="wide_"):
     z = np.load(os.path.join(mg.OUT, f"{source}.npz"))
     counts, X = np.asarray(z["counts"], dtype=np.int64), np.asarray(z["design"], dtype=float)
     assert z["contrast"][shrink_index] == 1.0 and np.count_nonzero(z["contrast"]) == 1, "the stored SEs must be those of shrink_index"
@@ -71,17 +72,18 @@ def gen_calls(name, source, shrink_index, adapt=True):
     head = min(HEAD, HEAD_BYTES // (8 * p * p))
     assert len(seen) == G, (len(seen), G)
     nit, nfev = np.array(seen, dtype=np.int64).T
-    np.savez_compressed(os.path.join(mg.OUT, f"wide_shrink_{name}.npz"), counts=counts, X=X, size=size, offset=offset, mle_lfc=mle_lfc,
+    np.savez_compressed(os.path.join(mg.OUT, f"{prefix}shrink_{name}.npz"), counts=counts, X=X, size=size, offset=offset, mle_lfc=mle_lfc,
                         mle_se=mle_se, prior_var=np.float64(prior_var), prior_scale=np.float64(prior_scale),
                         prior_no_shrink_scale=np.float64(15.0), shrink_index=np.int64(shrink_index), lfcs=lfcs,
                         inv_hessians_head=np.ascontiguousarray(ih[:head]), inv_hessian_col=np.ascontiguousarray(ih[:, :, shrink_index]),
                         converged=np.asarray(conv, dtype=float), nit=nit, nfev=nfev)
-    print(f"wide_shrink_{name}: G={G} p={X.shape[1]} idx={shrink_index} prior_scale={prior_scale:.4g} "
+    print(f"{prefix}shrink_{name}: G={G} p={X.shape[1]} idx={shrink_index} prior_scale={prior_scale:.4g} "
           f"converged={np.mean(conv):.3f} nfev median {int(np.median(nfev))} max {int(nfev.max())}")
 
 
-def gen_tape(name, source, coeff_idx):
-    """deseq2() + summary() + lfc_shrink(coeff) through the real orchestrator on the counts and design of a wide_* fixture."""
+def gen_tape(name, source, coeff_idx, prefix="wide_"):
+    """deseq2() + summary() + lfc_shrink(coeff) through the real orchestrator on the counts and design of a wide_* / large_*
+    fixture."""
     from pydeseq2.ds import DeseqStats
 
     z = np.load(os.path.join(mg.OUT, f"{source}.npz"))
@@ -118,9 +120,9 @@ def gen_tape(name, source, coeff_idx):
                prior_var=np.float64(prior_var), final_log2FoldChange=shr_log2, final_lfcSE=shr_se, converged=np.asarray(conv, dtype=float),
                mle_log2FoldChange=mle_log2, results_log2FoldChange=res["log2FoldChange"].values, results_lfcSE=res["lfcSE"].values,
                results_pvalue=res["pvalue"].values, results_padj=res["padj"].values, results_baseMean=res["baseMean"].values)
-    np.savez_compressed(os.path.join(mg.OUT, f"wide_shrinktape_{name}.npz"), **out)
+    np.savez_compressed(os.path.join(mg.OUT, f"{prefix}shrinktape_{name}.npz"), **out)
     same = np.allclose(out["results_log2FoldChange"], shr_log2, equal_nan=True, rtol=0, atol=0)
-    print(f"wide_shrinktape_{name}: G={counts.shape[1]} p={X.shape[1]} idx={coeff_idx} prior_scale={float(k['prior_scale']):.4g} "
+    print(f"{prefix}shrinktape_{name}: G={counts.shape[1]} p={X.shape[1]} idx={coeff_idx} prior_scale={float(k['prior_scale']):.4g} "
           f"results_df holds the shrunk column: {same}")
 
 
