@@ -141,6 +141,11 @@ int pdq_host_free(pdq_ctx* ctx, void* hptr);
 int pdq_memcpy_h2d(pdq_ctx* ctx, void* dst, const void* src, size_t bytes); /* async on ctx stream */
 int pdq_memcpy_d2h(pdq_ctx* ctx, void* dst, const void* src, size_t bytes); /* async on ctx stream */
 int pdq_memcpy_d2d(pdq_ctx* ctx, void* dst, const void* src, size_t bytes); /* async on ctx stream */
+/* Device-to-host copy on a side branch of the ctx stream: ordered behind the work enqueued before it, overlapping the work
+ * enqueued after it.  pdq_side_join orders the ctx stream behind every side copy since the previous join; call it before the
+ * stream is synchronised or a capture ends (a captured pass then holds the copy as a branch of its graph). */
+int pdq_memcpy_d2h_side(pdq_ctx* ctx, void* dst, const void* src, size_t bytes);
+int pdq_side_join(pdq_ctx* ctx);
 /* async on ctx stream: `count` elements of `elem_bytes`, `src_stride` bytes apart on the device, packed into `dst` */
 int pdq_memcpy_d2h_strided(pdq_ctx* ctx, void* dst, const void* src, size_t elem_bytes, size_t src_stride, size_t count);
 int pdq_memset(pdq_ctx* ctx, void* dst, int value, size_t bytes);
@@ -361,6 +366,13 @@ int pdq_mom_dispersions_dev(pdq_ctx* ctx, const pdq_design* design, const int64_
                             double* normed_mean_out, double min_mu,
                             double* mu_hat_out /* (N,G), may be NULL: also the lin_reg_mu result, same projection */,
                             int64_t ld_mu);
+/* pdq_mom_dispersions_dev with mu_hat (the lin_reg_mu branch) followed by the genewise pdq_alpha_mle_hint_dev (alpha_hat = the
+ * start values, cr_reg on, no prior, no hint_in) as ONE persistent launch: each gene's start value and means are computed and
+ * stored, then searched from, by the same lanes.  Same outputs, bit for bit; `hint_out` may be NULL.  Where a warp of the search
+ * would work on more than 12 gene tiles, and for designs of more than PDQ_MAX_P columns, the two launches. */
+int pdq_mom_alpha_mle_dev(pdq_ctx* ctx, const pdq_design* design, const int64_t* counts, int64_t ld, int G, double min_disp,
+                          double max_disp, double min_mu, double* mom_out, double* normed_mean_out, double* mu_hat_out,
+                          int64_t ld_mu, double* alpha_out, double* converged_out, double* hint_out);
 /* Parametric dispersion trend INCLUDING the caller's outer loop (dds.py:1199-1275: fit, drop genes with
  * genewise/fitted outside [1e-4, 15), refit until sum(log(c/c_old)^2) < 1e-6) AND the dispersion prior
  * (dds.py:840-884: squared scaled MAD of the log residuals, prior variance), entirely on the device in one launch of
@@ -404,6 +416,12 @@ int pdq_gather_columns_dev(pdq_ctx* ctx, const double* in, int64_t ld_in, int N,
 int pdq_column_sums_dev(pdq_ctx* ctx, const int64_t* counts, int64_t ld, int N, int G, double* sums_out);
 int pdq_scatter_rows_dev(pdq_ctx* ctx, const double* in, double* out, const int* perm_dev, int n, int nvec, int64_t stride,
                          int width);
+/* Up to 16 segments of one buffer in one launch.  `seg` (host) holds `nseg` rows (offset in doubles, rows, width, permuted):
+ * out[offset + j * width + k] = in[offset + src[j] * width + k] for j < rows, k < width (src_dev: for each output row the row it
+ * comes from, e.g. the device column of each caller-order gene), or row j from row j when `permuted` is 0 (src_dev may then be
+ * NULL).  `out` is device memory or page-locked host memory (pdq_host_alloc): the kernel then writes the host block directly,
+ * with no copy behind it; it is complete when the stream reaches the work enqueued after the call. */
+int pdq_scatter_segments_dev(pdq_ctx* ctx, const double* in, double* out, const int* src_dev, int nseg, const int64_t* seg);
 int pdq_select_dispersions_dev(pdq_ctx* ctx, const double* genewise, const double* map, const double* fitted,
                                const double* trend_out16, size_t n, double min_disp, double max_disp,
                                double* disp_out, double* outlier_out);

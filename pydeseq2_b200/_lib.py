@@ -65,6 +65,8 @@ _SIGNATURES = {
     "pdq_memcpy_d2h": (C.c_int, [c_ctx, C.c_void_p, c_dptr, C.c_size_t]),
     "pdq_memcpy_d2h_strided": (C.c_int, [c_ctx, C.c_void_p, c_dptr, C.c_size_t, C.c_size_t, C.c_size_t]),
     "pdq_memcpy_d2d": (C.c_int, [c_ctx, c_dptr, c_dptr, C.c_size_t]),
+    "pdq_memcpy_d2h_side": (C.c_int, [c_ctx, C.c_void_p, c_dptr, C.c_size_t]),
+    "pdq_side_join": (C.c_int, [c_ctx]),
     "pdq_memset": (C.c_int, [c_ctx, c_dptr, C.c_int, C.c_size_t]),
     "pdq_sync": (C.c_int, [c_ctx]),
     "pdq_event_record": (C.c_int, [c_ctx, C.c_int]),
@@ -105,6 +107,8 @@ _SIGNATURES = {
                                     C.c_int, c_dptr, c_dptr, c_dptr]),
     "pdq_mom_dispersions_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, C.c_double, C.c_double, c_dptr,
                                           c_dptr, C.c_double, c_dptr, C.c_int64]),
+    "pdq_mom_alpha_mle_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, C.c_double, C.c_double, C.c_double, c_dptr,
+                                        c_dptr, c_dptr, C.c_int64, c_dptr, c_dptr, c_dptr]),
     "pdq_calculate_cooks": (C.c_int, [c_ctx, i64p, C.c_int64, C.c_int, C.c_int, f64p, f64p, C.c_int, f64p, f64p, C.c_int64,
                                       C.c_double, f64p, f64p, f64p, f64p]),
     "pdq_cooks_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int64, C.c_int, c_dptr, c_dptr, C.c_int64, C.c_double, c_dptr,
@@ -133,6 +137,7 @@ _SIGNATURES = {
     "pdq_gather_columns_dev": (C.c_int, [c_ctx, c_dptr, C.c_int64, C.c_int, c_dptr, C.c_int, c_dptr, C.c_int64]),
     "pdq_column_sums_dev": (C.c_int, [c_ctx, c_dptr, C.c_int64, C.c_int, C.c_int, c_dptr]),
     "pdq_scatter_rows_dev": (C.c_int, [c_ctx, c_dptr, c_dptr, c_dptr, C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "pdq_scatter_segments_dev": (C.c_int, [c_ctx, c_dptr, c_dptr, c_dptr, C.c_int, i64p]),
     "pdq_select_dispersions_dev": (C.c_int, [c_ctx, c_dptr, c_dptr, c_dptr, c_dptr, C.c_size_t, C.c_double, C.c_double, c_dptr,
                                              c_dptr]),
     "pdq_mu_from_lfc_dev": (C.c_int, [c_ctx, c_design, c_dptr, C.c_int, c_dptr, C.c_int64]),
@@ -267,6 +272,15 @@ class Context:
     def d2h(self, arr: np.ndarray, dptr):
         assert arr.flags.c_contiguous
         self.check(self.lib.pdq_memcpy_d2h(self.h, arr.ctypes.data_as(C.c_void_p), c_dptr(dptr), arr.nbytes))
+
+    def d2h_side(self, arr: np.ndarray, dptr):
+        """Like :meth:`d2h`, on a branch of the stream that overlaps the work enqueued after it; :meth:`side_join` ends the branch."""
+        assert arr.flags.c_contiguous
+        self.check(self.lib.pdq_memcpy_d2h_side(self.h, arr.ctypes.data_as(C.c_void_p), c_dptr(dptr), arr.nbytes))
+
+    def side_join(self):
+        """Order the stream behind every :meth:`d2h_side` copy since the previous join."""
+        self.check(self.lib.pdq_side_join(self.h))
 
     def d2h_strided(self, arr: np.ndarray, dptr, stride: int):
         """arr[i] = the element at dptr + i * stride bytes (one element per `stride` bytes of device memory)."""

@@ -159,6 +159,9 @@ struct pdq_ctx {
     void* grid_scratch = nullptr;  // accumulators of the grid-wide trend fit
     cudaStream_t pstream[2] = {nullptr, nullptr};  // gene-block pipeline of the host-buffer entry points
     cudaEvent_t pfork = nullptr, pjoin[2] = {nullptr, nullptr};
+    cudaStream_t cstream = nullptr;  // side copies of the resident pass (pdq_memcpy_d2h_side): a branch that rejoins `stream`
+    cudaEvent_t cfork = nullptr, cjoin = nullptr;
+    bool side_pending = false;       // a side copy was enqueued since the last pdq_side_join
     int pipeline = 4;        // gene blocks per pipelined call; PDQ_PIPELINE=0 disables
     int debug = 0;           // PDQ_DEBUG_* test hooks
     int wide = 0;            // designs of up to PDQ_MAX_P_WIDE columns (pdq_set_wide_designs)
@@ -298,7 +301,10 @@ extern "C" int pdq_ctx_create(int device, pdq_ctx** out) {
         cudaStreamCreateWithFlags(&c->pstream[1], cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->pfork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->pjoin[0], cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->pjoin[1], cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreateWithFlags(&c->pjoin[1], cudaEventDisableTiming) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&c->cstream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&c->cfork, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&c->cjoin, cudaEventDisableTiming) != cudaSuccess) {
         delete c;
         return PDQ_ERR_CUDA;
     }
@@ -329,6 +335,9 @@ extern "C" void pdq_ctx_destroy(pdq_ctx* c) {
     if (c->pfork) cudaEventDestroy(c->pfork);
     for (auto& ev : c->pjoin)
         if (ev) cudaEventDestroy(ev);
+    if (c->cstream) cudaStreamDestroy(c->cstream);
+    if (c->cfork) cudaEventDestroy(c->cfork);
+    if (c->cjoin) cudaEventDestroy(c->cjoin);
     for (int i = 0; i < 2; ++i) {
         if (c->stage[i]) cudaFreeHost(c->stage[i]);
         if (c->stage_ev[i]) cudaEventDestroy(c->stage_ev[i]);
@@ -439,6 +448,25 @@ extern "C" int pdq_memcpy_d2h(pdq_ctx* c, void* dst, const void* src, size_t byt
 extern "C" int pdq_memcpy_d2h_strided(pdq_ctx* c, void* dst, const void* src, size_t elem_bytes, size_t src_stride, size_t count) {
     if (!c || elem_bytes == 0 || src_stride < elem_bytes) return PDQ_ERR_INVALID;
     if (count) CU(c, cudaMemcpy2DAsync(dst, elem_bytes, src, src_stride, elem_bytes, count, cudaMemcpyDeviceToHost, c->stream));
+    return PDQ_OK;
+}
+// A device-to-host copy on a branch of the context's stream: it starts behind the work enqueued so far and runs while the work
+// enqueued after it does; pdq_side_join puts the stream behind every side copy since the last join.  Under stream capture the
+// pair becomes a branch of the graph.
+extern "C" int pdq_memcpy_d2h_side(pdq_ctx* c, void* dst, const void* src, size_t bytes) {
+    if (!c) return PDQ_ERR_INVALID;
+    CU(c, cudaEventRecord(c->cfork, c->stream));
+    CU(c, cudaStreamWaitEvent(c->cstream, c->cfork, 0));
+    CU(c, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->cstream));
+    c->side_pending = true;
+    return PDQ_OK;
+}
+extern "C" int pdq_side_join(pdq_ctx* c) {
+    if (!c) return PDQ_ERR_INVALID;
+    if (!c->side_pending) return PDQ_OK;  // nothing to join (and under capture the side stream may not be part of the graph)
+    c->side_pending = false;
+    CU(c, cudaEventRecord(c->cjoin, c->cstream));
+    CU(c, cudaStreamWaitEvent(c->stream, c->cjoin, 0));
     return PDQ_OK;
 }
 extern "C" int pdq_memcpy_d2d(pdq_ctx* c, void* dst, const void* src, size_t bytes) {
@@ -852,6 +880,33 @@ extern "C" int pdq_mom_dispersions_dev(pdq_ctx* c, const pdq_design* d, const in
                 "mom_dispersions");
 }
 
+extern "C" int pdq_mom_alpha_mle_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, double min_disp,
+                                     double max_disp, double min_mu, double* mom, double* normed_mean, double* mu_hat, int64_t ld_mu,
+                                     double* alpha, double* conv, double* hint_out) {
+    CHECK_CTX(c);
+    if (!d || !counts || !mom || !normed_mean || !mu_hat || !alpha || !conv || G <= 0 || ld < G || ld_mu < G)
+        return fail(c, PDQ_ERR_INVALID, "pdq_mom_alpha_mle_dev: bad arguments");
+    if (d->d.N == d->d.p) return fail(c, PDQ_ERR_INVALID, "The number of samples and the number of design variables are equal");
+    void* status;
+    if (int e = ensure(c, kBufStatus, (size_t)G * sizeof(int), &status)) return e;
+    // The fold pays where a warp works on few tiles per launch, as the MAP -> LFC hand-off does: the start values then run at the
+    // search's occupancy (3 blocks per SM) instead of their own, which costs more than the saved drain and ramp-up once the
+    // streaming is long.  Whole resident pass on H100: 3 % faster at C2 (3.2 tiles per resident search warp), 6 % slower at the C5
+    // shard (19.7) (DESIGN.md §5).  Above 12 tiles the two launches, as in pdq_map_irls_wald_dev.
+    const LaunchCfg lcfg = cfg(c, G, d->d.N);
+    if ((int64_t)(G + (32 >> lcfg.lgT) - 1) / (32 >> lcfg.lgT) > (int64_t)12 * 12 * lcfg.sm_count) {
+        if (int e = done(c, launch_mom_from_counts(lcfg, d->d, counts, ld, G, min_disp, max_disp, mom, normed_mean, min_mu, mu_hat, ld_mu),
+                         "mom_dispersions"))
+            return e;
+        return done(c, launch_alpha_mle(lcfg, d->d, counts, ld, G, mu_hat, ld_mu, mom, min_disp, max_disp, 1.0, nullptr, 1, 0, alpha, conv,
+                                        (int*)status, nullptr, hint_out),
+                    "alpha_mle");
+    }
+    return done(c, launch_mom_alpha(lcfg, d->d, counts, ld, G, min_disp, max_disp, min_mu, mom, normed_mean, mu_hat, ld_mu,
+                                    alpha, conv, (int*)status, hint_out),
+                "mom_alpha_mle");
+}
+
 extern "C" int pdq_mu_from_lfc_dev(pdq_ctx* c, const pdq_design* d, const double* lfc, int G, double* mu, int64_t ld_out) {
     CHECK_CTX(c);
     if (!d || !lfc || !mu || G <= 0 || ld_out < G) return fail(c, PDQ_ERR_INVALID, "pdq_mu_from_lfc_dev: bad arguments");
@@ -957,6 +1012,25 @@ extern "C" int pdq_scatter_rows_dev(pdq_ctx* c, const double* in, double* out, c
     CHECK_CTX(c);
     if (!in || !out || !perm_dev || n < 0 || nvec < 1 || width < 1 || stride < n) return fail(c, PDQ_ERR_INVALID, "pdq_scatter_rows_dev: bad arguments");
     return done(c, launch_scatter_rows(c->stream, in, out, perm_dev, n, nvec, stride, width), "scatter_rows");
+}
+
+extern "C" int pdq_scatter_segments_dev(pdq_ctx* c, const double* in, double* out, const int* src_dev, int nseg, const int64_t* seg) {
+    CHECK_CTX(c);
+    if (!in || !out || !seg || nseg < 1 || nseg > kMaxScatterSegs) return fail(c, PDQ_ERR_INVALID, "pdq_scatter_segments_dev: bad arguments");
+    for (int i = 0; i < nseg; ++i)
+        if (seg[4 * i] < 0 || seg[4 * i + 1] < 0 || seg[4 * i + 1] > INT32_MAX || seg[4 * i + 2] < 1 || seg[4 * i + 2] > INT32_MAX ||
+            (seg[4 * i + 3] && !src_dev))
+            return fail(c, PDQ_ERR_INVALID, "pdq_scatter_segments_dev: bad segment %d", i);
+    // page-locked host memory is written through its device address (the same pointer under unified addressing)
+    cudaPointerAttributes at{};
+    CU(c, cudaPointerGetAttributes(&at, out));
+    if (at.type == cudaMemoryTypeHost) {
+        if (!at.devicePointer) return fail(c, PDQ_ERR_INVALID, "pdq_scatter_segments_dev: host `out` is not mapped into the device");
+        out = static_cast<double*>(at.devicePointer);
+    } else if (at.type == cudaMemoryTypeUnregistered) {
+        return fail(c, PDQ_ERR_INVALID, "pdq_scatter_segments_dev: `out` is pageable host memory");
+    }
+    return done(c, launch_scatter_segments(c->stream, in, out, src_dev, nseg, seg), "scatter_segments");
 }
 
 extern "C" int pdq_select_dispersions_dev(pdq_ctx* c, const double* genewise, const double* map, const double* fitted,

@@ -108,6 +108,24 @@ int launch_mom_from_counts(const LaunchCfg& c, const DesignDev& d, const int64_t
     PDQ_ROUTE_WIDE(launch_mom_from_counts, d.p, c, d, counts, ld, G, min_disp, max_disp, alpha, normed_mean, min_mu, mu_hat, ld_mu)
 }
 
+#define DECL_MOMALPHA(sfx)                                                                                                \
+    int launch_mom_alpha##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, double, double, double, double*, \
+                              double*, double*, int64_t, double*, double*, int*, double*);
+PDQ_UNITS(DECL_MOMALPHA)
+int launch_mom_alpha(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp, double max_disp,
+                     double min_mu, double* mom, double* normed_mean, double* mu_hat, int64_t ld_mu, double* alpha, double* conv,
+                     int* status, double* hint_out) {
+    if (d.p > PDQ_MAX_P) {  // the wide-design kernels have no fold: the two launches, same results
+        const int n1 = launch_mom_from_counts(c, d, counts, ld, G, min_disp, max_disp, mom, normed_mean, min_mu, mu_hat, ld_mu);
+        if (n1 < 0) return n1;
+        const int n2 = launch_alpha_mle(c, d, counts, ld, G, mu_hat, ld_mu, mom, min_disp, max_disp, 1.0, nullptr, 1, 0, alpha, conv,
+                                        status, nullptr, hint_out);
+        return n2 < 0 ? n2 : n1 + n2;
+    }
+    PDQ_ROUTE(launch_mom_alpha, d.p, c, d, counts, ld, G, min_disp, max_disp, min_mu, mom, normed_mean, mu_hat, ld_mu, alpha, conv, status,
+              hint_out)
+}
+
 #define DECL_MULFC(sfx) int launch_mu_from_lfc##sfx(const LaunchCfg&, const DesignDev&, const double*, int, double*, int64_t);
 PDQ_UNITS_ALL(DECL_MULFC)
 int launch_mu_from_lfc(const LaunchCfg& c, const DesignDev& d, const double* lfc, int G, double* mu, int64_t ld_out) {

@@ -1488,9 +1488,10 @@ PDQ_UNROLL_P
 
 // Resident pipeline: rough + moments estimators, their min/clip (dds.py:1140-1162), the normalised mean (dds.py:708) and --
 // because lin_reg_mu is the SAME least-squares projection of counts/sf (utils.py:711-713 vs :846-848) -- optionally the
-// initial mu_hat = max(sf * X beta, min_mu) (utils.py:682-715), in two sweeps over the gene instead of six.
+// initial mu_hat = max(sf * X beta, min_mu) (utils.py:682-715), in two sweeps over the gene instead of six.  Returns the clipped
+// start value, the same in every lane of the group (k_mom_alpha hands it to the dispersion search in registers).
 template <int P>
-PDQ_HD void mom_fused_gene(const Group& grp, const DesignS& d, const SmallMat<P>& pinv, const int64_t* y, int64_t ld,
+PDQ_HD double mom_fused_gene(const Group& grp, const DesignS& d, const SmallMat<P>& pinv, const int64_t* y, int64_t ld,
                            double s_mean_inv, double min_disp, double max_disp, double min_mu, double* alpha_out,
                            double* mean_out, double* mu_out, int64_t ld_out, bool valid) {
     double v[P];
@@ -1542,12 +1543,13 @@ PDQ_UNROLL_P
     if (!(mde == mde)) mde = 0.0;  // np.nan_to_num
     else if (mde > 1.7976931348623157e308) mde = 1.7976931348623157e308;
     else if (mde < -1.7976931348623157e308) mde = -1.7976931348623157e308;
+    double a = (mde < rough) ? mde : rough;                                // np.minimum (dds.py:1158)
+    a = (a < min_disp) ? min_disp : ((a > max_disp) ? max_disp : a);       // np.clip (dds.py:1161)
     if (valid && grp.si == 0) {
-        double a = (mde < rough) ? mde : rough;                                // np.minimum (dds.py:1158)
-        a = (a < min_disp) ? min_disp : ((a > max_disp) ? max_disp : a);       // np.clip (dds.py:1161)
         *alpha_out = a;
         *mean_out = m;
     }
+    return a;
 }
 
 // returns the moments estimate; `mean_out` = per-gene mean of the normalised counts, `all_zero` flag

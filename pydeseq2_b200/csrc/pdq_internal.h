@@ -91,6 +91,12 @@ int launch_moments(const LaunchCfg&, const DesignDev&, const double* normed, int
 int launch_mom_from_counts(const LaunchCfg&, const DesignDev&, const int64_t* counts, int64_t ld, int G,
                            double min_disp, double max_disp, double* alpha, double* normed_mean, double min_mu, double* mu_hat,
                            int64_t ld_mu);
+// the lin_reg_mu branch's start values and the genewise dispersion search in one persistent launch (k_mom_alpha, then k_alpha_grid):
+// what launch_mom_from_counts followed by launch_alpha_mle (cr_reg on, no prior, alpha_hat = mom) writes, bit for bit.  `mu_hat`
+// is required.  LaunchCfg::tickets as for launch_map_irls.
+int launch_mom_alpha(const LaunchCfg&, const DesignDev&, const int64_t* counts, int64_t ld, int G, double min_disp, double max_disp,
+                     double min_mu, double* mom, double* normed_mean, double* mu_hat, int64_t ld_mu, double* alpha, double* conv,
+                     int* status, double* hint_out);
 int launch_mu_from_lfc(const LaunchCfg&, const DesignDev&, const double* lfc, int G, double* mu, int64_t ld_out);
 
 int launch_trend_fit(const LaunchCfg&, const double* x, const double* t, double* scratch3n, size_t n, int x_is_mean,
@@ -104,6 +110,9 @@ int launch_lfc_shrink(const LaunchCfg&, const DesignDev&, const int64_t* counts,
 int launch_gather_cols(cudaStream_t stream, const double* in, int64_t ld_in, int N, const int* idx, int R, double* out, int64_t ld_out);
 int launch_column_sums(cudaStream_t stream, const int64_t* counts, int64_t ld, int N, int G, double* sums);
 int launch_scatter_rows(cudaStream_t stream, const double* in, double* out, const int* perm, int n, int nvec, int64_t stride, int width);
+// `seg` (host): nseg rows of (offset in doubles, rows, width, permuted); see pdq_scatter_segments_dev
+constexpr int kMaxScatterSegs = 16;
+int launch_scatter_segments(cudaStream_t stream, const double* in, double* out, const int* src, int nseg, const int64_t* seg);
 int launch_hash(cudaStream_t stream, int sm_count, const void* dptr, size_t words, uint64_t* out2 /* device, zeroed */);
 int launch_fp64_peak(const LaunchCfg&, double* out /* sm_count * 8 * 256 doubles */, int iters, double* flop);
 int launch_size_factors(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, double* logmeans,

@@ -652,6 +652,63 @@ __global__ void __launch_bounds__(kBlock) k_mom_from_counts(const __grid_constan
                       a.mu_hat ? a.mu_hat + g : nullptr, a.ld_mu, valid);
 }
 
+// ---- method-of-moments start values folded into the genewise dispersion search (lin_reg_mu branch of the resident pass) --------
+// k_mom_from_counts and k_alpha_mle are per-gene functions with the same lane layout, and the search of a gene needs only that gene's
+// start value and initial means.  k_mom_alpha runs mom_fused_gene on each ticket tile and then alpha_gene on the same tile: the
+// start value stays in registers, and every lane reads back the means it has just stored.  One launch instead of a grid that drains
+// and a second that ramps up and reads the counts again; mom, means and mu_hat still go to HBM for the stages behind the search.
+// Control words (LaunchCfg::tickets + kFoldWords) are kept consistent by the kernel itself, as in k_map_irls: the last block zeroes
+// the ticket counter and moves the count of flagged genes to the word k_alpha_grid reads, so the launch needs no memset node.
+constexpr int kFoldWords = 25;  // offset of the control words in LaunchCfg::tickets (behind the words of k_map_irls)
+enum { kFoldTicket = 0, kFoldGridCnt = 1, kFoldBlocks = 2, kFoldGridOut = 3 };
+
+template <int P>
+struct MomAlphaArgs {
+    AlphaArgs<P> al;  // genewise search: al.mu = mu_hat, al.alpha_hat unused; al.ticket + 1 = the flagged-gene word of k_alpha_grid
+    SmallMat<P> pinv;
+    double s_mean_inv, min_disp, max_disp, min_mu;  // start values: clip bounds of dds.py:1161, floor of lin_reg_mu
+    double *mom, *means, *mu_hat;
+    int* words;  // control words above
+};
+
+template <int P, bool STAGED>
+__global__ void __launch_bounds__(kBlock, PDQ_ALPHA_MINB) k_mom_alpha(const __grid_constant__ MomAlphaArgs<P> a) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const DesignS d = stage_design_t<true, STAGED ? 1 : 0>(a.al.dv, P, smem);
+    Group grp;
+    int g;
+    bool valid;
+    const int gpw = 32 >> a.al.lgT;
+    double* psi = reinterpret_cast<double*>(smem + scratch_off(a.al.dv, true)) +
+                  (size_t)((threadIdx.x >> 5) * gpw + ((threadIdx.x & 31) & (gpw - 1))) * (2 * kPsiK);
+    int* ticket = a.words + kFoldTicket;
+    int ahead = draw_ticket(ticket);
+    while (next_tile(ticket, a.al.lgT, a.al.G, grp, g, valid, ahead, a.al.descending != 0)) {
+        const double alpha_hat = mom_fused_gene<P>(grp, d, a.pinv, a.al.counts + g, a.al.ld, a.s_mean_inv, a.min_disp, a.max_disp,
+                                                   a.min_mu, a.mom + g, a.means + g, a.mu_hat + g, a.al.ld_mu, valid);
+        // lanes of padding genes (clamped to gene G - 1) read the means another group of this warp has just stored
+        __syncwarp();
+        alpha_gene<P>(grp, d, a.al.prm, a.al.counts + g, a.al.ld, a.mu_hat + g, a.al.ld_mu, alpha_hat, a.al.alpha + g, a.al.conv + g,
+                      a.al.status + g, valid, psi, nullptr, a.al.hint_out ? a.al.hint_out + 2 * (int64_t)g : nullptr);
+        if (valid && grp.si == 0) {
+            if (a.al.force) {
+                a.al.status[g] = kAlphaNeedsGrid;
+                a.al.conv[g] = 0.0;
+            }
+            if (a.al.status[g] == kAlphaNeedsGrid) atomicAdd(a.words + kFoldGridCnt, 1);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        if (atomicAdd(a.words + kFoldBlocks, 1) == (int)gridDim.x - 1) {  // the kernel's last block
+            a.words[kFoldGridOut] = atomicExch(a.words + kFoldGridCnt, 0);
+            a.words[kFoldTicket] = 0;
+            a.words[kFoldBlocks] = 0;
+        }
+    }
+}
+
 template <int P>
 struct CooksArgs {
     DesignView dv;
@@ -1423,6 +1480,28 @@ __global__ void k_scatter_rows(const double* __restrict__ in, double* __restrict
     out[((int64_t)v * stride + perm[j]) * width + k] = in[((int64_t)v * stride + j) * width + k];
 }
 
+// Several (offset, rows, width) segments of one buffer in one launch, as a gather: out[off + j * width + k] = in[off + src[j] *
+// width + k], or row j from row j when the segment is not permuted (a record that rides along with the per-gene vectors).  Stores
+// are contiguous, so `out` may be page-locked host memory: the rows then cross the bus as full write bursts, with no copy node
+// behind the launch.  The segments' element counts are laid end to end over the grid; `start` holds their running sums.
+struct ScatterSegs {
+    int n;
+    int64_t off[kMaxScatterSegs], start[kMaxScatterSegs + 1];
+    int rows[kMaxScatterSegs], width[kMaxScatterSegs], permuted[kMaxScatterSegs];
+};
+
+__global__ void k_scatter_segments(const double* __restrict__ in, double* __restrict__ out, const int* __restrict__ src,
+                                   const __grid_constant__ ScatterSegs s) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= s.start[s.n]) return;
+    int i = 0;
+    while (t >= s.start[i + 1]) ++i;
+    const int64_t r = t - s.start[i];
+    const int w = s.width[i];
+    const int j = (int)(r / w), k = (int)(r - (int64_t)j * w);
+    out[s.off[i] + r] = in[s.off[i] + (int64_t)(s.permuted[i] ? src[j] : j) * w + k];
+}
+
 // ---- content checksum of a device buffer: the device half of the residency cache of pdq_api.cu (host_hash there computes the
 // same two wrapping sums with host threads).  HBM-bound.
 __global__ void __launch_bounds__(256) k_hash(const uint64_t* __restrict__ w, size_t n, unsigned long long* out) {
@@ -1659,6 +1738,35 @@ int PDQ_TUFN(launch_mom_from_counts)(const LaunchCfg& c, const DesignDev& d, con
     return 1;
 }
 
+int PDQ_TUFN(launch_mom_alpha)(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, double min_disp,
+                               double max_disp, double min_mu, double* mom, double* normed_mean, double* mu_hat, int64_t ld_mu,
+                               double* alpha, double* conv, int* status, double* hint_out) {
+    PDQ_DISPATCH_P(d.p, {
+        MomAlphaArgs<P> a;
+        int* words = c.tickets + kFoldWords;
+        // genewise search (cr_reg on, no prior); k_alpha_grid behind the launch reads the flagged-gene count at ticket[1] =
+        // the word the kernel's last block fills
+        a.al = AlphaArgs<P>{{d.pack, d.N, d.staged ? (int)(d.smem_bytes - 16) : 0}, AlphaParams{log(min_disp), log(max_disp), 1.0, 1, 0},
+                            counts, ld, G, c.lgT, mu_hat, ld_mu, mom, alpha, conv, status, nullptr, words + kFoldGridOut - 1,
+                            (c.debug & PDQ_DEBUG_FORCE_ALPHA_GRID) ? 1 : 0, nullptr, hint_out, alpha_descending()};
+        a.pinv = pinv_of<P>(d);
+        a.s_mean_inv = d.s_mean_inv; a.min_disp = min_disp; a.max_disp = max_disp; a.min_mu = min_mu;
+        a.mom = mom; a.means = normed_mean; a.mu_hat = mu_hat; a.words = words;
+        const size_t smem_alpha = d.smem_bytes + kMathTabBytes + (size_t)kWarps * (32 >> c.lgT) * 2 * kPsiK * sizeof(double);
+        if (int e = prep(k_alpha_grid<P>, d.smem_bytes)) return e;
+        if (d.staged) {
+            if (int e = prep(k_mom_alpha<P, true>, smem_alpha)) return e;
+            k_mom_alpha<P, true><<<persistent_grid(k_mom_alpha<P, true>, smem_alpha, c.sm_count, G, c.lgT), kBlock, smem_alpha, c.stream>>>(a);
+        } else {
+            if (int e = prep(k_mom_alpha<P, false>, smem_alpha)) return e;
+            k_mom_alpha<P, false><<<persistent_grid(k_mom_alpha<P, false>, smem_alpha, c.sm_count, G, c.lgT), kBlock, smem_alpha, c.stream>>>(a);
+        }
+        k_alpha_grid<P><<<fallback_grid(c.sm_count, G, c.lgT), kBlock, d.smem_bytes, c.stream>>>(a.al);
+    });
+    if (int e = check_launch()) return e;
+    return 2;
+}
+
 int PDQ_TUFN(launch_mu_from_lfc)(const LaunchCfg& c, const DesignDev& d, const double* lfc, int G, double* mu, int64_t ld_out) {
     PDQ_DISPATCH_P(d.p, {
         MuLfcArgs<P> a{{d.pack, d.N, d.staged ? (int)(d.smem_bytes - 16) : 0}, lfc, G, c.lgT, mu, ld_out};
@@ -1813,6 +1921,23 @@ int launch_scatter_rows(cudaStream_t stream, const double* in, double* out, cons
     const int64_t total = (int64_t)n * width * nvec;
     if (total <= 0) return 0;
     k_scatter_rows<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, out, perm, n, nvec, stride, width);
+    if (int e = check_launch()) return e;
+    return 1;
+}
+
+int launch_scatter_segments(cudaStream_t stream, const double* in, double* out, const int* src, int nseg, const int64_t* seg) {
+    if (nseg < 1 || nseg > kMaxScatterSegs) return PDQ_ERR_INVALID;
+    ScatterSegs s{};
+    s.n = nseg;
+    for (int i = 0; i < nseg; ++i) {
+        s.off[i] = seg[4 * i];
+        s.rows[i] = (int)seg[4 * i + 1];
+        s.width[i] = (int)seg[4 * i + 2];
+        s.permuted[i] = seg[4 * i + 3] != 0;
+        s.start[i + 1] = s.start[i] + (int64_t)s.rows[i] * s.width[i];
+    }
+    if (s.start[nseg] <= 0) return 0;
+    k_scatter_segments<<<(unsigned)((s.start[nseg] + 255) / 256), 256, 0, stream>>>(in, out, src, s);
     if (int e = check_launch()) return e;
     return 1;
 }

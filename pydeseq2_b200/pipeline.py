@@ -443,6 +443,10 @@ class ResidentFit:
         # entry point keeps the three launches where a warp has many tiles per launch.  False: the three launches always (the
         # reference of tests/test_gpu_fused_tail.py and scripts/tail_bench.py)
         self.fuse_tail = True
+        # on the lin_reg_mu branch: the start values and the genewise search in one persistent launch (pdq_mom_alpha_mle_dev), which
+        # keeps each gene's start value in registers instead of draining one grid and ramping up the next.  Bit-identical results.
+        # False: the two launches always (the reference of tests/test_gpu_pass_glue.py and scripts/pass_glue_bench.py)
+        self.fold_moments = True
         # how gene shards exchange: "peer" = one kernel per exchange storing into every peer's HBM over NVLink (sharding.PeerWindow),
         # "nccl" = grouped NCCL all-gathers, "auto" = peer when the ranks can map each other's memory (one node), else NCCL
         self.exchange = os.environ.get("PDQ_EXCHANGE", "auto")
@@ -450,7 +454,7 @@ class ResidentFit:
         # Device-side gene order: columns sorted by total count at upload.  IRLS iteration counts follow the expression level and
         # the four genes of a warp iterate in lock step, so neighbours of similar expression waste fewer repeated sweeps (22 % ->
         # 4 % of the IRLS sweeps on the synthetic cohorts).  Per-gene arithmetic is position-independent: results are bit-identical
-        # and are returned in the caller's order (one scatter at the end of a pass).
+        # and are returned in the caller's order (one scatter per half of the result slab, see _place).
         self.sort_genes = sort_genes
         self._perm = self._inv = None
         self._graph, self._graph_key, self._eager_key, self._graph_epoch = None, None, None, -1
@@ -559,8 +563,8 @@ class ResidentFit:
         self.G = G
         G, N, p = self.G, self.N, self.p
         ng = N * G * 8
-        # every per-gene result lives in ONE device slab mirrored by one page-locked host block: a pass ends with a single
-        # device-to-host copy instead of a dozen small ones.  With gene shards every vector is laid out with the LARGEST shard's
+        # every per-gene result lives in ONE device slab mirrored by one page-locked host block: a pass copies it in two halves
+        # (below) instead of a dozen small copies.  With gene shards every vector is laid out with the LARGEST shard's
         # length `Gs` and NaN behind this shard's last gene (written here, once): the slab then is directly the send
         # segment of the exchanges (peer-memory push kernel or equal-count NCCL all-gathers) -- no per-step padding, no staging.
         per_gene = ("mom", "means", "gw", "gw_conv", "map", "map_conv", "disp", "conv", "pv", "stat", "se", "outlier",
@@ -583,14 +587,29 @@ class ResidentFit:
         self._slab_off["beta"] = (off, p)
         off += Gs * p
         self.d_t16, self._h["t16"] = self.d_slab + off * 8, self._h_slab[off:off + 16]
-        self._off_beta, self._off_t16, self._n_vec = off - Gs * p, off, len(per_gene)
+        self._off_beta, self._off_t16 = off - Gs * p, off
         self._h_slab[off:off + 16] = 0.0
         self.ctx.h2d(self.d_slab, self._h_slab)  # NaN pads (and zeros) land on the device once
         self.d_nfb = self._dev("nfb", 64)
         c_d = self._lib_mod.c_dptr
         self._perm = self._inv = None
         self.d_slab_out = self.d_slab
-        if self.sort_genes and G >= 256:
+        # The slab reaches the caller's order and the host in two halves.  The genewise half (start values, means, genewise
+        # dispersions and flags) is final when the genewise search ends: it is reordered and copied to the host on a branch of the
+        # stream while the trend and the tail run.  The tail half and the trend record follow at the end of the pass; the Cook's
+        # vectors only when they are computed.  Segments: (offset in doubles, rows, width, permuted) for pdq_scatter_segments_dev.
+        sort = self.sort_genes and G >= 256
+        vec = lambda names: [(self._slab_off[k][0], G, 1, int(sort)) for k in names]  # noqa: E731
+        tail = ("map", "map_conv", "disp", "conv", "pv", "stat", "se", "outlier")
+        cooks = ("robust_disp", "cooks_outlier", "cooks_replaced")
+        rest = [(self._off_beta, G, p, int(sort)), (self._off_t16, 16, 1, 0)]
+        self._seg_gw = np.array(vec(("mom", "means", "gw", "gw_conv")), dtype=np.int64)
+        self._seg_tail = {False: np.array(vec(tail) + rest, dtype=np.int64), True: np.array(vec(tail + cooks) + rest, dtype=np.int64)}
+        # host ranges of the halves (all per-gene vectors are Gs long, in the order of per_gene)
+        o = self._slab_off
+        self._h_gw = [(0, o["map"][0])]
+        self._h_tail = {False: [(o["map"][0], o["robust_disp"][0]), (self._off_beta, total)], True: [(o["map"][0], total)]}
+        if sort:
             d_raw = self.ctx.malloc(ng)
             try:
                 fill(d_raw)
@@ -605,6 +624,8 @@ class ResidentFit:
                 self._inv[perm] = np.arange(G, dtype=np.int32)
                 self.d_perm = self._dev("perm", G * 4)
                 self.ctx.h2d(self.d_perm, perm)
+                self.d_inv = self._dev("inv", G * 4)  # device column of each caller-order gene: the rows the reorder gathers
+                self.ctx.h2d(self.d_inv, self._inv)
                 # 8-byte words are moved as they are: the same gather serves int64 counts and float64 arrays
                 self.ctx.check(self.lib.pdq_gather_columns_dev(self.ctx.h, c_d(d_raw), G, N, c_d(self.d_perm), G, c_d(gs.counts), G))
                 self.ctx.sync()
@@ -618,15 +639,21 @@ class ResidentFit:
         if self.design is None:
             self.device_size_factors()
 
-    def _to_caller_order(self):
-        """Enqueue the scatter of the pass' per-gene results from the device's gene order into the caller's (no-op when unsorted)."""
-        if self._perm is None:
+    def _to_caller_order(self, seg, host=False):
+        """Enqueue the slab segments ``seg`` (``_seg_gw`` or ``_seg_tail``) in the caller's gene order, one launch: into
+        ``d_slab_out`` (no-op when unsorted), or with ``host`` straight into the page-locked host block, with no copy behind it."""
+        if self._perm is None and not host:
             return
-        L, h, c_d = self.lib, self.ctx.h, self._lib_mod.c_dptr
-        self.ctx.check(L.pdq_scatter_rows_dev(h, c_d(self.d_slab), c_d(self.d_slab_out), c_d(self.d_perm), self.G, self._n_vec, self.Gs, 1))
-        self.ctx.check(L.pdq_scatter_rows_dev(h, c_d(self.d_slab + self._off_beta * 8), c_d(self.d_slab_out + self._off_beta * 8),
-                                              c_d(self.d_perm), self.G, 1, self.Gs, self.p))
-        self.ctx.check(L.pdq_memcpy_d2d(h, c_d(self.d_slab_out + self._off_t16 * 8), c_d(self.d_t16), 16 * 8))
+        c_d, i64p = self._lib_mod.c_dptr, self._lib_mod.i64p
+        out = self._h_slab.ctypes.data if host else self.d_slab_out
+        src = c_d(self.d_inv) if self._perm is not None else None
+        self.ctx.check(self.lib.pdq_scatter_segments_dev(self.ctx.h, c_d(self.d_slab), c_d(out), src, len(seg), seg.ctypes.data_as(i64p)))
+
+    def _copy_out(self, ranges, side=False):
+        """Enqueue the device-to-host copies of the caller-ordered slab's ``ranges`` ((start, end) in doubles); ``side``: on the
+        branch of the stream that :meth:`run` joins at the end of the pass."""
+        for a, b in ranges:
+            (self.ctx.d2h_side if side else self.ctx.d2h)(self._h_slab[a:b], self.d_slab_out + a * 8)
 
     def _window(self, n_all):
         """The peer-memory receive window of this fit (collective on first use; None = exchange through NCCL)."""
@@ -669,11 +696,16 @@ class ResidentFit:
             self.design = None
 
     # -- one pass ----------------------------------------------------------------------------------
-    def _enqueue_genewise(self, gs, check, begin):
+    def _enqueue_genewise(self, gs, check, begin, fold=True):
         """Steps 1-3 of a pass (``fit_genewise_dispersions``, dds.py:713-797) on the gene set ``gs``, enqueued without
-        synchronising."""
+        synchronising.  ``fold`` (with ``fold_moments``, lin_reg_mu branch): steps 1 and 3 as one launch; stage timings need the
+        separate launches."""
         L, h, d, G = self.lib, self.ctx.h, self.design, gs.G
         c_d = self._lib_mod.c_dptr
+        if fold and self.fold_moments and self.lin_branch:
+            check(L.pdq_mom_alpha_mle_dev(h, d, c_d(gs.counts), G, G, self.min_disp, self.max_disp, self.min_mu, c_d(gs.mom),
+                                          c_d(gs.means), c_d(gs.mu_hat), G, c_d(gs.gw), c_d(gs.gw_conv), c_d(gs.hint)))
+            return
         # 1. method-of-moments start values + normalised means (dds.py:1140-1162, :708)
         begin("mom_dispersions")
         #    -- and, on the lin_reg_mu branch (dds.py:747-756), the initial mu_hat from the same projection
@@ -779,7 +811,10 @@ class ResidentFit:
         d_fitted = d_fit_all + rank * m * 8  # this shard's slice of the fitted curve
 
         def enqueue():
-            self._enqueue_genewise(gs, check, begin)  # steps 1-3
+            self._enqueue_genewise(gs, check, begin, fold=not profile)  # steps 1-3
+            # the genewise half of the slab is final: to the caller's order, and to the host while the rest of the pass runs
+            self._to_caller_order(self._seg_gw)
+            self._copy_out(self._h_gw, side=True)
             # 4. trend + prior: global over ALL genes of ALL shards (dds.py:799-884).  With gene shards the per-gene
             #    vectors are exchanged first, device to device (peer-memory push kernel or grouped NCCL all-gathers); the fit itself
             #    is one launch (a thread-block cluster, or a cooperative grid from 65 536 genes).
@@ -794,24 +829,32 @@ class ResidentFit:
                                           c_d(d_t16), c_d(d_fit_all)))
                 self._tail(gs, d_fitted, d_t16 + 9 * 8, 0.0, contrast, lfc_null, alt_hypothesis, begin, check, fused)
                 self._cooks(begin, check)
-                if self._perm is not None:
+                if self.comm is None:
+                    # the tail half of the results + the trend record: written into the host block by the reorder launch itself
                     begin("to_caller_order")
-                    self._to_caller_order()
+                    self._to_caller_order(self._seg_tail[self.with_cooks], host=True)
                     if profile:
                         check(0)
-                if d_table_all is not None or win is not None:
-                    # end-of-call exchange (SURVEY.md §8e / north star): ONE exchange of the whole result slab -- dispersions,
-                    # coefficients, flags, Wald statistics of every shard -- after which each rank holds the full tables in HBM
-                    begin("gather_results")
-                    exchange_tables()
-                    if profile:
-                        check(0)
-            ctx.d2h(self._h_slab, self.d_slab_out)  # every per-gene result of THIS shard + the trend record, one copy
+                else:
+                    if self._perm is not None:
+                        begin("to_caller_order")
+                        self._to_caller_order(self._seg_tail[self.with_cooks])
+                        if profile:
+                            check(0)
+                    if d_table_all is not None or win is not None:
+                        # end-of-call exchange (SURVEY.md §8e / north star): ONE exchange of the whole result slab -- dispersions,
+                        # coefficients, flags, Wald statistics of every shard -- after which each rank holds the full tables in HBM
+                        begin("gather_results")
+                        exchange_tables()
+                        if profile:
+                            check(0)
+                    self._copy_out(self._h_tail[self.with_cooks])  # the tail half of THIS shard's results + the trend record
+            ctx.side_join()
 
         # The pass is ~20 launches + copies with no host synchronisation in between: after one eager pass (which allocates
         # every buffer) the identical sequence is captured into a CUDA graph and replayed with a single call.
-        key = (fit_type, contrast.tobytes(), float(lfc_null), alt_hypothesis, G, self.with_cooks, n_all, self.fuse_tail, self.gather,
-               win is not None)
+        key = (fit_type, contrast.tobytes(), float(lfc_null), alt_hypothesis, G, self.with_cooks, n_all, self.fuse_tail, self.fold_moments,
+               self.gather, win is not None)
         # a captured pass holds pointers into context-owned scratch (per-gene status words, trend scratch); host-buffer calls on the
         # same context may have re-allocated it since: the context counts re-allocations, a stale graph is dropped and re-captured
         if events:
@@ -863,10 +906,12 @@ class ResidentFit:
             ctx.h2d(d_fit_all, fit_all)
             self._tail(gs, d_fitted, None, prior_var, contrast, lfc_null, alt_hypothesis, begin, check, fused)
             self._cooks(begin, check)
-            self._to_caller_order()
-            if self.comm is not None:
+            if self.comm is None:
+                self._to_caller_order(self._seg_tail[self.with_cooks], host=True)
+            else:
+                self._to_caller_order(self._seg_tail[self.with_cooks])
                 exchange_tables()
-            ctx.d2h(self._h_slab, self.d_slab_out)
+                self._copy_out(self._h_tail[self.with_cooks])
             ctx.sync()
             self._check_tail()
         gw = np.clip(H["gw"], self.min_disp, self.max_disp)
