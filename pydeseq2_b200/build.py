@@ -19,7 +19,7 @@ UNITS = [("pdq_api.cu", "pdq_api", ()), ("pdq_dispatch.cu", "pdq_dispatch", ()),
         [("pdq_kernels.cu", f"pdq_kernels_p{p}", (f"-DPDQ_TU_P={p}", "-Xptxas", "-O1")) for p in WIDE_P]
 # (ptxas -O1 for the wide widths: 12 s instead of 85 s per unit; their kernels keep the small matrices in local memory anyway)
 SOURCES = sorted({u[0] for u in UNITS})
-HEADERS = ["pdq_math.cuh", "pdq_fast.cuh", "pdq_tables.h", "pdq_trend.cuh", "pdq_gene.cuh", "pdq_shrink.cuh", "pdq_vst.cuh", "pdq_padj.cuh", "pdq_internal.h",
+HEADERS = ["pdq_math.cuh", "pdq_fast.cuh", "pdq_tables.h", "pdq_trend.cuh", "pdq_gene.cuh", "pdq_shrink.cuh", "pdq_vst.cuh", "pdq_padj.cuh", "pdq_team.cuh", "pdq_internal.h",
            "pdq_host_linalg.h", os.path.join("..", "..", "include", "pydeseq2_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-fopenmp", "--expt-relaxed-constexpr"]
