@@ -548,22 +548,30 @@ extern "C" void pdq_graph_destroy(pdq_ctx* c, pdq_graph* g) {
 }
 
 // --------------------------------------------------------------------------------------------- design pack
-// the widest design the context accepts: PDQ_MAX_P, PDQ_MAX_P_WIDE after pdq_set_wide_designs(ctx, 1), PDQ_MAX_P_LARGE after
-// pdq_set_large_designs(ctx, 1) as well
+// the widest design the context fits: PDQ_MAX_P, PDQ_MAX_P_WIDE after pdq_set_wide_designs(ctx, 1), PDQ_MAX_P_LARGE with large on too
 static int max_p(const pdq_ctx* c) { return !c->wide ? PDQ_MAX_P : (c->large ? PDQ_MAX_P_LARGE : PDQ_MAX_P_WIDE); }
 
-static int check_width(pdq_ctx* c, int p) {
-    if (p > PDQ_MAX_P && !c->wide) return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
+// Whether the context takes a design of p columns, for a fit or (`shrink`) for apeGLM shrinkage: up to max_p(c) columns, and for
+// shrinkage of more than PDQ_MAX_P columns pdq_set_wide_shrink on top, of more than PDQ_MAX_P_WIDE pdq_set_large_shrink too.
+// PDQ_OK, or the refusal the opt-ins call for (PDQ_ERR_UNSUPPORTED, behind `prefix`); p < 1 is refused as pdq_design_create does.
+static int design_width(pdq_ctx* c, int p, bool shrink = false, const char* prefix = "") {
+    if (p < 1) return fail(c, PDQ_ERR_INVALID, "pdq_design_create: bad arguments");
+    auto no_shrink = [&](int q) {
+        return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", q);
+    };
+    if (shrink && p > PDQ_MAX_P && !c->wide_shrink) return no_shrink(PDQ_MAX_P);
     if (p > max_p(c))
-        return fail(c, PDQ_ERR_UNSUPPORTED, "design has %d columns; wide designs support p <= %d", p, max_p(c));
+        return fail(c, PDQ_ERR_UNSUPPORTED, "%sdesign has %d columns; %s p <= %d", prefix, p,
+                    c->wide ? "wide designs support" : "this build supports", max_p(c));
+    if (shrink && p > PDQ_MAX_P_WIDE && !c->large_shrink) return no_shrink(PDQ_MAX_P_WIDE);
     return PDQ_OK;
 }
 
 static int design_create(pdq_ctx* c, const double* X, const double* sf, bool offsets, int N, int p, pdq_design** out) {
     if (!c || !X || !out || N <= 0 || p < 1) return fail(c, PDQ_ERR_INVALID, "pdq_design_create: bad arguments");
-    if (int e = check_width(c, p)) return e;
+    if (int e = design_width(c, p)) return e;
     CU(c, cudaSetDevice(c->device));
-    pdq_design* d = new pdq_design();
+    pdq_design* d = new pdq_design();  // value-initialised: every device pointer starts null
     DesignDev& dd = d->d;
     dd.N = N;
     dd.p = p;
@@ -580,51 +588,31 @@ static int design_create(pdq_ctx* c, const double* X, const double* sf, bool off
     dd.smem_bytes = (dd.staged ? pack_bytes : 0) + 16;
     std::vector<double> pinv((size_t)p * p);
     design_linear_algebra(X, N, p, pinv.data(), &dd.full_rank);
+    auto bail = [&](const char* what) {
+        pdq_design_destroy(c, d);
+        return fail(c, PDQ_ERR_CUDA, "%s failed", what);
+    };
     if (p <= PDQ_MAX_P) {
         memcpy(dd.pinv, pinv.data(), pinv.size() * 8);
     } else if (cudaMalloc((void**)&dd.pinv_dev, pinv.size() * 8) != cudaSuccess ||
                cudaMemcpy(dd.pinv_dev, pinv.data(), pinv.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess ||
                cudaMalloc((void**)&dd.wald_dev, ((size_t)p * (p + 1) / 2 + 1 + p) * 8) != cudaSuccess) {
-        if (dd.pinv_dev) cudaFree(dd.pinv_dev);
-        if (dd.wald_dev) cudaFree(dd.wald_dev);
-        delete d;
-        return fail(c, PDQ_ERR_CUDA, "cudaMalloc/cudaMemcpy(pseudo-inverse) failed");
+        return bail("cudaMalloc/cudaMemcpy(pseudo-inverse)");
     }
     if (p > PDQ_MAX_P_WIDE)
         if (const char* e = getenv("PDQ_LARGE_WARPS")) dd.warps = atoi(e);  // tuning hook (A/B runs): 2, 4 or 8 warps per gene
     dd.few_rows = design_distinct_rows(X, N, p, 16) <= 16;
     if (const char* e = getenv("PDQ_IRLS_MEMO")) dd.few_rows = dd.few_rows && atoi(e) != 0;  // tuning hook (A/B runs)
-    {
-        const std::vector<int> plan = design_cell_plan(X, N, p);
-        dd.n_cells = plan[0];
-        dd.plan_len = (int)plan.size();
-        dd.n_in_cells = dd.plan_len - (2 + dd.n_cells + 1);
-        dd.cell_plan = nullptr;
-        if (cudaMalloc((void**)&dd.cell_plan, plan.size() * sizeof(int)) != cudaSuccess ||
-            cudaMemcpy(dd.cell_plan, plan.data(), plan.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess) {
-            if (dd.cell_plan) cudaFree(dd.cell_plan);
-            if (dd.pinv_dev) cudaFree(dd.pinv_dev);
-            if (dd.wald_dev) cudaFree(dd.wald_dev);
-            delete d;
-            return fail(c, PDQ_ERR_CUDA, "cudaMalloc/cudaMemcpy(cell plan) failed");
-        }
-    }
-    if (cudaMalloc((void**)&dd.pack, pack.size() * 8) != cudaSuccess) {
-        cudaFree(dd.cell_plan);
-        if (dd.pinv_dev) cudaFree(dd.pinv_dev);
-        if (dd.wald_dev) cudaFree(dd.wald_dev);
-        delete d;
-        return fail(c, PDQ_ERR_CUDA, "cudaMalloc(design pack) failed");
-    }
+    const std::vector<int> plan = design_cell_plan(X, N, p);
+    dd.n_cells = plan[0];
+    dd.plan_len = (int)plan.size();
+    dd.n_in_cells = dd.plan_len - (2 + dd.n_cells + 1);
+    if (cudaMalloc((void**)&dd.cell_plan, plan.size() * sizeof(int)) != cudaSuccess ||
+        cudaMemcpy(dd.cell_plan, plan.data(), plan.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess)
+        return bail("cudaMalloc/cudaMemcpy(cell plan)");
+    if (cudaMalloc((void**)&dd.pack, pack.size() * 8) != cudaSuccess) return bail("cudaMalloc(design pack)");
     // synchronous copy: `pack` is a temporary
-    if (cudaMemcpy(dd.pack, pack.data(), pack.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) {
-        cudaFree(dd.pack);
-        cudaFree(dd.cell_plan);
-        if (dd.pinv_dev) cudaFree(dd.pinv_dev);
-        if (dd.wald_dev) cudaFree(dd.wald_dev);
-        delete d;
-        return fail(c, PDQ_ERR_CUDA, "cudaMemcpy(design pack) failed");
-    }
+    if (cudaMemcpy(dd.pack, pack.data(), pack.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) return bail("cudaMemcpy(design pack)");
     *out = d;
     return PDQ_OK;
 }
@@ -647,7 +635,8 @@ extern "C" void pdq_design_destroy(pdq_ctx* c, pdq_design* d) {
 static int cached_design(pdq_ctx* c, const double* X, const double* sf, int N, int p, pdq_design** out, bool offsets = false) {
     // a deseq2() pass alternates between three packs -- (X, sf), (X, no sf), (ones, sf) -- so a one-entry cache would
     // rebuild (SVD, cell plan, two cudaMallocs, two synchronous copies) on almost every call: keep the last few
-    if (int e = check_width(c, p)) return e;  // a cached wide pack is refused again once the opt-in is off
+    // a cached wide pack is refused again once the opt-in is off (entry points whose later checks rank below it ran it already)
+    if (int e = design_width(c, p)) return e;
     const size_t nx = (size_t)N * p;
     for (size_t i = 0; i < c->dcache.size(); ++i) {
         DesignCacheEntry& e = c->dcache[i];
@@ -682,12 +671,60 @@ static int cached_design(pdq_ctx* c, const double* X, const double* sf, int N, i
 static int done(pdq_ctx* c, int rc, const char* what) {
     if (rc < 0) {
         if (rc == PDQ_ERR_UNSUPPORTED)
-            return fail(c, rc, "%s: unsupported design (p=%d..%d, shared-memory stage <= %zu bytes)", what, 1, max_p(c),
-                        kMaxDynSmem);
+            return fail(c, rc, "%s: unsupported design (p=%d..%d, shared-memory stage <= %zu bytes)", what, 1, max_p(c), kMaxDynSmem);
         return fail(c, rc, "%s: kernel launch failed: %s", what, cudaGetErrorString(cudaGetLastError()));
     }
     c->launches += rc;
     return PDQ_OK;
+}
+
+// ---- operations: the checks and the launch behind both forms of an entry point
+// An operation's semantic checks (those beyond null pointers and sizes) run before anything is staged, so that a refused call
+// leaves the residency cache and the context's buffers as they were.  The device form launches once; the host-buffer form once
+// per gene block, passing the block's slice of the per-gene scratch.
+static int check_alt(pdq_ctx* c, int alt, const char* refusal) {
+    return alt < 0 || alt > 4 ? fail(c, PDQ_ERR_INVALID, "%s", refusal) : PDQ_OK;
+}
+
+static int check_prior(pdq_ctx* c, int prior_reg, const double* prior_var_dev, double prior_disp_var) {
+    return prior_reg && !prior_var_dev && !(prior_disp_var > 0.0) ? fail(c, PDQ_ERR_INVALID, "alpha_mle: prior_reg needs prior_disp_var > 0") : PDQ_OK;
+}
+
+static int check_not_square(pdq_ctx* c, int N, int p) {
+    return N == p ? fail(c, PDQ_ERR_INVALID, "The number of samples and the number of design variables are equal") : PDQ_OK;
+}
+
+static int check_shrink(pdq_ctx* c, int p, int shrink_index, double prior_no_shrink_scale, double prior_scale) {
+    const bool bad = shrink_index < 0 || shrink_index >= p || !(prior_no_shrink_scale > 0.0) || !(prior_scale > 0.0);
+    return bad ? fail(c, PDQ_ERR_INVALID, "pdq_lfc_shrink_dev: bad arguments") : PDQ_OK;
+}
+
+// The fused launches (MAP -> LFC hand-off, moments fold) pay where a warp works on few tiles per launch; above 12 tiles per
+// resident warp of the search the stages run as separate launches
+static bool many_tiles(const LaunchCfg& lc, int G) {
+    const int gpw = 32 >> lc.lgT;
+    return (int64_t)(G + gpw - 1) / gpw > (int64_t)12 * 12 * lc.sm_count;
+}
+
+// `status`: per-gene scratch of G ints, nullptr for the context's
+static int irls_op(pdq_ctx* c, const LaunchCfg& lc, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* disp,
+                   const IrlsHost& h, double* beta, double* mu, double* hat, int64_t ld_out, double* conv, int* status, int* n_fallback,
+                   const WaldHost* w = nullptr) {
+    void* st = status;
+    if (!st)
+        if (int e = ensure(c, kBufStatus, (size_t)G * sizeof(int), &st)) return e;
+    return done(c, launch_irls(lc, d, counts, ld, G, disp, h, beta, mu, hat, ld_out, conv, (int*)st, n_fallback, w), w ? "irls+wald" : "irls");
+}
+
+static int alpha_mle_op(pdq_ctx* c, const LaunchCfg& lc, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu,
+                        int64_t ld_mu, const double* alpha_hat, double min_disp, double max_disp, double prior_disp_var,
+                        const double* prior_var_dev, int cr_reg, int prior_reg, double* alpha, double* conv, int* status,
+                        const double* hint_in = nullptr, double* hint_out = nullptr) {
+    void* st = status;
+    if (!st)
+        if (int e = ensure(c, kBufStatus, (size_t)G * sizeof(int), &st)) return e;
+    return done(c, launch_alpha_mle(lc, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_disp_var, prior_var_dev, cr_reg,
+                                    prior_reg, alpha, conv, (int*)st, hint_in, hint_out), "alpha_mle");
 }
 
 extern "C" int pdq_lin_reg_mu_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, double min_mu,
@@ -703,10 +740,8 @@ extern "C" int pdq_irls_dev(pdq_ctx* c, const pdq_design* d, const int64_t* coun
     CHECK_CTX(c);
     if (!d || !counts || !disp || !beta || !mu || !hat || !conv || G <= 0 || ld < G || ld_out < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_irls_dev: bad arguments");
-    void* status;
-    if (int e = ensure(c, kBufStatus, (size_t)G * sizeof(int), &status)) return e;
-    IrlsHost h{min_mu, beta_tol, min_beta, max_beta, maxiter};
-    return done(c, launch_irls(cfg(c, G, d->d.N), d->d, counts, ld, G, disp, h, beta, mu, hat, ld_out, conv, (int*)status, n_fallback_dev), "irls");
+    return irls_op(c, cfg(c, G, d->d.N), d->d, counts, ld, G, disp, IrlsHost{min_mu, beta_tol, min_beta, max_beta, maxiter}, beta, mu, hat,
+                   ld_out, conv, nullptr, n_fallback_dev);
 }
 
 extern "C" int pdq_irls_wald_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, const double* disp,
@@ -715,43 +750,31 @@ extern "C" int pdq_irls_wald_dev(pdq_ctx* c, const pdq_design* d, const int64_t*
                                  const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
     CHECK_CTX(c);
     if (!d || !counts || !disp || !beta || !mu || !hat || !conv || G <= 0 || ld < G || ld_out < G || !ridge || !contrast || !pv ||
-        !stat || !se || alt < 0 || alt > 4)
+        !stat || !se)
         return fail(c, PDQ_ERR_INVALID, "pdq_irls_wald_dev: bad arguments");
-    void* status;
-    if (int e = ensure(c, kBufStatus, (size_t)G * sizeof(int), &status)) return e;
-    IrlsHost h{min_mu, beta_tol, min_beta, max_beta, maxiter};
+    if (int e = check_alt(c, alt, "pdq_irls_wald_dev: bad arguments")) return e;
     const WaldHost w{ridge, contrast, lfc_null, alt, pv, stat, se};
-    return done(c, launch_irls(cfg(c, G, d->d.N), d->d, counts, ld, G, disp, h, beta, mu, hat, ld_out, conv, (int*)status, n_fallback_dev, &w),
-                "irls+wald");
-}
-
-static int alpha_mle_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, const double* mu,
-                                 int64_t ld_mu, const double* alpha_hat, double min_disp, double max_disp, double prior_disp_var,
-                                 const double* prior_var_dev, int cr_reg, int prior_reg, double* alpha, double* conv,
-                         const double* hint_in, double* hint_out) {
-    CHECK_CTX(c);
-    if (!d || !counts || !mu || !alpha_hat || !alpha || !conv || G <= 0 || ld < G || ld_mu < G)
-        return fail(c, PDQ_ERR_INVALID, "pdq_alpha_mle_dev: bad arguments");
-    if (prior_reg && !prior_var_dev && !(prior_disp_var > 0.0)) return fail(c, PDQ_ERR_INVALID, "alpha_mle: prior_reg needs prior_disp_var > 0");
-    void* status;
-    if (int e = ensure(c, kBufStatus, (size_t)G * sizeof(int), &status)) return e;
-    return done(c, launch_alpha_mle(cfg(c, G, d->d.N), d->d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_disp_var,
-                                    prior_var_dev, cr_reg, prior_reg, alpha, conv, (int*)status, hint_in, hint_out), "alpha_mle");
-}
-
-extern "C" int pdq_alpha_mle_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, const double* mu,
-                                 int64_t ld_mu, const double* alpha_hat, double min_disp, double max_disp, double prior_disp_var,
-                                 const double* prior_var_dev, int cr_reg, int prior_reg, double* alpha, double* conv) {
-    return alpha_mle_dev(c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_disp_var, prior_var_dev, cr_reg, prior_reg, alpha,
-                         conv, nullptr, nullptr);
+    return irls_op(c, cfg(c, G, d->d.N), d->d, counts, ld, G, disp, IrlsHost{min_mu, beta_tol, min_beta, max_beta, maxiter}, beta, mu, hat,
+                   ld_out, conv, nullptr, n_fallback_dev, &w);
 }
 
 extern "C" int pdq_alpha_mle_hint_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, const double* mu,
                                       int64_t ld_mu, const double* alpha_hat, double min_disp, double max_disp, double prior_disp_var,
                                       const double* prior_var_dev, int cr_reg, int prior_reg, double* alpha, double* conv,
                                       const double* hint_in, double* hint_out) {
-    return alpha_mle_dev(c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_disp_var, prior_var_dev, cr_reg, prior_reg, alpha,
-                         conv, hint_in, hint_out);
+    CHECK_CTX(c);
+    if (!d || !counts || !mu || !alpha_hat || !alpha || !conv || G <= 0 || ld < G || ld_mu < G)
+        return fail(c, PDQ_ERR_INVALID, "pdq_alpha_mle_dev: bad arguments");
+    if (int e = check_prior(c, prior_reg, prior_var_dev, prior_disp_var)) return e;
+    return alpha_mle_op(c, cfg(c, G, d->d.N), d->d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_disp_var, prior_var_dev,
+                        cr_reg, prior_reg, alpha, conv, nullptr, hint_in, hint_out);
+}
+
+extern "C" int pdq_alpha_mle_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, const double* mu,
+                                 int64_t ld_mu, const double* alpha_hat, double min_disp, double max_disp, double prior_disp_var,
+                                 const double* prior_var_dev, int cr_reg, int prior_reg, double* alpha, double* conv) {
+    return pdq_alpha_mle_hint_dev(c, d, counts, ld, G, mu, ld_mu, alpha_hat, min_disp, max_disp, prior_disp_var, prior_var_dev, cr_reg,
+                                  prior_reg, alpha, conv, nullptr, nullptr);
 }
 
 extern "C" int pdq_map_irls_wald_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, const double* mu,
@@ -763,24 +786,25 @@ extern "C" int pdq_map_irls_wald_dev(pdq_ctx* c, const pdq_design* d, const int6
                                      const double* contrast, double lfc_null, int alt, double* pv, double* stat, double* se) {
     CHECK_CTX(c);
     if (!d || !counts || !mu || !fitted || !genewise || !hint_in || !trend_out16 || !map || !map_conv || !disp || !beta || !mu_out ||
-        !hat || !conv || G <= 0 || ld < G || ld_mu < G || ld_out < G || !ridge || !contrast || !pv || !stat || !se || alt < 0 || alt > 4)
+        !hat || !conv || G <= 0 || ld < G || ld_mu < G || ld_out < G || !ridge || !contrast || !pv || !stat || !se)
         return fail(c, PDQ_ERR_INVALID, "pdq_map_irls_wald_dev: bad arguments");
+    if (int e = check_alt(c, alt, "pdq_map_irls_wald_dev: bad arguments")) return e;
     if (!prior_var_dev && !(prior_disp_var > 0.0)) return fail(c, PDQ_ERR_INVALID, "pdq_map_irls_wald_dev: needs prior_disp_var > 0");
     // The hand-off pays where a warp works on few tiles per launch, so that the drained end of the search and the ramp-up of the
     // fit are a visible share of both: measured on H100 it gains 3-7 % up to ~10 tiles per resident warp of the search (12 per SM)
     // and loses 2.5 % at 20 (DESIGN.md §5).  Above 12 the three stages run as the three launches.
     const LaunchCfg lcfg = cfg(c, G, d->d.N);
-    const int gpw = 32 >> lcfg.lgT;
+    const IrlsHost h{min_mu, beta_tol, min_beta, max_beta, maxiter};
+    const WaldHost w{ridge, contrast, lfc_null, alt, pv, stat, se};
     // wide designs (p > PDQ_MAX_P) have no fused pair: always the three launches
-    if ((int64_t)(G + gpw - 1) / gpw > (int64_t)12 * 12 * lcfg.sm_count || d->d.p > PDQ_MAX_P) {
-        if (int e = alpha_mle_dev(c, d, counts, ld, G, mu, ld_mu, fitted, min_disp, max_disp, prior_disp_var, prior_var_dev, 1, 1, map,
-                                  map_conv, hint_in, nullptr))
+    if (many_tiles(lcfg, G) || d->d.p > PDQ_MAX_P) {
+        if (int e = alpha_mle_op(c, lcfg, d->d, counts, ld, G, mu, ld_mu, fitted, min_disp, max_disp, prior_disp_var, prior_var_dev, 1, 1, map,
+                                 map_conv, nullptr, hint_in, nullptr))
             return e;
         if (int e = done(c, launch_select_disp(lcfg, genewise, map, fitted, trend_out16, (size_t)G, min_disp, max_disp, disp, outlier),
                          "select_dispersions"))
             return e;
-        return pdq_irls_wald_dev(c, d, counts, ld, G, disp, min_mu, beta_tol, min_beta, max_beta, maxiter, beta, mu_out, hat, ld_out, conv,
-                                 nullptr, ridge, contrast, lfc_null, alt, pv, stat, se);
+        return irls_op(c, lcfg, d->d, counts, ld, G, disp, h, beta, mu_out, hat, ld_out, conv, nullptr, nullptr, &w);
     }
     void* status;
     if (int e = ensure(c, kBufStatus, 2 * (size_t)G * sizeof(int), &status)) return e;
@@ -803,8 +827,6 @@ extern "C" int pdq_map_irls_wald_dev(pdq_ctx* c, const pdq_design* d, const int6
     }
     const TailHost t{mu, ld_mu, fitted, genewise, hint_in, trend_out16, min_disp, max_disp, prior_disp_var, prior_var_dev, map, map_conv,
                      disp, outlier, beta, mu_out, hat, conv, ld_out, (int*)status, (int*)status + G, c->tile_done, c->tail_err_dev};
-    const IrlsHost h{min_mu, beta_tol, min_beta, max_beta, maxiter};
-    const WaldHost w{ridge, contrast, lfc_null, alt, pv, stat, se};
     return done(c, launch_map_irls(lcfg, d->d, counts, ld, G, t, h, w), "map+irls+wald");
 }
 
@@ -820,8 +842,9 @@ extern "C" int pdq_wald_test_dev(pdq_ctx* c, const pdq_design* d, const double* 
                                  int64_t ld_mu, int G, const double* ridge, const double* contrast, double lfc_null, int alt,
                                  double* pv, double* stat, double* se) {
     CHECK_CTX(c);
-    if (!d || !disp || !lfc || !mu || !ridge || !contrast || !pv || !stat || !se || G <= 0 || ld_mu < G || alt < 0 || alt > 4)
+    if (!d || !disp || !lfc || !mu || !ridge || !contrast || !pv || !stat || !se || G <= 0 || ld_mu < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_test_dev: bad arguments");
+    if (int e = check_alt(c, alt, "pdq_wald_test_dev: bad arguments")) return e;
     return done(c, launch_wald(cfg(c, G, d->d.N), d->d, disp, lfc, mu, ld_mu, G, ridge, contrast, lfc_null, alt, pv, stat, se), "wald_test");
 }
 
@@ -829,17 +852,10 @@ extern "C" int pdq_lfc_shrink_dev(pdq_ctx* c, const pdq_design* d, const int64_t
                                   double prior_no_shrink_scale, double prior_scale, int shrink_index, double* lfcs, double* inv_hessians,
                                   double* conv, int* status) {
     CHECK_CTX(c);
-    if (!d || !counts || !size || !lfcs || !inv_hessians || !conv || !status || G <= 0 || ld < G || shrink_index < 0 ||
-        shrink_index >= d->d.p || !(prior_no_shrink_scale > 0.0) || !(prior_scale > 0.0))
+    if (!d || !counts || !size || !lfcs || !inv_hessians || !conv || !status || G <= 0 || ld < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_lfc_shrink_dev: bad arguments");
-    if (d->d.p > PDQ_MAX_P) {
-        if (!c->wide_shrink)
-            return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
-        if (int e = check_width(c, d->d.p)) return e;  // a pack made before the wide-design opt-in was turned off
-    }
-    if (d->d.p > PDQ_MAX_P_WIDE && !c->large_shrink)  // reached with wide shrinkage and large designs on only (refused above otherwise)
-        return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented",
-                    PDQ_MAX_P_WIDE);
+    if (int e = check_shrink(c, d->d.p, shrink_index, prior_no_shrink_scale, prior_scale)) return e;
+    if (int e = design_width(c, d->d.p, true)) return e;  // also refuses a pack made before an opt-in was turned off
     return done(c, launch_lfc_shrink(cfg(c, G, d->d.N), d->d, counts, ld, G, size, prior_no_shrink_scale, prior_scale, shrink_index, lfcs,
                                      inv_hessians, conv, status), "lfc_shrink");
 }
@@ -875,7 +891,7 @@ extern "C" int pdq_mom_dispersions_dev(pdq_ctx* c, const pdq_design* d, const in
     CHECK_CTX(c);
     if (!d || !counts || !alpha || !normed_mean || G <= 0 || ld < G || (mu_hat_out && ld_mu < G))
         return fail(c, PDQ_ERR_INVALID, "pdq_mom_dispersions_dev: bad arguments");
-    if (d->d.N == d->d.p) return fail(c, PDQ_ERR_INVALID, "The number of samples and the number of design variables are equal");
+    if (int e = check_not_square(c, d->d.N, d->d.p)) return e;
     return done(c, launch_mom_from_counts(cfg(c, G, d->d.N), d->d, counts, ld, G, min_disp, max_disp, alpha, normed_mean, min_mu, mu_hat_out, ld_mu),
                 "mom_dispersions");
 }
@@ -886,7 +902,7 @@ extern "C" int pdq_mom_alpha_mle_dev(pdq_ctx* c, const pdq_design* d, const int6
     CHECK_CTX(c);
     if (!d || !counts || !mom || !normed_mean || !mu_hat || !alpha || !conv || G <= 0 || ld < G || ld_mu < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_mom_alpha_mle_dev: bad arguments");
-    if (d->d.N == d->d.p) return fail(c, PDQ_ERR_INVALID, "The number of samples and the number of design variables are equal");
+    if (int e = check_not_square(c, d->d.N, d->d.p)) return e;
     void* status;
     if (int e = ensure(c, kBufStatus, (size_t)G * sizeof(int), &status)) return e;
     // The fold pays where a warp works on few tiles per launch, as the MAP -> LFC hand-off does: the start values then run at the
@@ -894,13 +910,12 @@ extern "C" int pdq_mom_alpha_mle_dev(pdq_ctx* c, const pdq_design* d, const int6
     // streaming is long.  Whole resident pass on H100: 3 % faster at C2 (3.2 tiles per resident search warp), 6 % slower at the C5
     // shard (19.7) (DESIGN.md §5).  Above 12 tiles the two launches, as in pdq_map_irls_wald_dev.
     const LaunchCfg lcfg = cfg(c, G, d->d.N);
-    if ((int64_t)(G + (32 >> lcfg.lgT) - 1) / (32 >> lcfg.lgT) > (int64_t)12 * 12 * lcfg.sm_count) {
+    if (many_tiles(lcfg, G)) {
         if (int e = done(c, launch_mom_from_counts(lcfg, d->d, counts, ld, G, min_disp, max_disp, mom, normed_mean, min_mu, mu_hat, ld_mu),
                          "mom_dispersions"))
             return e;
-        return done(c, launch_alpha_mle(lcfg, d->d, counts, ld, G, mu_hat, ld_mu, mom, min_disp, max_disp, 1.0, nullptr, 1, 0, alpha, conv,
-                                        (int*)status, nullptr, hint_out),
-                    "alpha_mle");
+        return alpha_mle_op(c, lcfg, d->d, counts, ld, G, mu_hat, ld_mu, mom, min_disp, max_disp, 1.0, nullptr, 1, 0, alpha, conv, (int*)status,
+                            nullptr, hint_out);
     }
     return done(c, launch_mom_alpha(lcfg, d->d, counts, ld, G, min_disp, max_disp, min_mu, mom, normed_mean, mu_hat, ld_mu,
                                     alpha, conv, (int*)status, hint_out),
@@ -1392,12 +1407,6 @@ static int call_end(pdq_ctx* c, const Pipe* p, std::initializer_list<pdq_ctx::Re
     return PDQ_OK;
 }
 
-static int pipe_end(pdq_ctx* c, const Pipe& p) {
-    if (int e = pipe_join(c, p)) return e;
-    CU(c, cudaStreamSynchronize(c->stream));
-    return 0;
-}
-
 // column block [g0, g0+gb) of an (N, G) array, host pitch ld_h elements <-> device pitch ld_d elements
 static int cols_h2d(pdq_ctx* c, const Pipe& p, int b, void* dev, int64_t ld_d, const void* host, int64_t ld_h, int N, size_t elem) {
     if (!p.on) return h2d_2d(c, dev, host, ld_h, N, p.G, elem);
@@ -1406,7 +1415,7 @@ static int cols_h2d(pdq_ctx* c, const Pipe& p, int b, void* dev, int64_t ld_d, c
     return 0;
 }
 static int cols_d2h(pdq_ctx* c, const Pipe& p, int b, void* host, int64_t ld_h, const void* dev, int64_t ld_d, int N, size_t elem) {
-    if (!p.on) return copy_d2h(c, host, dev, (size_t)N * p.G * elem);
+    if (!p.on && ld_h == p.G && ld_d == p.G) return copy_d2h(c, host, dev, (size_t)N * p.G * elem);
     CU(c, cudaMemcpy2DAsync((char*)host + (size_t)p.g0(b) * elem, (size_t)ld_h * elem, (const char*)dev + (size_t)p.g0(b) * elem,
                             (size_t)ld_d * elem, (size_t)p.gb(b) * elem, N, cudaMemcpyDeviceToHost, p.st(b)));
     return 0;
@@ -1477,9 +1486,9 @@ extern "C" int pdq_irls(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, in
         const int g0 = pp.g0(b), gb = pp.gb(b);
         if (up_c)
             if (int e = cols_h2d(c, pp, b, dc, G, counts, ld, N, 8)) return e;
-        if (int e = done(c, launch_irls(pp.cfg_for(b, N), d->d, (const int64_t*)dc + g0, G, gb, (const double*)ddisp + g0, h,
-                                        (double*)dbeta + (size_t)g0 * p, (double*)dmu + g0, (double*)dhat + g0, G, (double*)dconv + g0,
-                                        (int*)status + g0, (int*)dmisc + b), "irls"))
+        if (int e = irls_op(c, pp.cfg_for(b, N), d->d, (const int64_t*)dc + g0, G, gb, (const double*)ddisp + g0, h,
+                            (double*)dbeta + (size_t)g0 * p, (double*)dmu + g0, (double*)dhat + g0, G, (double*)dconv + g0,
+                            (int*)status + g0, (int*)dmisc + b))
             return e;
         if (int e = cols_d2h(c, pp, b, mu_out, G, dmu, G, N, 8)) return e;
         if (int e = cols_d2h(c, pp, b, hat_out, G, dhat, G, N, 8)) return e;
@@ -1502,9 +1511,10 @@ extern "C" int pdq_alpha_mle(pdq_ctx* c, const int64_t* counts, int64_t ld, int 
     CHECK_CTX(c);
     if (!counts || !X || !mu || !alpha_hat || !alpha_out || !conv_out || N <= 0 || G <= 0 || ld < G || ld_mu < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_alpha_mle: bad arguments");
+    if (int e = design_width(c, p)) return e;
+    if (int e = check_prior(c, prior_reg, nullptr, prior_disp_var)) return e;
     pdq_design* d;
     if (int e = cached_design(c, X, nullptr, N, p, &d)) return e;
-    const size_t ng = (size_t)N * G;
     void *dc, *dmu, *dah, *dal, *dconv;
     res_begin(c);
     bool up_c, up_m;
@@ -1513,7 +1523,6 @@ extern "C" int pdq_alpha_mle(pdq_ctx* c, const int64_t* counts, int64_t ld, int 
     if (int e = ensure(c, kBufC, (size_t)G * 8, &dah)) return e;
     if (int e = ensure(c, kBufD, (size_t)G * 8, &dal)) return e;
     if (int e = ensure(c, kBufE, (size_t)G * 8, &dconv)) return e;
-    if (prior_reg && !(prior_disp_var > 0.0)) return fail(c, PDQ_ERR_INVALID, "alpha_mle: prior_reg needs prior_disp_var > 0");
     void* status;
     if (int e = ensure(c, kBufStatus, (size_t)G * sizeof(int), &status)) return e;
     Pipe pp;
@@ -1525,9 +1534,9 @@ extern "C" int pdq_alpha_mle(pdq_ctx* c, const int64_t* counts, int64_t ld, int 
             if (int e = cols_h2d(c, pp, b, dc, G, counts, ld, N, 8)) return e;
         if (up_m)
             if (int e = cols_h2d(c, pp, b, dmu, G, mu, ld_mu, N, 8)) return e;
-        if (int e = done(c, launch_alpha_mle(pp.cfg_for(b, N), d->d, (const int64_t*)dc + g0, G, gb, (const double*)dmu + g0, G,
-                                             (const double*)dah + g0, min_disp, max_disp, prior_disp_var, nullptr, cr_reg, prior_reg,
-                                             (double*)dal + g0, (double*)dconv + g0, (int*)status + g0), "alpha_mle"))
+        if (int e = alpha_mle_op(c, pp.cfg_for(b, N), d->d, (const int64_t*)dc + g0, G, gb, (const double*)dmu + g0, G, (const double*)dah + g0,
+                                 min_disp, max_disp, prior_disp_var, nullptr, cr_reg, prior_reg, (double*)dal + g0, (double*)dconv + g0,
+                                 (int*)status + g0))
             return e;
     }
     if (int e = pipe_join(c, pp)) return e;
@@ -1542,9 +1551,10 @@ extern "C" int pdq_wald_test(pdq_ctx* c, const double* X, int N, int p, const do
     CHECK_CTX(c);
     if (!X || !disp || !lfc || !mu || !ridge || !contrast || !pv_out || !stat_out || !se_out || N <= 0 || G <= 0 || ld_mu < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_test: bad arguments");
+    if (int e = design_width(c, p)) return e;
+    if (int e = check_alt(c, alt, "pdq_wald_test: unknown alternative")) return e;
     pdq_design* d;
     if (int e = cached_design(c, X, nullptr, N, p, &d)) return e;
-    const size_t ng = (size_t)N * G;
     void *dmu, *ddisp, *dlfc, *dp, *ds, *dse;
     res_begin(c);
     bool up_m;
@@ -1554,7 +1564,6 @@ extern "C" int pdq_wald_test(pdq_ctx* c, const double* X, int N, int p, const do
     if (int e = ensure(c, kBufE, (size_t)G * 8, &dp)) return e;
     if (int e = ensure(c, kBufF, (size_t)G * 8, &ds)) return e;
     if (int e = ensure(c, kBufG, (size_t)G * 8, &dse)) return e;
-    if (alt < 0 || alt > 4) return fail(c, PDQ_ERR_INVALID, "pdq_wald_test: unknown alternative");
     Pipe pp;
     if (int e = vec_h2d(c, ddisp, disp, (size_t)G * 8)) return e;
     if (int e = vec_h2d(c, dlfc, lfc, (size_t)G * p * 8)) return e;
@@ -1584,10 +1593,7 @@ extern "C" int pdq_wald_contrasts(pdq_ctx* c, const double* X, const double* sf,
     if (!X || !sf || !disp || !lfc || !ridge || !contrasts || !lfc_null || !alt || !pv_out || !stat_out || !se_out || N <= 0 || p <= 0 ||
         G <= 0 || K <= 0 || ld_out < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: bad arguments");
-    if (p > PDQ_MAX_P && !c->wide)
-        return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; this build supports p <= %d", p, PDQ_MAX_P);
-    if (p > max_p(c))
-        return fail(c, PDQ_ERR_UNSUPPORTED, "pdq_wald_contrasts: design has %d columns; wide designs support p <= %d", p, max_p(c));
+    if (int e = design_width(c, p, false, "pdq_wald_contrasts: ")) return e;
     std::vector<double> tab((size_t)K * (p + 2));
     if (const int k = wald_contrast_table(K, p, contrasts, lfc_null, alt, tab.data()); k >= 0)
         return fail(c, PDQ_ERR_INVALID, "pdq_wald_contrasts: unknown alternative %d (contrast %d)", alt[k], k);
@@ -1614,16 +1620,8 @@ extern "C" int pdq_wald_contrasts(pdq_ctx* c, const double* X, const double* sf,
                                                   gb, ridge, K, (const double*)dtab, (double*)dp + g0, (double*)ds + g0, (double*)dse + g0, G),
                          "wald_contrasts"))
             return e;
-        for (int i = 0; i < 3; ++i) {
-            if (pp.on) {
-                if (int e = cols_d2h(c, pp, b, outs[i], ld_out, douts[i], G, K, 8)) return e;
-            } else if (ld_out == G) {
-                if (int e = copy_d2h(c, outs[i], douts[i], kg * 8)) return e;
-            } else {
-                CU(c, cudaMemcpy2DAsync(outs[i], (size_t)ld_out * 8, douts[i], (size_t)G * 8, (size_t)G * 8, K, cudaMemcpyDeviceToHost,
-                                        c->stream));
-            }
-        }
+        for (int i = 0; i < 3; ++i)
+            if (int e = cols_d2h(c, pp, b, outs[i], ld_out, douts[i], G, K, 8)) return e;
     }
     return call_end(c, &pp, {});
 }
@@ -1632,10 +1630,9 @@ extern "C" int pdq_fit_rough_dispersions(pdq_ctx* c, const double* normed, int64
                                          double* alpha_out) {
     CHECK_CTX(c);
     if (!normed || !X || !alpha_out || N <= 0 || G <= 0 || ld < G) return fail(c, PDQ_ERR_INVALID, "pdq_fit_rough_dispersions: bad arguments");
-    if (N == p) return fail(c, PDQ_ERR_INVALID, "The number of samples and the number of design variables are equal");
+    if (int e = check_not_square(c, N, p)) return e;
     pdq_design* d;
     if (int e = cached_design(c, X, nullptr, N, p, &d)) return e;
-    const size_t ng = (size_t)N * G;
     void *dn, *da;
     res_begin(c);
     bool up_n;
@@ -1657,7 +1654,6 @@ extern "C" int pdq_fit_moments_dispersions(pdq_ctx* c, const double* normed, int
     std::vector<double> ones((size_t)N, 1.0);
     pdq_design* d;
     if (int e = cached_design(c, ones.data(), sf, N, 1, &d)) return e;
-    const size_t ng = (size_t)N * G;
     void *dn, *da, *dz;
     res_begin(c);
     bool up_n;
@@ -1715,13 +1711,11 @@ extern "C" int pdq_lfc_shrink_nbinom_glm(pdq_ctx* c, const double* X, const int6
     CHECK_CTX(c);
     if (!X || !counts || !size || !offset || !lfcs_out || !inv_hessians_out || !conv_out || N <= 0 || G <= 0 || ld < G)
         return fail(c, PDQ_ERR_INVALID, "pdq_lfc_shrink_nbinom_glm: bad arguments");
+    if (int e = design_width(c, p)) return e;
+    if (int e = design_width(c, p, true)) return e;
+    if (int e = check_shrink(c, p, shrink_index, prior_no_shrink_scale, prior_scale)) return e;
     pdq_design* d;  // the kernel reads the offsets from the log-size-factor row of the design pack
     if (int e = cached_design(c, X, offset, N, p, &d, true)) return e;
-    if (p > PDQ_MAX_P && !c->wide_shrink)
-        return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented", PDQ_MAX_P);
-    if (p > PDQ_MAX_P_WIDE && !c->large_shrink)  // with or without wide shrinkage
-        return fail(c, PDQ_ERR_UNSUPPORTED, "lfc_shrink: apeGLM shrinkage of designs with more than %d columns is not implemented",
-                    PDQ_MAX_P_WIDE);
     void *dc, *dsize, *dbeta, *dih, *dconv, *status;
     res_begin(c);
     bool up_c;
@@ -1734,6 +1728,7 @@ extern "C" int pdq_lfc_shrink_nbinom_glm(pdq_ctx* c, const double* X, const int6
     if (up_c)
         if (int e = h2d_2d(c, dc, counts, ld, N, G, 8)) return e;
     CU(c, cudaMemcpyAsync(dsize, size, (size_t)G * 8, cudaMemcpyHostToDevice, c->stream));
+    // the one launch site of apeGLM shrinkage, whose checks (passed above, before anything was staged) it runs again
     if (int e = pdq_lfc_shrink_dev(c, d, (const int64_t*)dc, G, G, (const double*)dsize, prior_no_shrink_scale, prior_scale, shrink_index,
                                    (double*)dbeta, (double*)dih, (double*)dconv, (int*)status))
         return e;
@@ -1835,12 +1830,7 @@ extern "C" int pdq_vst_transform(pdq_ctx* c, const int64_t* counts, int64_t ld, 
                                                  c0, c1, (double*)dout + pp.g0(b), G),
                          "vst_transform"))
             return e;
-        if (ld_out == G) {
-            if (int e = cols_d2h(c, pp, b, out, G, dout, G, N, 8)) return e;
-        } else {
-            CU(c, cudaMemcpy2DAsync((char*)out + (size_t)pp.g0(b) * 8, (size_t)ld_out * 8, (const char*)dout + (size_t)pp.g0(b) * 8,
-                                    (size_t)G * 8, (size_t)pp.gb(b) * 8, N, cudaMemcpyDeviceToHost, pp.st(b)));
-        }
+        if (int e = cols_d2h(c, pp, b, out, ld_out, dout, G, N, 8)) return e;
     }
     return call_end(c, &pp, {});
 }
