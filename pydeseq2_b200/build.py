@@ -10,16 +10,18 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libpydeseq2_b200.so")
-# translation units: (source, object tag, extra defines).  pdq_kernels.cu is compiled once for p = 1..8 and once per wide design
-# width p = 9..16 (see the note at its top); pdq_wide.cu holds the kernels of designs of 17..128 columns, one build for every width
-# (p is a run-time argument there; 65..128 columns are its team-per-gene instantiations).  The units are independent and compile in parallel.
+# translation units: (source, object tag, extra defines).  pdq_kernels.cu holds the per-gene kernels of designs of up to 16 columns
+# and is compiled once for p = 1..8 and once per wide design width p = 9..16 (see the note at its top); pdq_wide.cu holds the
+# kernels of designs of 17..128 columns, one build for every width (p is a run-time argument there; 65..128 columns are its
+# team-per-gene instantiations); pdq_common.cu holds the kernels that do not depend on the design width.  The units are independent
+# and compile in parallel.
 WIDE_P = tuple(range(9, 17))
 UNITS = [("pdq_api.cu", "pdq_api", ()), ("pdq_dispatch.cu", "pdq_dispatch", ()), ("pdq_io.cpp", "pdq_io", ()), ("pdq_padj.cu", "pdq_padj", ()), ("pdq_wide.cu", "pdq_wide", ()),
-         ("pdq_kernels.cu", "pdq_kernels_p1to8", ())] + \
+         ("pdq_common.cu", "pdq_common", ()), ("pdq_kernels.cu", "pdq_kernels_p1to8", ())] + \
         [("pdq_kernels.cu", f"pdq_kernels_p{p}", (f"-DPDQ_TU_P={p}", "-Xptxas", "-O1")) for p in WIDE_P]
 # (ptxas -O1 for the wide widths: 12 s instead of 85 s per unit; their kernels keep the small matrices in local memory anyway)
 SOURCES = sorted({u[0] for u in UNITS})
-HEADERS = ["pdq_math.cuh", "pdq_fast.cuh", "pdq_tables.h", "pdq_trend.cuh", "pdq_gene.cuh", "pdq_shrink.cuh", "pdq_vst.cuh", "pdq_padj.cuh", "pdq_team.cuh", "pdq_internal.h",
+HEADERS = ["pdq_math.cuh", "pdq_fast.cuh", "pdq_tables.h", "pdq_trend.cuh", "pdq_gene.cuh", "pdq_shrink.cuh", "pdq_vst.cuh", "pdq_padj.cuh", "pdq_team.cuh", "pdq_launch.cuh", "pdq_internal.h",
            "pdq_host_linalg.h", os.path.join("..", "..", "include", "pydeseq2_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-fopenmp", "--expt-relaxed-constexpr"]

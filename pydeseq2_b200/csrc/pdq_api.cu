@@ -1,6 +1,6 @@
 // pdq_api.cu -- the C ABI declared in include/pydeseq2_b200.h (context, memory, host-buffer and
 // device-resident entry points, NCCL gene-shard exchange).  Host code only; kernels live in
-// pdq_kernels.cu.
+// pdq_kernels.cu, pdq_wide.cu, pdq_common.cu and pdq_padj.cu.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <math.h>
@@ -960,7 +960,8 @@ extern "C" int pdq_size_factors_dev(pdq_ctx* c, const int64_t* counts, int64_t l
     if (!lm)
         if (int e = ensure(c, kBufF, (size_t)G * 8, &lm)) return e;
     if (int e = ensure(c, kBufB, (size_t)N * G * 8, &scratch)) return e;
-    return done(c, launch_size_factors(cfg(c, G, N), counts, ld, N, G, (double*)lm, (double*)scratch, sf_out), "size_factors");
+    return done(c, launch_size_factors_ex(cfg(c, G, N), counts, ld, N, G, 0 /* ratio */, nullptr, (double*)lm, nullptr, (double*)scratch, sf_out),
+                "size_factors");
 }
 
 static int sf_ex_check(pdq_ctx* c, const void* counts, const void* sf_out, int64_t ld, int N, int G, int kind, const char* what) {

@@ -1,8 +1,9 @@
 // pdq_dispatch.cu -- routes a launch to the translation unit that owns the design's width.
 //
-// pdq_kernels.cu is compiled once for p = 1..8 (p x p algebra unrolled in registers) and once per wide width p = 9..16
-// (same source, the small matrices in local memory): see the note at the top of that file and pydeseq2_b200/build.py.  Every
-// unit exports its launchers under a suffixed name; the functions declared in pdq_internal.h live here.  Designs of 17..128
+// pdq_kernels.cu holds the per-gene kernels and is compiled once for p = 1..8 (p x p algebra unrolled in registers) and once per
+// wide width p = 9..16 (same source, the small matrices in local memory): see the note at the top of that file and
+// pydeseq2_b200/build.py.  Every unit exports its launchers under a suffixed name; the per-gene launchers declared in
+// pdq_internal.h live here (those that do not depend on the design width are in pdq_common.cu).  Designs of 17..128
 // columns (only created on contexts that opted in: 65..128 columns are a second opt-in) go to pdq_wide.cu's launchers (`_wide`),
 // which pick the team width from the design.  The fused MAP -> LFC pair has none and reports PDQ_ERR_UNSUPPORTED for them;
 // apeGLM shrinkage reaches its wide launcher only on a context that also opted in to wide shrinkage (pdq_set_wide_shrink,

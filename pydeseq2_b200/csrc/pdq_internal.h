@@ -1,4 +1,4 @@
-// pdq_internal.h -- host-side declarations shared by pdq_api.cu (C ABI) and pdq_kernels.cu (launchers).
+// pdq_internal.h -- host-side declarations shared by pdq_api.cu (C ABI) and the kernel units (launchers).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -50,7 +50,8 @@ struct WaldHost {
     double *pv, *stat, *se;  // device, one per gene
 };
 
-// launchers (pdq_kernels.cu); each returns the number of kernels launched or a negative pdq_status
+// launchers: those that take a DesignDev route by width (pdq_dispatch.cu) to pdq_kernels.cu or pdq_wide.cu, the others are in
+// pdq_common.cu; each returns the number of kernels launched or a negative pdq_status
 int launch_lin_reg_mu(const LaunchCfg&, const DesignDev&, const int64_t* counts, int64_t ld, int G, double min_mu,
                       double* mu_out, int64_t ld_out);
 int launch_irls(const LaunchCfg&, const DesignDev&, const int64_t* counts, int64_t ld, int G, const double* disp,
@@ -115,8 +116,6 @@ constexpr int kMaxScatterSegs = 16;
 int launch_scatter_segments(cudaStream_t stream, const double* in, double* out, const int* src, int nseg, const int64_t* seg);
 int launch_hash(cudaStream_t stream, int sm_count, const void* dptr, size_t words, uint64_t* out2 /* device, zeroed */);
 int launch_fp64_peak(const LaunchCfg&, double* out /* sm_count * 8 * 256 doubles */, int iters, double* flop);
-int launch_size_factors(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, double* logmeans,
-                        double* scratch, double* sf_out);
 // kind kSfRatio / kSfPoscounts (pdq_trend.cuh); `control` (G,) may be NULL; `kept` (G,) scratch, NULL only for ratio over every gene
 int launch_size_factors_ex(const LaunchCfg&, const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control,
                            double* logmeans, double* kept, double* scratch, double* sf_out);

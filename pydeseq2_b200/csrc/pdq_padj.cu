@@ -13,6 +13,7 @@
 #include <cub/cub.cuh>
 
 #include "pdq_internal.h"
+#include "pdq_launch.cuh"
 #include "pdq_padj.cuh"
 
 namespace pdq {
@@ -245,7 +246,7 @@ int sort_rows(const PadjScratch& s, int G, int K, cudaStream_t st) {
 int keys(const PadjScratch& s, int G, int K, const double* row_cutoff, cudaStream_t st) {
     if (cudaMemsetAsync(s.counters, 0, (size_t)(K + 1) * sizeof(int), st) != cudaSuccess) return PDQ_ERR_CUDA;
     k_padj_keys<<<dim3((G + kTPB - 1) / kTPB, K), kTPB, 0, st>>>(s.keys_in, s.vals_in, G, s.bm, row_cutoff, s.counters, s.counters + K);
-    if (cudaGetLastError() != cudaSuccess) return PDQ_ERR_CUDA;
+    if (int e = check_launch()) return e;
     const int r = sort_rows(s, G, K, st);
     return r < 0 ? r : r + 1;
 }
@@ -290,7 +291,7 @@ int launch_padj_rejections(cudaStream_t st, const PadjScratch& s, int G, int K, 
     if (cub::DeviceRadixSort::SortKeys(s.temp, tb, s.bm, s.bm_sorted, G, 0, 64, st) != cudaSuccess) return PDQ_ERR_CUDA;
     k_padj_cutoffs<<<1, kPadjMaxTheta, 0, st>>>(s.bm_sorted, G, s.theta, n_theta, s.cutoffs);
     k_padj_masks<<<gb, kTPB, 0, st>>>(s.bm, G, s.cutoffs, n_theta, s.masks);
-    if (cudaGetLastError() != cudaSuccess) return PDQ_ERR_CUDA;
+    if (int e = check_launch()) return e;
     const int nk = keys(s, G, K, nullptr, st);
     if (nk < 0) return nk;
     if (cudaMemsetAsync(s.num_rej, 0, (size_t)K * n_theta * 4, st) != cudaSuccess) return PDQ_ERR_CUDA;
@@ -298,7 +299,7 @@ int launch_padj_rejections(cudaStream_t st, const PadjScratch& s, int G, int K, 
     k_padj_scan<<<K * n_theta, kTPB, 0, st>>>(s.chunk_counts, nc, s.totals);
     k_padj_reject<<<dim3(nc, K), kTPB, 0, st>>>(s.keys, s.vals, s.masks, s.counters, s.chunk_counts, s.totals, G, n_theta, nc, alpha,
                                                 s.num_rej);
-    if (cudaGetLastError() != cudaSuccess) return PDQ_ERR_CUDA;
+    if (int e = check_launch()) return e;
     return 1 + 2 + nk + 3;
 }
 
@@ -309,7 +310,7 @@ int launch_padj_bh(cudaStream_t st, const PadjScratch& s, int G, int K, double* 
     k_padj_bh_min<<<dim3(nc, K), kTPB, 0, st>>>(s.keys, s.counters, G, nc, s.chunk_min);
     k_padj_bh_suffix<<<K, kTPB, 0, st>>>(s.chunk_min, nc, s.suffix);
     k_padj_bh_out<<<dim3(nc, K), kTPB, 0, st>>>(s.keys, s.vals, s.counters, G, nc, s.suffix, padj, ld_out);
-    if (cudaGetLastError() != cudaSuccess) return PDQ_ERR_CUDA;
+    if (int e = check_launch()) return e;
     return nk + 3;
 }
 

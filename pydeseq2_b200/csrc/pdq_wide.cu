@@ -30,6 +30,7 @@
 
 #include "pdq_gene.cuh"
 #include "pdq_internal.h"
+#include "pdq_launch.cuh"
 #include "pdq_shrink.cuh"
 #include "pdq_team.cuh"
 
@@ -1138,15 +1139,6 @@ template __global__ void k_wide_lfc_shrink<1>(const __grid_constant__ ShrinkArgs
 // ---------------------------------------------------------------------------------------------
 // launch helpers
 // ---------------------------------------------------------------------------------------------
-template <class K>
-int prep(K kernel, size_t smem) {
-    if (smem > kMaxDynSmem) return PDQ_ERR_UNSUPPORTED;
-    if (smem > 48 * 1024 && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return PDQ_ERR_CUDA;
-    return 0;
-}
-
-inline int check_launch() { return cudaGetLastError() == cudaSuccess ? 0 : PDQ_ERR_CUDA; }
 inline size_t ws_bytes(int p, int W = 1) { return wide_ws_doubles(p, W) * sizeof(double); }
 inline WideBase base_of(const DesignDev& d, int G) { return WideBase{d.pack, d.pinv_dev, d.N, d.p, G}; }
 
@@ -1223,10 +1215,10 @@ int with_warps(const DesignDev& d, F&& f, WsBytes ws = ws_bytes) {
     }
 }
 
-// one block of W warps per gene with its workspace; returns the number of launches, the `puts` Wald uploads included
+// one block of W warps per gene with its workspace of ws(p, W) bytes; returns the number of launches, the `puts` Wald uploads included
 template <int W, class A>
-int launch_team(const LaunchCfg& c, const DesignDev& d, int G, void (*kernel)(A), const A& a, int puts = 0) {
-    const size_t smem = ws_bytes(d.p, W);
+int launch_team(const LaunchCfg& c, const DesignDev& d, int G, void (*kernel)(A), const A& a, int puts = 0, WsBytes ws = ws_bytes) {
+    const size_t smem = ws(d.p, W);
     if (int e = prep(kernel, smem)) return e;
     kernel<<<G, 32 * W, smem, c.stream>>>(a);
     if (int e = check_launch()) return e;
@@ -1247,12 +1239,11 @@ int launch_irls_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* coun
     int puts = 0;
     IrlsArgsW a{};
     a.b = base_of(d, G);
-    a.prm = IrlsParams{h.min_mu, h.beta_tol, h.min_beta, h.max_beta, h.maxiter, d.full_rank, d.few_rows,
-                       (c.debug & PDQ_DEBUG_FAIL_IRLS_OPTIMIZER) ? 1 : 0};
+    a.prm = irls_params(h, d, c.debug);
     a.counts = counts; a.ld = ld; a.disp = disp;
     a.beta = beta; a.mu = mu; a.hat = hat; a.conv = conv; a.ld_out = ld_out;
     a.status = status; a.n_fallback = n_fallback;
-    a.force = (c.debug & PDQ_DEBUG_FORCE_IRLS_OPTIMIZER) ? 1 : 0;
+    a.force = hook(c.debug, PDQ_DEBUG_FORCE_IRLS_OPTIMIZER);
     a.with_wald = w ? 1 : 0;
     if (w) {
         if ((puts = put_wald(c, d, w->ridge, w->contrast, a.wald)) < 0) return puts;
@@ -1266,8 +1257,8 @@ int launch_irls_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* coun
 int launch_alpha_mle_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, int64_t ld_mu,
                           const double* alpha_hat, double min_disp, double max_disp, double prior_var, const double* prior_var_dev, int cr_reg,
                           int prior_reg, double* alpha, double* conv, int* status, const double* hint_in, double* hint_out) {
-    const AlphaArgsW a{base_of(d, G), AlphaParams{log(min_disp), log(max_disp), prior_var, cr_reg, prior_reg}, counts, ld, mu, ld_mu,
-                       alpha_hat, alpha, conv, status, prior_var_dev, (c.debug & PDQ_DEBUG_FORCE_ALPHA_GRID) ? 1 : 0, hint_in, hint_out};
+    const AlphaArgsW a{base_of(d, G), alpha_params(min_disp, max_disp, prior_var, cr_reg, prior_reg), counts, ld, mu, ld_mu,
+                       alpha_hat, alpha, conv, status, prior_var_dev, hook(c.debug, PDQ_DEBUG_FORCE_ALPHA_GRID), hint_in, hint_out};
     return with_warps(d, [&](auto w) { return launch_team<decltype(w)::value>(c, d, G, k_wide_alpha_mle<decltype(w)::value>, a); });
 }
 
@@ -1337,15 +1328,7 @@ int launch_lfc_shrink_wide(const LaunchCfg& c, const DesignDev& d, const int64_t
     const ShrinkArgsW a{base_of(d, G), ShrinkParams{1.0 / (prior_no_shrink_scale * prior_no_shrink_scale), prior_scale * prior_scale, shrink_index},
                         counts, ld, size, beta, inv_hessian, conv, status};
     return with_warps(
-        d,
-        [&](auto tw) {
-            constexpr int W = decltype(tw)::value;
-            const size_t smem = shrink_ws_bytes(d.p, W);
-            if (int e = prep(k_wide_lfc_shrink<W>, smem)) return e;
-            k_wide_lfc_shrink<W><<<G, 32 * W, smem, c.stream>>>(a);
-            if (int e = check_launch()) return e;
-            return 1;
-        },
+        d, [&](auto w) { return launch_team<decltype(w)::value>(c, d, G, k_wide_lfc_shrink<decltype(w)::value>, a, 0, shrink_ws_bytes); },
         shrink_ws_bytes);
 }
 
