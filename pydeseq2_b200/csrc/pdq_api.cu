@@ -123,7 +123,7 @@ struct NcclApi {
 };
 static const int kNcclFloat64 = 8;  // ncclDataType_t::ncclFloat64 (stable across NCCL 2.x)
 
-enum { kBufCounts, kBufA, kBufB, kBufC, kBufD, kBufE, kBufF, kBufG, kBufStatus, kBufMisc, kBufKeep, kBufRes, kBufPadj, kNumBufs };
+enum { kBufCounts, kBufA, kBufB, kBufC, kBufD, kBufE, kBufF, kBufG, kBufStatus, kBufMisc, kBufKeep, kBufRes, kBufPadj, kBufCooks, kNumBufs };
 
 struct DesignCacheEntry {
     pdq_design* d = nullptr;
@@ -949,8 +949,11 @@ extern "C" int pdq_cooks_dev(pdq_ctx* c, const pdq_design* d, const int64_t* cou
     if (!d || !counts || !mu || !hat || !robust_disp_out || !outlier_out || !replaced_out || G <= 0 || ld < G || ld2 < G ||
         (cooks_out && ld_out < G))
         return fail(c, PDQ_ERR_INVALID, "pdq_cooks_dev: bad arguments");
+    void* ws = nullptr;
+    if (const size_t bytes = cooks_ws_bytes(d->d, G))
+        if (int e = ensure(c, kBufCooks, bytes, &ws)) return e;
     return done(c, launch_cooks(cfg(c, G, d->d.N), d->d, counts, ld, G, mu, hat, ld2, cutoff, cooks_out, ld_out, robust_disp_out, outlier_out,
-                                replaced_out), "cooks");
+                                replaced_out, (double*)ws), "cooks");
 }
 
 extern "C" int pdq_size_factors_dev(pdq_ctx* c, const int64_t* counts, int64_t ld, int N, int G, double* sf_out, double* logmeans_out) {

@@ -731,6 +731,12 @@ int launch_trend_eval(const LaunchCfg& c, const double* means, size_t n, const d
     return 1;
 }
 
+size_t cooks_ws_bytes(const DesignDev& d, int G) {
+    if (cooks_in_smem(d)) return 0;
+    const size_t chunk = (size_t)cooks_chunk(d), genes = ((size_t)G + kWarps - 1) / kWarps * kWarps;
+    return (genes < chunk ? genes : chunk) * cooks_gene_bytes(d);
+}
+
 int launch_gather_cols(cudaStream_t stream, const double* in, int64_t ld_in, int N, const int* idx, int R, double* out, int64_t ld_out) {
     if (R <= 0 || N <= 0) return 0;
     k_gather_cols<<<dim3((unsigned)((R + 127) / 128), (unsigned)N), 128, 0, stream>>>(in, ld_in, N, idx, R, out, ld_out);

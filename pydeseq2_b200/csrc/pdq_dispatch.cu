@@ -135,11 +135,11 @@ int launch_mu_from_lfc(const LaunchCfg& c, const DesignDev& d, const double* lfc
 
 #define DECL_COOKS(sfx)                                                                                                          \
     int launch_cooks##sfx(const LaunchCfg&, const DesignDev&, const int64_t*, int64_t, int, const double*, const double*, int64_t, \
-                          double, double*, int64_t, double*, double*, double*);
+                          double, double*, int64_t, double*, double*, double*, double*);
 PDQ_UNITS_ALL(DECL_COOKS)
 int launch_cooks(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
-                 int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced) {
-    PDQ_ROUTE_WIDE(launch_cooks, d.p, c, d, counts, ld, G, mu, hat, ld2, cutoff, cooks, ld_out, disp, outlier, replaced)
+                 int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced, double* ws) {
+    PDQ_ROUTE_WIDE(launch_cooks, d.p, c, d, counts, ld, G, mu, hat, ld2, cutoff, cooks, ld_out, disp, outlier, replaced, ws)
 }
 
 #define DECL_SHRINK(sfx)                                                                                                      \

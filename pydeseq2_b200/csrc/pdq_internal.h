@@ -103,8 +103,12 @@ int launch_mu_from_lfc(const LaunchCfg&, const DesignDev&, const double* lfc, in
 int launch_trend_fit(const LaunchCfg&, const double* x, const double* t, double* scratch3n, size_t n, int x_is_mean,
                      double lo, double hi, int outer, double min_disp, double trigamma_c, int with_prior, double* out16);
 int launch_trend_eval(const LaunchCfg&, const double* means, size_t n, const double* out16, double* fitted);
+// `ws`: cooks_ws_bytes(d, G) bytes of device workspace, null when that is 0
 int launch_cooks(const LaunchCfg&, const DesignDev&, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
-                 int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced);
+                 int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced, double* ws);
+// bytes of the global workspace launch_cooks stages the genes' cell members in: 0 where they fit in shared memory (see
+// cooks_in_smem, pdq_launch.cuh)
+size_t cooks_ws_bytes(const DesignDev& d, int G);
 int launch_lfc_shrink(const LaunchCfg&, const DesignDev&, const int64_t* counts, int64_t ld, int G, const double* size,
                       double prior_no_shrink_scale, double prior_scale, int shrink_index, double* beta, double* inv_hessian,
                       double* conv, int* status);

@@ -712,24 +712,30 @@ struct CooksArgs {
     double* cooks;
     int64_t ld_out;
     double *disp, *outlier, *replaced;
+    double* ws;  // null: the cell plan and the genes' cell members in shared memory; else the members in ws, one slot per gene
 };
 
-// Cook's distances + trimmed-moments dispersions (dds.py:986-1040); the gene's cell members are staged in shared memory
+// Cook's distances + trimmed-moments dispersions (dds.py:986-1040); the gene's cell members are staged in shared memory, or in
+// the global workspace where they do not fit (cooks_in_smem)
 template <int P>
 __global__ void __launch_bounds__(kBlock) k_cooks(const __grid_constant__ CooksArgs<P> a) {
     extern __shared__ __align__(128) unsigned char smem[];
     const DesignS d = stage_design(a.dv, P, smem);
     int* plan_s = reinterpret_cast<int*>(smem + scratch_off(a.dv, false));
-    for (int i = threadIdx.x; i < a.plan_len; i += blockDim.x) plan_s[i] = a.plan[i];
+    if (!a.ws)
+        for (int i = threadIdx.x; i < a.plan_len; i += blockDim.x) plan_s[i] = a.plan[i];
     __syncthreads();
     Group grp;
     int g;
     bool valid;
     map_lanes(a.lgT, a.G, grp, g, valid);
-    const CellPlan plan{plan_s + 2 + a.n_cells + 1, plan_s + 2, a.n_cells, plan_s[1]};
+    const int* pl = a.ws ? a.plan : plan_s;
+    const CellPlan plan{pl + 2 + a.n_cells + 1, pl + 2, a.n_cells, pl[1]};
     const size_t plan_bytes = ((size_t)a.plan_len * 4 + 15) & ~(size_t)15;
     const int gslot = (threadIdx.x >> 5) * grp.gpw + ((threadIdx.x & 31) & (grp.gpw - 1));
-    double* vals = reinterpret_cast<double*>(smem + scratch_off(a.dv, false) + plan_bytes) + (size_t)gslot * 2 * a.n_in_cells;
+    // the slots of the lanes map_lanes marks invalid lie past G - 1's: they never share one with a valid gene
+    double* vals = a.ws ? a.ws + ((size_t)blockIdx.x * kWarps * grp.gpw + gslot) * 2 * a.n_in_cells
+                        : reinterpret_cast<double*>(smem + scratch_off(a.dv, false) + plan_bytes) + (size_t)gslot * 2 * a.n_in_cells;
     cooks_gene<P>(grp, d, plan, a.counts + g, a.ld, a.mu + g, a.hat + g, a.ld2, a.cutoff, vals, vals + a.n_in_cells,
                   a.cooks ? a.cooks + g : nullptr, a.ld_out, a.disp + g, a.outlier + g, a.replaced + g, valid);
 }
@@ -1098,20 +1104,25 @@ int PDQ_TUFN(launch_mu_from_lfc)(const LaunchCfg& c, const DesignDev& d, const d
 }
 
 int PDQ_TUFN(launch_cooks)(const LaunchCfg& c0, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
-                 int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced) {
-    // the per-gene staging (2 * n_in_cells doubles) bounds the genes per block: widen the lane groups until it fits
+                 int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced, double* ws) {
+    // the per-gene staging (2 * n_in_cells doubles) bounds the genes per block: widen the lane groups until it fits, and past 32
+    // lanes stage in the workspace, cooks_chunk genes per launch
     LaunchCfg c = c0;
-    const size_t plan_bytes = ((size_t)d.plan_len * 4 + 15) & ~(size_t)15;
-    auto need = [&](int lgT) { return d.smem_bytes + plan_bytes + (size_t)kWarps * (32 >> lgT) * 2 * d.n_in_cells * sizeof(double); };
-    while (c.lgT < 5 && need(c.lgT) > 96 * 1024) ++c.lgT;
-    if (need(c.lgT) > kMaxDynSmem) return PDQ_ERR_UNSUPPORTED;
+    while (c.lgT < 5 && cooks_smem(d, c.lgT) > 96 * 1024) ++c.lgT;
+    const bool global = !cooks_in_smem(d);
+    const int chunk = global ? cooks_chunk(d) : G;
+    if (global && (!ws || chunk < 1)) return PDQ_ERR_UNSUPPORTED;
+    int launches = 0;
     PDQ_DISPATCH_P(d.p, {
-        CooksArgs<P> a{view_of(d), d.cell_plan, d.plan_len, d.n_cells, d.n_in_cells, counts, ld, G, c.lgT, mu, hat, ld2,
-                       cutoff, cooks, ld_out, disp, outlier, replaced};
-        if (int e = launch_genes(c, k_cooks<P>, a, need(c.lgT), G)) return e;
+        for (int g0 = 0; g0 < G; g0 += chunk, ++launches) {
+            const int n = G - g0 < chunk ? G - g0 : chunk;
+            CooksArgs<P> a{view_of(d), d.cell_plan, d.plan_len, d.n_cells, d.n_in_cells, counts + g0, ld, n, c.lgT, mu + g0, hat + g0, ld2,
+                           cutoff, cooks ? cooks + g0 : nullptr, ld_out, disp + g0, outlier + g0, replaced + g0, global ? ws : nullptr};
+            if (int e = launch_genes(c, k_cooks<P>, a, global ? d.smem_bytes : cooks_smem(d, c.lgT), n)) return e;
+        }
     });
     if (int e = check_launch()) return e;
-    return 1;
+    return launches;
 }
 
 int PDQ_TUFN(launch_lfc_shrink)(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* size,

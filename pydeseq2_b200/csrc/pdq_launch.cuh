@@ -44,6 +44,25 @@ int prep(K kernel, size_t smem) {
 
 inline int check_launch() { return cudaGetLastError() == cudaSuccess ? 0 : PDQ_ERR_CUDA; }
 
+// Cook's distances stage 2 * n_in_cells doubles per gene (cooks_gene_cols).  k_cooks holds a block's kWarps * 32 / T genes next to
+// the design pack and the cell plan, k_wide_cooks one gene.  Where that does not fit in shared memory even at 32 lanes per gene
+// (narrow designs from about 3 400 samples in cells, wide ones from about 14 500), every gene gets a slot of a global workspace
+// instead, and the launchers run the genes in chunks of cooks_chunk genes so that the workspace stays within kCooksWsBytes.
+constexpr size_t kCooksWsBytes = (size_t)1 << 30;
+inline size_t cooks_gene_bytes(const DesignDev& d) { return 2 * (size_t)d.n_in_cells * sizeof(double); }
+inline size_t cooks_plan_bytes(const DesignDev& d) { return ((size_t)d.plan_len * 4 + 15) & ~(size_t)15; }
+inline size_t cooks_smem(const DesignDev& d, int lgT) {  // k_cooks with its genes in shared memory
+    return d.smem_bytes + cooks_plan_bytes(d) + (size_t)kWarps * (32 >> lgT) * cooks_gene_bytes(d);
+}
+inline bool cooks_in_smem(const DesignDev& d) { return (d.p > PDQ_MAX_P ? cooks_gene_bytes(d) : cooks_smem(d, 5)) <= kMaxDynSmem; }
+// genes per launch with the global workspace: a multiple of kWarps (the genes of a k_cooks block at 32 lanes); 0 when not even
+// one block's genes fit in kCooksWsBytes
+inline int cooks_chunk(const DesignDev& d) {
+    size_t k = kCooksWsBytes / cooks_gene_bytes(d);
+    if (k > (size_t)(1 << 30)) k = (size_t)1 << 30;
+    return (int)(k - k % kWarps);
+}
+
 // a test hook of the launch (LaunchCfg::debug, PDQ_DEBUG_*) as the 0 / 1 switch the kernels take
 inline int hook(int debug, int flag) { return (debug & flag) ? 1 : 0; }
 

@@ -806,6 +806,7 @@ struct CooksArgsW {
     double* cooks;
     int64_t ld_out;
     double *disp, *outlier, *replaced;
+    double* ws;  // null: the gene's cell members in shared memory; else in ws, one slot per gene (cooks_in_smem)
 };
 
 __global__ void __launch_bounds__(32) k_wide_cooks(const __grid_constant__ CooksArgsW a) {
@@ -814,7 +815,8 @@ __global__ void __launch_bounds__(32) k_wide_cooks(const __grid_constant__ Cooks
     const DesignS d = design_of(a.b.pack, a.b.N, a.b.p);
     const CellPlan plan{a.plan + 2 + a.n_cells + 1, a.plan + 2, a.n_cells, a.plan[1]};
     const Group grp{lane_id(), 32, 1};
-    cooks_gene_cols(grp, d, a.b.p, plan, a.counts + g, a.ld, a.mu + g, a.hat + g, a.ld2, a.cutoff, wsm, wsm + a.n_in_cells,
+    double* st = a.ws ? a.ws + (size_t)g * 2 * a.n_in_cells : wsm;
+    cooks_gene_cols(grp, d, a.b.p, plan, a.counts + g, a.ld, a.mu + g, a.hat + g, a.ld2, a.cutoff, st, st + a.n_in_cells,
                     a.cooks ? a.cooks + g : nullptr, a.ld_out, a.disp + g, a.outlier + g, a.replaced + g, true);
 }
 
@@ -1311,14 +1313,21 @@ int launch_mu_from_lfc_wide(const LaunchCfg& c, const DesignDev& d, const double
 }
 
 int launch_cooks_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
-                      int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced) {
-    const size_t smem = 2 * (size_t)d.n_in_cells * sizeof(double);
-    const CooksArgsW a{base_of(d, G), d.cell_plan, d.n_cells, d.n_in_cells, counts, ld, mu, hat, ld2, cutoff, cooks, ld_out, disp,
-                       outlier, replaced};
+                      int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced, double* ws) {
+    const bool global = !cooks_in_smem(d);
+    const int chunk = global ? cooks_chunk(d) : G;
+    if (global && (!ws || chunk < 1)) return PDQ_ERR_UNSUPPORTED;
+    const size_t smem = global ? 0 : cooks_gene_bytes(d);
     if (int e = prep(k_wide_cooks, smem)) return e;
-    k_wide_cooks<<<G, 32, smem, c.stream>>>(a);
+    int launches = 0;
+    for (int g0 = 0; g0 < G; g0 += chunk, ++launches) {
+        const int n = G - g0 < chunk ? G - g0 : chunk;
+        const CooksArgsW a{base_of(d, n), d.cell_plan, d.n_cells, d.n_in_cells, counts + g0, ld, mu + g0, hat + g0, ld2, cutoff,
+                           cooks ? cooks + g0 : nullptr, ld_out, disp + g0, outlier + g0, replaced + g0, global ? ws : nullptr};
+        k_wide_cooks<<<n, 32, smem, c.stream>>>(a);
+    }
     if (int e = check_launch()) return e;
-    return 1;
+    return launches;
 }
 
 int launch_lfc_shrink_wide(const LaunchCfg& c, const DesignDev& d, const int64_t* counts, int64_t ld, int G, const double* size,

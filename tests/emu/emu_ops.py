@@ -169,3 +169,10 @@ class EmuOps:
         assert self._lanes().emu_cooks(_p(counts, i64p), C.c_int64(ld), N, G, _p(sf, f64p), _p(X, f64p), p, _p(mu, f64p), _p(hat, f64p),
                                        C.c_int64(ld2), C.c_double(cutoff), _p(cooks, f64p) if cooks is not None else None,
                                        _p(disp, f64p), _p(outlier, f64p), _p(replaced, f64p)) == 0
+
+    def cooks_cols(self, counts, ld, N, G, sf, X, p, mu, hat, ld2, cutoff, cooks, disp, outlier, replaced):
+        """`cooks` with the design width at run time (emu_cooks_cols): the routine k_wide_cooks runs, for any p."""
+        assert self._lanes().emu_cooks_cols(_p(counts, i64p), C.c_int64(ld), N, G, _p(sf, f64p), _p(X, f64p), p, _p(mu, f64p),
+                                            _p(hat, f64p), C.c_int64(ld2), C.c_double(cutoff),
+                                            _p(cooks, f64p) if cooks is not None else None, _p(disp, f64p), _p(outlier, f64p),
+                                            _p(replaced, f64p)) == 0

@@ -398,6 +398,27 @@ int emu_cooks(const int64_t* counts, int64_t ld, int N, int G, const double* sf,
     return 0;
 }
 
+// k_wide_cooks: cooks_gene_cols with the design width `p` at run time (any p >= 1, no template width), at the lane count of
+// emu_set_lanes (the device runs it at 32)
+int emu_cooks_cols(const int64_t* counts, int64_t ld, int N, int G, const double* sf, const double* X, int p, const double* mu,
+                   const double* hat, int64_t ld2, double cutoff, double* cooks, double* disp, double* outlier, double* replaced) {
+    if (p < 1) return -2;
+    std::vector<double> buf;
+    design_pack(X, sf, false, N, p, buf);
+    const DesignS d{buf.data(), buf.data() + p, buf.data() + p + 1, N, design_row_stride(p), host_math_table()};
+    const std::vector<int> plan = design_cell_plan(X, N, p);
+    const int n_cells = plan[0];
+    const int nf = (int)plan.size() - (2 + n_cells + 1);
+    const CellPlan cp{plan.data() + 2 + n_cells + 1, plan.data() + 2, n_cells, plan[1]};
+    std::vector<double> vals((size_t)2 * nf);
+    for (int g = 0; g < G; ++g)
+        with_lanes([&](const Group& grp) {
+            cooks_gene_cols(grp, d, p, cp, counts + g, ld, mu + g, hat + g, ld2, cutoff, vals.data(), vals.data() + nf,
+                            cooks ? cooks + g : nullptr, G, disp + g, outlier + g, replaced + g, true);
+        });
+    return 0;
+}
+
 // pdq_size_factors_ex (k_log_means, k_size_factor_median, k_size_factor_geomean; one "thread"): `control` and `logmeans` (G,), the
 // raw log means, may be NULL; -2 (PDQ_ERR_INVALID) for an unknown kind
 int emu_size_factors_ex(const int64_t* counts, int64_t ld, int N, int G, int kind, const uint8_t* control, double* sf, double* logmeans) {
