@@ -62,8 +62,9 @@ struct TrendSums {
 
 // xs[i]: covariate; ts[i]: target, NaN when the gene is not (or no longer) part of the fit.  Both are prepared once per
 // launch by trend_prepare (clip, 1/mean, validity), so that a pass is: two loads, one reciprocal, one log, ten sums.
+// The sums g1, h01, h11, f01, f11 are taken over the covariate less `xc` (see trend_fit_once); xc = 0 gives the plain sums.
 template <class R>
-PDQ_HD TrendSums trend_sums(R& red, const double* xs, const double* ts, size_t n, double c0, double c1) {
+PDQ_HD TrendSums trend_sums(R& red, const double* xs, const double* ts, size_t n, double c0, double c1, double xc = 0.0) {
     double L = 0, g0 = 0, g1 = 0, h00 = 0, h01 = 0, h11 = 0, f00 = 0, f01 = 0, f11 = 0, cnt = 0;
     for (size_t i = red.tid(); i < n; i += red.nthreads()) {
         const double tv = ts[i];
@@ -74,16 +75,17 @@ PDQ_HD TrendSums trend_sums(R& red, const double* xs, const double* ts, size_t n
         const double r = tv * im;
         L += r + fast_log(m);
         const double gi = -(r - 1.0) * im;             // d/dm (t/m + log m) = (1 - t/m)/m
+        const double xd = xv - xc;
         g0 += gi;
-        g1 += gi * xv;
+        g1 += gi * xd;
         const double hi2 = (2.0 * r - 1.0) * im * im;  // d2/dm2
         h00 += hi2;
-        h01 += hi2 * xv;
-        h11 += hi2 * xv * xv;
+        h01 += hi2 * xd;
+        h11 += hi2 * xd * xd;
         const double fi = im * im;                     // expected (Fisher) curvature
         f00 += fi;
-        f01 += fi * xv;
-        f11 += fi * xv * xv;
+        f01 += fi * xd;
+        f11 += fi * xd * xd;
         cnt += 1.0;
     }
     double v[10] = {L, g0, g1, h00, h01, h11, f00, f01, f11, cnt};
@@ -100,17 +102,44 @@ PDQ_HD TrendSums trend_sums(R& red, const double* xs, const double* ts, size_t n
 // reference (default_inference.py:221); later rounds of the outer loop warm-start from the previous optimum -- the
 // minimiser does not depend on the start, only the iteration count does.  Every trial point costs ONE pass: the sums at
 // the candidate serve both the Armijo test and, once accepted, the next Newton direction.
+//
+// When the covariate is (nearly) constant over the fitted genes, 1 and x are (nearly) collinear: the Fisher determinant
+// f00 f11 - f01^2 is then cancellation, down to rounding noise, and a step through it can land anywhere (inf, or a point
+// that is not a minimiser).  Below kSing f00 f11 the fit measures the covariate from its smallest fitted value xc, once,
+// and solves for the step in (c0 + c1 xc, c1): the same point and the same steps in exact arithmetic, but the terms
+// x - xc are small, and exact wherever x lies within a factor two of xc (Sterbenz), as it does for every nearly constant
+// covariate, so the sums no longer cancel to rounding noise.  Their determinant a d - b^2 still
+// cancels where most of the weight lies far from xc, to about 1/n relative at worst, which double precision resolves.
+// kSing: the relative determinant is the weighted variance of x over its weighted mean square; real covariates (1 / mean over
+// orders of magnitude) sit near 0.1-1, and a uniform spread of s relative gives about s^2 / 3.  1e-5 takes every spread below
+// ~5e-3 (the plain solve failed to reach the minimiser at spreads of 1e-9 to 1e-3) and leaves every realistic fit, and every
+// pinned record, on the plain path.
+// A covariate that is exactly constant leaves only m = c0 + c1 x identified; the step then moves m to its optimum by the
+// shortest step in (c0, c1), which makes the fit the minimiser nearest its start.
 template <class R>
 PDQ_HD bool trend_fit_once(R& red, const double* xs, const double* ts, size_t n, double& c0, double& c1, double& loss,
                            int& iters) {
-    const double kLB = 1e-12;  // bounds=[(1e-12, inf)] (default_inference.py:224)
+    const double kLB = 1e-12;    // bounds=[(1e-12, inf)] (default_inference.py:224)
+    const double kSing = 1e-5;   // relative Fisher determinant below which 1 and x count as nearly collinear (see above)
+    bool centred = false;
+    double xc = 0.0;
     TrendSums s = trend_sums(red, xs, ts, n, c0, c1);
     ++iters;
     for (int it = 0; it < 200; ++it) {
         loss = s.L / s.n;
         if (!(s.L == s.L) || s.n < 2.0) return false;
+        if (!centred && !(s.f00 * s.f11 - s.f01 * s.f01 > kSing * s.f00 * s.f11)) {
+            double mx = -HUGE_VAL;
+            for (size_t i = red.tid(); i < n; i += red.nthreads())
+                if (ts[i] == ts[i]) mx = fmax(mx, -xs[i]);
+            xc = -red.max_one(mx);
+            centred = true;
+            s = trend_sums(red, xs, ts, n, c0, c1, xc);
+            ++iters;
+        }
+        const double gc1 = centred ? fma(xc, s.g0, s.g1) : s.g1;  // dL/dc1
         // variables held at the lower bound with the gradient pushing outward are fixed
-        const bool fix0 = (c0 <= kLB && s.g0 > 0.0), fix1 = (c1 <= kLB && s.g1 > 0.0);
+        const bool fix0 = (c0 <= kLB && s.g0 > 0.0), fix1 = (c1 <= kLB && gc1 > 0.0);
         double d0 = 0.0, d1 = 0.0;
         {
             double a = s.h00, b = s.h01, d = s.h11;
@@ -118,26 +147,35 @@ PDQ_HD bool trend_fit_once(R& red, const double* xs, const double* ts, size_t n,
             if (!pd) { a = s.f00; b = s.f01; d = s.f11; }  // Fisher scoring: always positive definite
             if (fix0 && fix1) return true;
             if (fix0) {
-                d1 = -s.g1 / d;
+                d1 = -gc1 / (centred ? fma(xc, fma(xc, a, 2.0 * b), d) : d);  // curvature in c1 alone: sum w x^2
             } else if (fix1) {
                 d0 = -s.g0 / a;
+            } else if (centred && !(d > 0.0)) {  // every fitted x equals xc: the shortest step that moves m by -g0 / a
+                const double dm = -s.g0 / a, w = 1.0 / fma(xc, xc, 1.0);
+                d0 = dm * w;
+                d1 = dm * xc * w;
             } else {
                 const double det = a * d - b * b;
                 d0 = -(d * s.g0 - b * s.g1) / det;
                 d1 = -(a * s.g1 - b * s.g0) / det;
+                if (centred) d0 = fma(-xc, d1, d0);  // the step in c0 + c1 xc, back to c0
             }
         }
-        const double dec = -(s.g0 * d0 + s.g1 * d1);           // Newton decrement (>= 0 for a descent direction)
+        const double dec = -(s.g0 * d0 + gc1 * d1);             // Newton decrement (>= 0 for a descent direction)
         const bool endgame = dec <= 1e-9 * fabs(s.L);           // the summed loss no longer resolves progress in FP64
-        double step = 1.0, n0 = c0, n1 = c1;
+        // on a nearly constant covariate a step that carries a free coefficient across its bound stops there: projecting the
+        // whole step instead keeps the other coefficient's share of a very long step, far from any minimiser
+        const double a0 = (centred && c0 > kLB && c0 + d0 < kLB) ? (c0 - kLB) / -d0 : HUGE_VAL;
+        const double a1 = (centred && c1 > kLB && c1 + d1 < kLB) ? (c1 - kLB) / -d1 : HUGE_VAL;
+        double step = fmin(1.0, fmin(a0, a1)), n0 = c0, n1 = c1;
         TrendSums sn = s;
         bool acc = false;
         for (int ls = 0; ls < 40; ++ls) {
-            n0 = fmax(fma(step, d0, c0), kLB);
-            n1 = fmax(fma(step, d1, c1), kLB);
-            sn = trend_sums(red, xs, ts, n, n0, n1);
+            n0 = step >= a0 ? kLB : fmax(fma(step, d0, c0), kLB);
+            n1 = step >= a1 ? kLB : fmax(fma(step, d1, c1), kLB);
+            sn = trend_sums(red, xs, ts, n, n0, n1, xc);
             ++iters;
-            if (endgame || sn.L <= s.L + 1e-4 * (s.g0 * (n0 - c0) + s.g1 * (n1 - c1))) {
+            if (endgame || sn.L <= s.L + 1e-4 * (s.g0 * (n0 - c0) + gc1 * (n1 - c1))) {
                 acc = true;
                 break;
             }
