@@ -935,11 +935,9 @@ extern "C" int pdq_trend_fit_dev(pdq_ctx* c, const double* means, const double* 
     void* scratch;
     if (int e = ensure(c, kBufRes, 3 * n * 8, &scratch)) return e;
     LaunchCfg lc{c->stream, 0, c->prop.multiProcessorCount, c->tickets, c->debug, c->grid_scratch};
-    if (int e = done(c, launch_trend_fit(lc, means, genewise, (double*)scratch, n, 1, min_disp, max_disp, 1, min_disp, trigamma_c, 1, out16),
-                     "trend_fit"))
-        return e;
-    if (fitted) return done(c, launch_trend_eval(lc, means, n, out16, fitted), "trend_eval");
-    return PDQ_OK;
+    return done(c, launch_trend_fit(lc, means, genewise, (double*)scratch, n, 1, min_disp, max_disp, 1, min_disp, trigamma_c, 1, out16,
+                                    fitted),
+                "trend_fit");
 }
 
 extern "C" int pdq_cooks_dev(pdq_ctx* c, const pdq_design* d, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,

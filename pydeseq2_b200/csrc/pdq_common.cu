@@ -19,15 +19,14 @@ namespace {
 // ---- dispersion trend + prior: the whole gamma-GLM fit (all iterations, all outer rounds) and the MAD-based prior
 // variance in ONE launch of one thread-block cluster.  Per iteration the blocks reduce their partial sums with warp
 // shuffles + shared memory, exchange the block totals through distributed shared memory (DSMEM stores into every
-// peer's slot table) and meet at one cluster barrier; all blocks then hold identical totals and take identical
-// decisions, so no further communication is needed.
+// peer's slot table) and meet at one cluster barrier; every warp then adds up the same slots in the same order, so all
+// threads hold identical totals and take identical decisions, and no further communication is needed.
 constexpr int kTrendK = 10;        // packed sums per reduction
 constexpr int kTrendMaxCluster = 16;
 
 struct ClusterReducer {
     double* warp_part;  // [32][kTrendK]
     double* slots;      // [2][kTrendMaxCluster][kTrendK], written by every block of the cluster (DSMEM)
-    double* totals;     // [2][kTrendK]: the cluster-wide sums, broadcast to the block's threads
     unsigned rank, nblocks;
     int parity;
     unsigned* vmerged = nullptr;              // [2][kVBins] (median_bins only)
@@ -173,44 +172,37 @@ struct ClusterReducer {
             if (lane == 0) warp_part[warp * kTrendK + j] = w;
         }
         __syncthreads();
-        if ((int)threadIdx.x < ks) {
-            double tot = 0.0;
+        // thread u = r k + j stores the block's value j into peer r's slot table: one DSMEM store per thread instead of a loop over
+        // the peers.  The threads of one j add the warp partials in the same order, so every peer receives the same bits
+        for (unsigned u = threadIdx.x; u < (unsigned)k * nblocks; u += blockDim.x) {
+            const int j = (int)(u % (unsigned)k);
+            const unsigned r = u / (unsigned)k;
             const int nw = blockDim.x >> 5;
-            for (int w = 0; w < nw; ++w) tot += warp_part[w * kTrendK + threadIdx.x];
-            if (nblocks > 1) {
-                for (unsigned r = 0; r < nblocks; ++r) {
-                    double* remote = cluster.map_shared_rank(slots, r);
-                    remote[(parity * kTrendMaxCluster + rank) * kTrendK + threadIdx.x] = tot;
-                }
+            double tot;
+            if (j < ks) {
+                tot = 0.0;
+                for (int w = 0; w < nw; ++w) tot += warp_part[w * kTrendK + j];
             } else {
-                slots[parity * kTrendMaxCluster * kTrendK + threadIdx.x] = tot;
+                tot = warp_part[j];
+                for (int w = 1; w < nw; ++w) tot = fmax(tot, warp_part[w * kTrendK + j]);
             }
-        }
-        if ((int)threadIdx.x >= ks && (int)threadIdx.x < k) {
-            double m = warp_part[threadIdx.x];
-            const int nw = blockDim.x >> 5;
-            for (int w = 1; w < nw; ++w) m = fmax(m, warp_part[w * kTrendK + threadIdx.x]);
-            if (nblocks > 1) {
-                for (unsigned r = 0; r < nblocks; ++r)
-                    cluster.map_shared_rank(slots, r)[(parity * kTrendMaxCluster + rank) * kTrendK + threadIdx.x] = m;
-            } else {
-                slots[parity * kTrendMaxCluster * kTrendK + threadIdx.x] = m;
-            }
+            double* dst = slots + (parity * kTrendMaxCluster + rank) * kTrendK + j;
+            if (nblocks > 1) dst = cluster.map_shared_rank(dst, r);
+            *dst = tot;
         }
         if (nblocks > 1) cluster.sync(); else __syncthreads();  // release the DSMEM stores / acquire the peers'
-        // k threads add up the blocks' slots, everybody reads the k totals (broadcast reads).  Having EVERY thread
-        // add nblocks * k slots itself would cost 160 shared-memory reads per thread and pass.
-        if ((int)threadIdx.x < ks) {
-            double tot = 0.0;
-            for (unsigned r = 0; r < nblocks; ++r) tot += slots[(parity * kTrendMaxCluster + r) * kTrendK + threadIdx.x];
-            totals[parity * kTrendK + threadIdx.x] = tot;
-        } else if ((int)threadIdx.x < k) {
-            double m = slots[parity * kTrendMaxCluster * kTrendK + threadIdx.x];
-            for (unsigned r = 1; r < nblocks; ++r) m = fmax(m, slots[(parity * kTrendMaxCluster + r) * kTrendK + threadIdx.x]);
-            totals[parity * kTrendK + threadIdx.x] = m;
+        // lane j of every warp adds up the blocks' slots of value j, and the warp shares the k totals by shuffles: no block barrier.
+        // Having EVERY thread add nblocks * k slots itself would cost 160 shared-memory reads per thread and pass.  The slots of
+        // this parity are next written two reductions later, behind the next cluster barrier, which every thread reaches only
+        // after these reads
+        double tot = 0.0;
+        if (lane < ks) {
+            for (unsigned r = 0; r < nblocks; ++r) tot += slots[(parity * kTrendMaxCluster + r) * kTrendK + lane];
+        } else if (lane < k) {
+            tot = slots[parity * kTrendMaxCluster * kTrendK + lane];
+            for (unsigned r = 1; r < nblocks; ++r) tot = fmax(tot, slots[(parity * kTrendMaxCluster + r) * kTrendK + lane]);
         }
-        __syncthreads();
-        for (int j = 0; j < k; ++j) v[j] = totals[parity * kTrendK + j];
+        for (int j = 0; j < k; ++j) v[j] = __shfl_sync(0xffffffffu, tot, j);
         parity ^= 1;
 #else
         (void)v;
@@ -281,28 +273,61 @@ struct ClusterReducer {
 #endif
 };
 
-__global__ void __launch_bounds__(1024) k_trend_prior(const double* __restrict__ x, const double* __restrict__ t,
+// The fit's vectors and the prior's residuals, per thread.  LOCAL: xs and ts in the block's dynamic shared memory (`per` elements
+// per thread each; the residuals reuse xs, which the fit no longer reads), read on chip in every pass; otherwise global scratch.
+// Both visit the genes in the same order and do the same arithmetic: the results do not depend on the choice.
+template <bool LOCAL>
+struct TrendVecs;
+template <>
+struct TrendVecs<true> {
+    LocalVec xs, ts, res;
+    __device__ TrendVecs(double* smem, double*, size_t, unsigned per)
+        : xs{smem + threadIdx.x, blockDim.x}, ts{smem + (size_t)per * blockDim.x + threadIdx.x, blockDim.x}, res(xs) {}
+};
+template <>
+struct TrendVecs<false> {
+    double *xs, *ts, *res;
+    __device__ TrendVecs(double*, double* scratch, size_t n, unsigned) : xs(scratch), ts(scratch + n), res(scratch + 2 * n) {}
+};
+
+// fitted = c0 + c1 / mean (dds.py:1267-1275) once the coefficients are final, the genes split as in the fit
+template <class R>
+__device__ void trend_fitted(R& red, const double* means, size_t n, const TrendOut& o, double* fitted) {
+    if (fitted)
+        for (size_t i = red.tid(); i < n; i += red.nthreads()) fitted[i] = o.c0 + o.c1 / means[i];
+}
+
+// MAXT: the largest block the instance runs, 512 or 1024.  The register cap that __launch_bounds__(1024) sets (64) spills the fit's
+// Newton state; blocks of up to 512 threads get 128 registers
+template <bool LOCAL, int MAXT>
+__global__ void __launch_bounds__(MAXT) k_trend_prior(const double* __restrict__ x, const double* __restrict__ t,
                                                       double* scratch /* 3 n doubles: xs | ts | res */, size_t n,
                                                       int x_is_mean, double lo, double hi, int outer, double min_disp,
-                                                      double trigamma_c, int with_prior, TrendOut* out) {
+                                                      double trigamma_c, int with_prior, TrendOut* out, double* fitted,
+                                                      unsigned per) {
+    // the tail of the pass is launched as this kernel's programmatic dependent: its blocks take the idle SMs and stage their
+    // design while the fit runs, and wait for this grid's completion (griddepcontrol.wait) before reading the record or `fitted`
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    extern __shared__ double lvec[];
     __shared__ double warp_part[32 * kTrendK];
     __shared__ double slots[2 * kTrendMaxCluster * kTrendK];
-    __shared__ double totals[2 * kTrendK];
     __shared__ unsigned hist[514];
     __shared__ SelShared sel;
     __shared__ unsigned vmerged[2 * kVBins];
     __shared__ unsigned sel_words[2];
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
-    ClusterReducer red{warp_part, slots, totals, cluster.block_rank(), cluster.num_blocks(), 0, vmerged, sel_words};
+    ClusterReducer red{warp_part, slots, cluster.block_rank(), cluster.num_blocks(), 0, vmerged, sel_words};
     for (int j = threadIdx.x; j < 2 * kVBins; j += blockDim.x) vmerged[j] = 0;  // first used behind the fit's cluster barriers
     if (threadIdx.x < 2) sel_words[threadIdx.x] = 0;
-    double *xs = scratch, *ts = scratch + n, *res = scratch + 2 * n;
-    trend_prepare(red, x, t, n, x_is_mean != 0, lo, hi, xs, ts);
-    TrendOut o = trend_fit_outer(red, xs, ts, n, outer != 0, false);
-    // the prior's candidate buffer reuses xs, last read by the fit before the prior's first cluster barrier
+    const TrendVecs<LOCAL> v(lvec, scratch, n, per);
+    trend_prepare(red, x, t, n, x_is_mean != 0, lo, hi, v.xs, v.ts);
+    TrendOut o = trend_fit_outer(red, v.xs, v.ts, n, outer != 0, false);
+    trend_fitted(red, x, n, o, fitted);
+    // the prior's candidate buffer is the global xs scratch: unused with LOCAL, last read by the fit before the prior's first
+    // cluster barrier otherwise
     if (with_prior && o.status == 0.0)
-        trend_prior_dev(red, x, t, n, lo, hi, min_disp, trigamma_c, res, reinterpret_cast<unsigned long long*>(xs), sel, hist, o);
+        trend_prior_dev(red, x, t, n, lo, hi, min_disp, trigamma_c, v.res, reinterpret_cast<unsigned long long*>(scratch), sel, hist, o);
     else
         red.sum_many(&o.n_used, 1);
     if (red.tid() == 0) *out = o;
@@ -425,25 +450,30 @@ struct GridReducer {
         return hist + 256;
     }
     __device__ void find_bin(const unsigned* hist, unsigned* out, size_t k, int& d, size_t& cum) {
-        ClusterReducer tmp{nullptr, nullptr, nullptr, 0u, 1u, 0};  // the single-block scan of the 256 merged bins
+        ClusterReducer tmp{nullptr, nullptr, 0u, 1u, 0};  // the single-block scan of the 256 merged bins
         tmp.find_bin(hist, out, k, d, cum);
     }
 };
 
+template <bool LOCAL>
 __global__ void __launch_bounds__(1024) k_trend_prior_grid(const double* __restrict__ x, const double* __restrict__ t,
                                                            double* scratch /* 3 n doubles: xs | ts | res */, size_t n, int x_is_mean,
                                                            double lo, double hi, int outer, double min_disp, double trigamma_c,
-                                                           int with_prior, TrendOut* out, GridScratch* gs) {
+                                                           int with_prior, TrendOut* out, GridScratch* gs, double* fitted,
+                                                           unsigned per) {
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // see k_trend_prior
+    extern __shared__ double lvec[];
     __shared__ double warp_part[32 * kTrendK];
     __shared__ double totals[kTrendK];
     __shared__ unsigned hist[514];
     __shared__ SelShared sel;
     GridReducer red{warp_part, totals, gs, 0, 0, 0};
-    double *xs = scratch, *ts = scratch + n, *res = scratch + 2 * n;
-    trend_prepare(red, x, t, n, x_is_mean != 0, lo, hi, xs, ts);
-    TrendOut o = trend_fit_outer(red, xs, ts, n, outer != 0, false);
-    if (with_prior && o.status == 0.0)  // candidate buffer: xs, as in k_trend_prior
-        trend_prior_dev(red, x, t, n, lo, hi, min_disp, trigamma_c, res, reinterpret_cast<unsigned long long*>(xs), sel, hist, o);
+    const TrendVecs<LOCAL> v(lvec, scratch, n, per);
+    trend_prepare(red, x, t, n, x_is_mean != 0, lo, hi, v.xs, v.ts);
+    TrendOut o = trend_fit_outer(red, v.xs, v.ts, n, outer != 0, false);
+    trend_fitted(red, x, n, o, fitted);
+    if (with_prior && o.status == 0.0)  // candidate buffer: the global xs scratch, as in k_trend_prior
+        trend_prior_dev(red, x, t, n, lo, hi, min_disp, trigamma_c, v.res, reinterpret_cast<unsigned long long*>(scratch), sel, hist, o);
     else
         red.sum_many(&o.n_used, 1);
     if (red.tid() == 0) *out = o;
@@ -480,7 +510,6 @@ __global__ void __launch_bounds__(1024) k_size_factor_median(const int64_t* __re
     __shared__ unsigned hist[514];
     __shared__ double warp_part[32 * kTrendK];
     __shared__ double slots[2 * kTrendMaxCluster * kTrendK];
-    __shared__ double totals[2 * kTrendK];
     __shared__ unsigned cnt_s;
     const int n = blockIdx.x;
     double* row = scratch + (size_t)n * G;
@@ -495,7 +524,7 @@ __global__ void __launch_bounds__(1024) k_size_factor_median(const int64_t* __re
     }
     atomicAdd(&cnt_s, cnt);
     __syncthreads();
-    ClusterReducer red{warp_part, slots, totals, 0u, 1u, 0};  // one block per sample: the single-block paths of the reducer
+    ClusterReducer red{warp_part, slots, 0u, 1u, 0};  // one block per sample: the single-block paths of the reducer
     const double med = median_of(red, row, (size_t)G, (size_t)cnt_s, false, 0.0, hist);
     if (threadIdx.x == 0) sf_out[n] = exp(med);
 }
@@ -513,12 +542,6 @@ __global__ void __launch_bounds__(1024) k_size_factor_geomean(double* sf, int N)
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += part[w];
     const double gm = exp(tot / (double)N);
     for (int n = threadIdx.x; n < N; n += blockDim.x) sf[n] = sf[n] / gm;
-}
-
-// fitted = c0 + c1 / mean (dds.py:1267-1275) from the device-resident coefficients
-__global__ void k_trend_eval(const double* __restrict__ means, size_t n, const TrendOut* __restrict__ c, double* fitted) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) fitted[i] = c->c0 + c->c1 / means[i];
 }
 
 // final dispersions (dds.py:918-932), elementwise: select_disp (pdq_gene.cuh) per gene
@@ -649,11 +672,30 @@ __global__ void __launch_bounds__(256) k_hash(const uint64_t* __restrict__ w, si
 
 }  // namespace
 
+// Per-thread share of the fit's two vectors in shared memory, or 0 when they do not fit there (the kernels then keep them in the
+// global scratch).  Within the 227 KB per block beside the kernels' static shared memory (40 KB)
+constexpr size_t kTrendLocalBytes = 160 * 1024;
+static unsigned trend_local_per(size_t n, size_t nthreads, unsigned block) {
+    const size_t per = (n + nthreads - 1) / nthreads;
+    return 2 * per * block * sizeof(double) <= kTrendLocalBytes ? (unsigned)per : 0u;
+}
+
+// The opt-in for the vectors' dynamic shared memory, on every launch: it belongs to the kernel on the current device, and one process
+// may drive several devices.  Not prep(): its 48 KB threshold is for kernels without static shared memory, and these hold 21-40 KB,
+// so that from a few KB of vectors on the block's total passes the 48 KB that needs no opt-in
+template <class K>
+static cudaError_t allow_local(K kernel, size_t smem) {
+    return smem ? cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrendLocalBytes) : cudaSuccess;
+}
+
 int launch_trend_fit(const LaunchCfg& c, const double* x, const double* t, double* scratch3n, size_t n, int x_is_mean,
-                     double lo, double hi, int outer, double min_disp, double trigamma_c, int with_prior, double* out16) {
+                     double lo, double hi, int outer, double min_disp, double trigamma_c, int with_prior, double* out16,
+                     double* fitted) {
     if (const char* e = getenv("PDQ_TREND_PRIOR")) {  // tuning hook: PDQ_TREND_PRIOR=0 skips the prior (times the fit alone)
         if (atoi(e) == 0) with_prior = 0;
     }
+    if (!x_is_mean) fitted = nullptr;
+    TrendOut* o16 = reinterpret_cast<TrendOut*>(out16);
     // large vectors: one block per SM, cooperative launch (k_trend_prior_grid); PDQ_TREND_GRID=0/1 forces the choice
     {
         const char* e = getenv("PDQ_TREND_GRID");
@@ -664,25 +706,19 @@ int launch_trend_fit(const LaunchCfg& c, const double* x, const double* t, doubl
             int blocks = (int)((n + 2047) / 2048);
             if (blocks > c.sm_count) blocks = c.sm_count;
             if (blocks < 1) blocks = 1;
-            TrendOut* o16 = reinterpret_cast<TrendOut*>(out16);
             GridScratch* gs = reinterpret_cast<GridScratch*>(c.grid_scratch);
+            unsigned per = trend_local_per(n, (size_t)blocks * 1024, 1024);
+            const size_t smem = 2 * (size_t)per * 1024 * sizeof(double);
+            auto kernel = per ? k_trend_prior_grid<true> : k_trend_prior_grid<false>;
+            if (allow_local(kernel, smem) != cudaSuccess) return PDQ_ERR_CUDA;
             void* args[] = {(void*)&x, (void*)&t, (void*)&scratch3n, (void*)&n, (void*)&x_is_mean, (void*)&lo, (void*)&hi, (void*)&outer,
-                            (void*)&min_disp, (void*)&trigamma_c, (void*)&with_prior, (void*)&o16, (void*)&gs};
-            if (cudaLaunchCooperativeKernel((const void*)k_trend_prior_grid, dim3(blocks), dim3(1024), args, 0, c.stream) == cudaSuccess) {
+                            (void*)&min_disp, (void*)&trigamma_c, (void*)&with_prior, (void*)&o16, (void*)&gs, (void*)&fitted, (void*)&per};
+            if (cudaLaunchCooperativeKernel((const void*)kernel, dim3(blocks), dim3(1024), args, smem, c.stream) == cudaSuccess) {
                 if (int e = check_launch()) return e;
                 return 1;
             }
             cudaGetLastError();  // cooperative launch not possible here: the cluster version below
         }
-    }
-    // cluster size: enough blocks for ~4 elements per thread; 8 is the portable maximum, 16 needs the opt-in attribute
-    static int max_cluster = 0;
-    if (!max_cluster) {
-        max_cluster = 8;
-        if (cudaFuncSetAttribute(k_trend_prior, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess)
-            max_cluster = kTrendMaxCluster;
-        else
-            cudaGetLastError();
     }
     // threads per block: the per-pass cost of a small fit is the reduction (ten packed sums through warp shuffles and shared
     // memory per warp), not the arithmetic -- 256 threads per block (~5 genes per thread at 20 000 genes) instead of 1024 cut
@@ -692,41 +728,43 @@ int launch_trend_fit(const LaunchCfg& c, const double* x, const double* t, doubl
         const int v = atoi(e);
         if (v == 256 || v == 512 || v == 1024) threads = (unsigned)v;
     }
+    // cluster size: enough blocks for ~4 elements per thread; 8 is the portable maximum, 16 needs the opt-in attribute (see launch)
     unsigned nb = 1;
-    while ((int)nb < max_cluster && (size_t)nb * threads * 4 < n) nb <<= 1;
+    while ((int)nb < kTrendMaxCluster && (size_t)nb * threads * 4 < n) nb <<= 1;
     if (const char* e = getenv("PDQ_TREND_CLUSTER")) {  // tuning hook: force the cluster size (1, 2, 4, 8, 16)
         const int v = atoi(e);
-        if (v >= 1 && v <= max_cluster && !(v & (v - 1))) nb = (unsigned)v;
+        if (v >= 1 && v <= kTrendMaxCluster && !(v & (v - 1))) nb = (unsigned)v;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(nb, 1, 1);
-    cfg.blockDim = dim3(threads, 1, 1);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = c.stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = nb;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t err = cudaLaunchKernelEx(&cfg, k_trend_prior, x, t, scratch3n, n, x_is_mean, lo, hi, outer, min_disp, trigamma_c,
-                                         with_prior, reinterpret_cast<TrendOut*>(out16));
+    auto launch = [&](unsigned blocks) {
+        const unsigned per = trend_local_per(n, (size_t)blocks * threads, threads);
+        auto kernel = threads > 512 ? (per ? k_trend_prior<true, 1024> : k_trend_prior<false, 1024>)
+                                    : (per ? k_trend_prior<true, 512> : k_trend_prior<false, 512>);
+        const size_t smem = 2 * (size_t)per * threads * sizeof(double);
+        // both opt-ins on every launch, for the kernel on the current device (see allow_local)
+        if (const cudaError_t e = allow_local(kernel, smem)) return e;
+        if (blocks > 8)
+            if (const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1)) return e;
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(blocks, 1, 1);
+        cfg.blockDim = dim3(threads, 1, 1);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = c.stream;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = blocks;
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        return cudaLaunchKernelEx(&cfg, kernel, x, t, scratch3n, n, x_is_mean, lo, hi, outer,
+                                  min_disp, trigamma_c, with_prior, o16, fitted, per);
+    };
+    cudaError_t err = launch(nb);
     if (err != cudaSuccess && nb > 8) {  // a 16-block cluster could not be placed: fall back to the portable size
         cudaGetLastError();
-        max_cluster = 8;
-        attr[0].val.clusterDim.x = 8;
-        cfg.gridDim = dim3(8, 1, 1);
-        err = cudaLaunchKernelEx(&cfg, k_trend_prior, x, t, scratch3n, n, x_is_mean, lo, hi, outer, min_disp, trigamma_c, with_prior,
-                                 reinterpret_cast<TrendOut*>(out16));
+        err = launch(8);
     }
     if (err != cudaSuccess) return PDQ_ERR_CUDA;
-    if (int e = check_launch()) return e;
-    return 1;
-}
-
-int launch_trend_eval(const LaunchCfg& c, const double* means, size_t n, const double* out16, double* fitted) {
-    k_trend_eval<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(means, n, reinterpret_cast<const TrendOut*>(out16), fitted);
     if (int e = check_launch()) return e;
     return 1;
 }

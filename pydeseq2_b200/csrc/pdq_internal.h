@@ -100,9 +100,10 @@ int launch_mom_alpha(const LaunchCfg&, const DesignDev&, const int64_t* counts, 
                      int* status, double* hint_out);
 int launch_mu_from_lfc(const LaunchCfg&, const DesignDev&, const double* lfc, int G, double* mu, int64_t ld_out);
 
+// `fitted` (may be null, x_is_mean only): c0 + c1 / x[i] from the final coefficients, written by the same launch
 int launch_trend_fit(const LaunchCfg&, const double* x, const double* t, double* scratch3n, size_t n, int x_is_mean,
-                     double lo, double hi, int outer, double min_disp, double trigamma_c, int with_prior, double* out16);
-int launch_trend_eval(const LaunchCfg&, const double* means, size_t n, const double* out16, double* fitted);
+                     double lo, double hi, int outer, double min_disp, double trigamma_c, int with_prior, double* out16,
+                     double* fitted = nullptr);
 // `ws`: cooks_ws_bytes(d, G) bytes of device workspace, null when that is 0
 int launch_cooks(const LaunchCfg&, const DesignDev&, const int64_t* counts, int64_t ld, int G, const double* mu, const double* hat,
                  int64_t ld2, double cutoff, double* cooks, int64_t ld_out, double* disp, double* outlier, double* replaced, double* ws);

@@ -423,6 +423,9 @@ __global__ void __launch_bounds__(kBlock, PHASE ? PDQ_IRLS_MINB : PDQ_ALPHA_MINB
     bool valid;
     int ahead = draw_ticket(ticket);
     if (PHASE == 0) {
+        // a programmatic dependent of the trend kernel (launch_map_irls): everything above is independent of the trend; the
+        // fitted curve and the trend record are read only behind the trend grid's completion
+        asm volatile("griddepcontrol.wait;" ::: "memory");
         AlphaParams prm = a.al.prm;
         if (a.al.prior_var_dev) prm.prior_var = *a.al.prior_var_dev;
         const double sq_logres = a.trend->squared_logres;
@@ -996,8 +999,12 @@ int PDQ_TUFN(launch_map_irls)(const LaunchCfg& c, const DesignDev& d, const int6
         if (int e = prep(k_alpha_grid<P>, d.smem_bytes)) return e;
         if (int e = prep(k_irls_deferred<P>, smem_tail)) return e;
         if (int e = prep(k_irls_optimizer<P>, d.smem_bytes)) return e;
-        // the MAP kernel, then the LFC kernel as its programmatic dependent (see k_map_irls)
-        if (int e = launch_persistent(c, d, smem_tail, G, a, [](auto s) { return k_map_irls<P, decltype(s)::value, 0>; })) return e;
+        // the MAP kernel as a programmatic dependent of what precedes it in the stream (the trend kernel in the resident pass), then
+        // the LFC kernel as the MAP kernel's (see k_map_irls).  Invariant: what the MAP kernel reads before its griddepcontrol.wait --
+        // the pass word, its ticket, the design pack -- is written by no kernel that triggers its dependents early.  Today the only
+        // kernels that do are k_trend_prior / k_trend_prior_grid (which write none of these) and the MAP kernel itself (whose
+        // dependent is the LFC kernel); any other predecessor completes, writes included, before the MAP kernel starts
+        if (int e = launch_persistent(c, d, smem_tail, G, a, [](auto s) { return k_map_irls<P, decltype(s)::value, 0>; }, true)) return e;
         if (int e = launch_persistent(c, d, smem_tail, G, a, [](auto s) { return k_map_irls<P, decltype(s)::value, 1>; }, true)) return e;
         const int wave = fallback_grid(c.sm_count, G, c.lgT);
         k_alpha_grid<P><<<wave, kBlock, d.smem_bytes, c.stream>>>(a.al);

@@ -56,6 +56,17 @@ struct SerialReducer {
     }
 };
 
+// A per-gene vector as one thread of the fit sees it: a plain array indexed by gene (element i at v[i]), or the thread's own
+// elements in its block's shared memory (LocalVec: its k-th gene, i = tid + k nthreads, at p[k stride]).  Every pass of the fit and
+// of the prior visits the genes with the same map, so a thread only ever reads the elements it wrote itself.
+struct LocalVec {
+    double* p;
+    unsigned stride;
+};
+PDQ_HD double& at(double* v, size_t i, size_t) { return v[i]; }
+PDQ_HD double at(const double* v, size_t i, size_t) { return v[i]; }
+PDQ_HD double& at(const LocalVec& v, size_t, size_t k) { return v.p[k * v.stride]; }
+
 struct TrendSums {
     double L, g0, g1, h00, h01, h11, f00, f01, f11, n;
 };
@@ -63,13 +74,13 @@ struct TrendSums {
 // xs[i]: covariate; ts[i]: target, NaN when the gene is not (or no longer) part of the fit.  Both are prepared once per
 // launch by trend_prepare (clip, 1/mean, validity), so that a pass is: two loads, one reciprocal, one log, ten sums.
 // The sums g1, h01, h11, f01, f11 are taken over the covariate less `xc` (see trend_fit_once); xc = 0 gives the plain sums.
-template <class R>
-PDQ_HD TrendSums trend_sums(R& red, const double* xs, const double* ts, size_t n, double c0, double c1, double xc = 0.0) {
+template <class R, class VX, class VT>
+PDQ_HD TrendSums trend_sums(R& red, const VX& xs, const VT& ts, size_t n, double c0, double c1, double xc = 0.0) {
     double L = 0, g0 = 0, g1 = 0, h00 = 0, h01 = 0, h11 = 0, f00 = 0, f01 = 0, f11 = 0, cnt = 0;
-    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
-        const double tv = ts[i];
+    for (size_t i = red.tid(), k = 0; i < n; i += red.nthreads(), ++k) {
+        const double tv = at(ts, i, k);
         if (!(tv == tv)) continue;  // dropped gene / np.nanmean skips NaN targets
-        const double xv = xs[i];
+        const double xv = at(xs, i, k);
         const double m = fma(c1, xv, c0);
         const double im = fast_rcp(m);
         const double r = tv * im;
@@ -116,9 +127,8 @@ PDQ_HD TrendSums trend_sums(R& red, const double* xs, const double* ts, size_t n
 // pinned record, on the plain path.
 // A covariate that is exactly constant leaves only m = c0 + c1 x identified; the step then moves m to its optimum by the
 // shortest step in (c0, c1), which makes the fit the minimiser nearest its start.
-template <class R>
-PDQ_HD bool trend_fit_once(R& red, const double* xs, const double* ts, size_t n, double& c0, double& c1, double& loss,
-                           int& iters) {
+template <class R, class VX, class VT>
+PDQ_HD bool trend_fit_once(R& red, const VX& xs, const VT& ts, size_t n, double& c0, double& c1, double& loss, int& iters) {
     const double kLB = 1e-12;    // bounds=[(1e-12, inf)] (default_inference.py:224)
     const double kSing = 1e-5;   // relative Fisher determinant below which 1 and x count as nearly collinear (see above)
     bool centred = false;
@@ -130,8 +140,8 @@ PDQ_HD bool trend_fit_once(R& red, const double* xs, const double* ts, size_t n,
         if (!(s.L == s.L) || s.n < 2.0) return false;
         if (!centred && !(s.f00 * s.f11 - s.f01 * s.f01 > kSing * s.f00 * s.f11)) {
             double mx = -HUGE_VAL;
-            for (size_t i = red.tid(); i < n; i += red.nthreads())
-                if (ts[i] == ts[i]) mx = fmax(mx, -xs[i]);
+            for (size_t i = red.tid(), k = 0; i < n; i += red.nthreads(), ++k)
+                if (at(ts, i, k) == at(ts, i, k)) mx = fmax(mx, -at(xs, i, k));
             xc = -red.max_one(mx);
             centred = true;
             s = trend_sums(red, xs, ts, n, c0, c1, xc);
@@ -193,16 +203,16 @@ PDQ_HD bool trend_fit_once(R& red, const double* xs, const double* ts, size_t n,
 }
 
 // validity, clipping and the covariate are resolved once: xs / ts are n doubles of scratch each
-template <class R>
-PDQ_HD void trend_prepare(R& red, const double* x, const double* t, size_t n, bool x_is_mean, double lo, double hi,
-                          double* xs, double* ts) {
-    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
+template <class R, class V>
+PDQ_HD void trend_prepare(R& red, const double* x, const double* t, size_t n, bool x_is_mean, double lo, double hi, const V& xs,
+                          const V& ts) {
+    for (size_t i = red.tid(), k = 0; i < n; i += red.nthreads(), ++k) {
         const double xv = x_is_mean ? 1.0 / x[i] : x[i];
         double tv = t[i];
         tv = (tv < lo) ? lo : ((tv > hi) ? hi : tv);
         const bool ok = (xv == xv) && (fabs(xv) <= 1.7976931348623157e308);  // drop inf / NaN covariates (dds.py:1225-1232)
-        xs[i] = xv;
-        ts[i] = ok ? tv : (0.0 / 0.0);
+        at(xs, i, k) = xv;
+        at(ts, i, k) = ok ? tv : (0.0 / 0.0);
     }
     // no barrier: xs[i] / ts[i] are owned by the thread that writes them here -- every later pass of the fit (trend_sums, the
     // drop loop, the `used` count) visits i = tid, tid + nthreads, ... with the same map, so each thread reads only its own writes
@@ -210,8 +220,8 @@ PDQ_HD void trend_prepare(R& red, const double* x, const double* t, size_t n, bo
 
 // Full outer loop of dds.py:1199-1275 on the prepared vectors; ts[i] is set to NaN when gene i is dropped.  With
 // `reduce_used` false, n_used is this thread's share of the count: the caller packs it into its next reduction.
-template <class R>
-PDQ_HD TrendOut trend_fit_outer(R& red, const double* xs, double* ts, size_t n, bool outer, bool reduce_used = true) {
+template <class R, class VX, class VT>
+PDQ_HD TrendOut trend_fit_outer(R& red, const VX& xs, const VT& ts, size_t n, bool outer, bool reduce_used = true) {
     double o0 = 0.1, o1 = 0.1, c0 = 1.0, c1 = 1.0, loss = 0.0;
     int rounds = 0, iters = 0;
     bool failed = false, last_conv = false;
@@ -229,16 +239,16 @@ PDQ_HD TrendOut trend_fit_outer(R& red, const double* xs, double* ts, size_t n, 
         }
         if (!outer) break;
         // drop genes far from the curve before refitting (dds.py:1255-1265)
-        for (size_t i = red.tid(); i < n; i += red.nthreads()) {
-            const double tv = ts[i];
+        for (size_t i = red.tid(), k = 0; i < n; i += red.nthreads(), ++k) {
+            const double tv = at(ts, i, k);
             if (!(tv == tv)) continue;
-            const double ratio = tv / fma(c1, xs[i], c0);
-            if (ratio < 1e-4 || ratio >= 15.0) ts[i] = 0.0 / 0.0;
+            const double ratio = tv / fma(c1, at(xs, i, k), c0);
+            if (ratio < 1e-4 || ratio >= 15.0) at(ts, i, k) = 0.0 / 0.0;
         }
         // no barrier: ts[i] stays owned by its thread (see trend_prepare)
     }
     double used = 0.0;
-    for (size_t i = red.tid(); i < n; i += red.nthreads()) used += (ts[i] == ts[i]) ? 1.0 : 0.0;
+    for (size_t i = red.tid(), k = 0; i < n; i += red.nthreads(), ++k) used += (at(ts, i, k) == at(ts, i, k)) ? 1.0 : 0.0;
     if (reduce_used) red.sum_many(&used, 1);
     TrendOut o;  // identical in every thread (all decisions were taken on block/cluster-wide sums), n_used aside (see above)
     o.c0 = c0;
@@ -284,14 +294,14 @@ PDQ_HD double f64_from_key(uint64_t k) {
 // k-th smallest (0-based) of { |res[i] - center| or res[i] } over the non-NaN entries.  The blocks of the cluster
 // histogram disjoint slices of the vector and merge their 256-bin histograms (reducer hist_* hooks); `hist` holds
 // 256 local bins + 256 merged bins + 2 result slots.
-template <class R>
-PDQ_HD double select_kth(R& red, const double* res, size_t n, bool absdev, double center, unsigned* hist, size_t k) {
+template <class R, class V>
+PDQ_HD double select_kth(R& red, const V& res, size_t n, bool absdev, double center, unsigned* hist, size_t k) {
     uint64_t prefix = 0, mask = 0;
     for (int shift = 56; shift >= 0; shift -= 8) {
         for (int b = red.local_tid(); b < 512; b += red.local_nthreads()) hist[b] = 0;
         red.hist_begin();
-        for (size_t i = red.tid(); i < n; i += red.nthreads()) {
-            const double r = res[i];
+        for (size_t i = red.tid(), j = 0; i < n; i += red.nthreads(), ++j) {
+            const double r = at(res, i, j);
             if (!(r == r)) continue;
             const uint64_t key = f64_key(absdev ? fabs(r - center) : r);
             if ((key & mask) == prefix) {
@@ -314,8 +324,8 @@ PDQ_HD double select_kth(R& red, const double* res, size_t n, bool absdev, doubl
     return f64_from_key(prefix);
 }
 
-template <class R>
-PDQ_HD double median_of(R& red, const double* res, size_t n, size_t cnt, bool absdev, double center, unsigned* hist) {
+template <class R, class V>
+PDQ_HD double median_of(R& red, const V& res, size_t n, size_t cnt, bool absdev, double center, unsigned* hist) {
     if (cnt == 0) return 0.0 / 0.0;  // np.median([]) = nan
     const size_t k = cnt / 2;
     const double hi = select_kth(red, res, n, absdev, center, hist, k);  // upper median
@@ -324,8 +334,8 @@ PDQ_HD double median_of(R& red, const double* res, size_t n, size_t cnt, bool ab
     // maximum starts at -inf, not at the lowest finite double: held-out size factors take medians of log ratios that hold -inf
     // (a zero count in a gene of the fit), and a lower median of -inf must stay -inf, as in np.median
     double less = 0.0, mx = -HUGE_VAL;
-    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
-        const double r = res[i];
+    for (size_t i = red.tid(), j = 0; i < n; i += red.nthreads(), ++j) {
+        const double r = at(res, i, j);
         if (!(r == r)) continue;
         const double v = absdev ? fabs(r - center) : r;
         if (v < hi) {
@@ -464,8 +474,8 @@ __device__ inline void find_vbin(SelShared& sh, size_t k) {
 // k-th smallest of { |res[i] - center| or res[i] } (0-based) over the non-NaN entries; when `lower`, also rank k - 1.  Returns
 // the exact values, as median_of.  [vlo, vhi] bounds the values.  `cand`: kCandCap keys of global scratch no thread reads
 // or writes meanwhile.  `slot` (0, 1) picks the reducer's merge buffers: the two medians of one launch use different slots.
-template <class R>
-__device__ double median_bins(R& red, const double* res, size_t n, size_t cnt, bool absdev, double center, double vlo,
+template <class R, class V>
+__device__ double median_bins(R& red, const V& res, size_t n, size_t cnt, bool absdev, double center, double vlo,
                               double vhi, int slot, unsigned long long* cand, SelShared& sh, unsigned* hist514) {
     if (cnt == 0) return 0.0 / 0.0;  // np.median([]) = nan
     const double width = vhi - vlo, scale = (double)kVBins / width;
@@ -475,8 +485,8 @@ __device__ double median_bins(R& red, const double* res, size_t n, size_t cnt, b
     const bool even = !(cnt & 1);
     for (int b = threadIdx.x; b < kVBins; b += blockDim.x) sh.hist[b] = 0;
     __syncthreads();
-    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
-        const double r = res[i];
+    for (size_t i = red.tid(), j = 0; i < n; i += red.nthreads(), ++j) {
+        const double r = at(res, i, j);
         if (!(r == r)) continue;
         atomicAdd(&sh.hist[vbin(absdev ? fabs(r - center) : r, vlo, scale)], 1u);
     }
@@ -488,8 +498,8 @@ __device__ double median_bins(R& red, const double* res, size_t n, size_t cnt, b
     const unsigned r_hi = (unsigned)k - before;
     const bool below = even && r_hi == 0;  // rank k - 1 is the largest value of the bins below b
     unsigned long long mx = 0ull;          // below every key of a non-NaN double
-    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
-        const double r = res[i];
+    for (size_t i = red.tid(), j = 0; i < n; i += red.nthreads(), ++j) {
+        const double r = at(res, i, j);
         if (!(r == r)) continue;
         const double v = absdev ? fabs(r - center) : r;
         const int bi = vbin(v, vlo, scale);
@@ -527,15 +537,15 @@ __device__ double median_bins(R& red, const double* res, size_t n, size_t cnt, b
 
 // trend_prior on the device: the count of prior genes, the fit's `used` count (this thread's share in out.n_used, see
 // trend_fit_outer) and the residuals' range share one reduction; the two medians run through median_bins.
-template <class R>
+template <class R, class V>
 __device__ void trend_prior_dev(R& red, const double* means, const double* t, size_t n, double lo, double hi, double min_disp,
-                                double trigamma_c, double* res, unsigned long long* cand, SelShared& sh, unsigned* hist514,
+                                double trigamma_c, const V& res, unsigned long long* cand, SelShared& sh, unsigned* hist514,
                                 TrendOut& out) {
     const double c0 = out.c0, c1 = out.c1;
     double v[4] = {0.0, out.n_used, -HUGE_VAL, -HUGE_VAL};  // count, used, max, -min
-    for (size_t i = red.tid(); i < n; i += red.nthreads()) {
+    for (size_t i = red.tid(), k = 0; i < n; i += red.nthreads(), ++k) {
         const double r = prior_residual(means, t, i, c0, c1, lo, hi, min_disp);
-        res[i] = r;  // each thread later reads only its own stride of res: no barrier needed
+        at(res, i, k) = r;  // each thread later reads only its own stride of res: no barrier needed
         if (!(r == r)) continue;
         v[0] += 1.0;
         v[2] = fmax(v[2], r);
